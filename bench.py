@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — CPR head img/s @1333x800 (BASELINE.json metric) on N B200s + HBM roofline of the neighbor gather.
+"""bench.py — CPR head img/s @1333x800 (BASELINE.json metric) on N H100s + HBM roofline of the neighbor gather.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Step = one pass of the CPR head over one batch of synthetic FPN tensors: CPRHead.simple_test == forward (4x conv3x3+GN+
-ReLU towers + class-logit map: hand-written tcgen05 implicit GEMM, fp32-accurate two-term fp16 split) + get_bboxes (fused bag
+ReLU towers + class-logit map: hand-written wgmma implicit GEMM, fp32-accurate two-term fp16 split) + get_bboxes (fused bag
 sampling / arg-max / nearest+classify filters / merge).
 Workload = BASELINE.json configs[1]: CPR R50-FPN 1333x800 (pad 800x1344 -> 100x168x256 map at stride 8), 500 points per
 image, 80 classes, radius 8 (K=289), batch 8 per GPU, fp32 (the reference runs fp32; no AMP in its CPR configs).
@@ -13,13 +13,13 @@ Image-parallel, weak scaling: every rank owns its own 8 images; no data-path col
 
   value   img/s with inputs resident in HBM, timed with CUDA events over exactly K steps, max over ranks
   e2e     same call with HOST (pinned) inputs: H2D of the FPN tensor + GT boxes and D2H of the detections inside the region
-  roofline        dominant kernel of the step = the tcgen05 conv3x3 (tensor bound): algorithmic FLOPs / CUDA-event time vs the
+  roofline        dominant kernel of the step = the wgmma conv3x3 (tensor bound): algorithmic FLOPs / CUDA-event time vs the
                   measured bf16 GEMM peak (MEASURED_PEAKS.json)
   roofline_gather neighbor-gather kernel (ptb_cpr_bag_gather, C=256 — the kernel BASELINE.json's target names), timed alone with
                   CUDA events in this process; algorithmic bytes per SURVEY.md §8d (166.5 MB/img); peak = MEASURED_PEAKS.json hbm_gbs
   cpu_baseline  the oracle port of the reference head (torch CPU ops, all host threads) on a bounded sample
 --impl reference: the reference's own CPU implementation of the same step (oracle port: the reference is pure Python
-and /root/reference does not exist on the GPU box) on all host cores: floor(cores/16) processes x 16 threads, one image each per step.
+and is not shipped with this project) on all host cores: floor(cores/16) processes x 16 threads, one image each per step.
 """
 import argparse
 import json
@@ -118,7 +118,7 @@ def synth_dense_anchors(seed, n_anchor=81840, n_gt=300, n_ign=5, size=(512, 640)
 
 # --------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock / throttle (clocks-event) reasons sampled DURING the timed region (B200_PROFILING.md recipe).  NVML is polled from
+    """SM clock / throttle (clocks-event) reasons sampled DURING the timed region.  NVML is polled from
     a thread of this process every 5 ms (the timed region of the default run lasts ~100 ms, shorter than nvidia-smi's start-up);
     when pynvml is missing the same fields are read from an `nvidia-smi -lms` child process instead."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
@@ -226,7 +226,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs, burst copy)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s HBM3)'
 
 
 def measured_tensor_peak():
@@ -234,7 +234,7 @@ def measured_tensor_peak():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['bf16_tflops']), 'measured (MEASURED_PEAKS.json bf16_tflops, burst cuBLAS bf16 GEMM)'
-    return 1590.0, 'fallback (B200_PROFILING.md 1.59 PFLOP/s bf16)'
+    return 989.0, 'fallback (H100 SXM data sheet, 989 TFLOP/s dense bf16 at 700 W)'
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -260,10 +260,10 @@ def bench_config(world):
     """the `config` object of the JSON line — IDENTICAL for both arms (the driver's same_config check); what differs per arm (how a
     step samples the workload) is stated in cpu_baseline.sample / extra."""
     return dict(workload=WORKLOAD, global_batch=CFG['B'] * world, parallelism=f'image-parallel x{world}, no data-path collective',
-                l2='two rotating input sets, each 137.6 MB > 126 MB L2 (inputs larger than L2)',
+                l2='two rotating input sets, each 137.6 MB > 50 MB L2 of an H100 (inputs larger than L2)',
                 fpn_layout='channels_last (NHWC storage, as an FPN run with memory_format=torch.channels_last emits it); an NCHW-contiguous '
                            'FPN output costs one extra transpose per step, reported as extra.nchw_to_nhwc_ms',
-                towers='tcgen05 implicit-GEMM conv3x3 (fp16 two-term split = fp32-level accuracy) + GN + ReLU (libptb_b200.so); point '
+                towers='wgmma implicit-GEMM conv3x3 (fp16 two-term split = fp32-level accuracy) + GN + ReLU (libptb_b200.so); point '
                        'path = libptb_b200.so; no cuDNN/cuBLAS in the step')
 
 
@@ -336,6 +336,18 @@ class _SkipP2PTrain(Exception):      # control flow only: a side measurement tha
     pass
 
 
+def dump_outputs(out_dir, res):
+    """CPRHead.simple_test's return value (one tuple of tensors per image) as out_dir/img<i>_<j>.npy, float32 (a few hundred KB)."""
+    if not isinstance(res, (list, tuple)) or not res:
+        raise SystemExit(f'--dump-outputs: the timed step returned {type(res).__name__}, not a list of per-image results')
+    os.makedirs(out_dir, exist_ok=True)
+    for i, per_img in enumerate(res):
+        for j, t in enumerate(per_img if isinstance(per_img, (list, tuple)) else [per_img]):
+            if not torch.is_tensor(t):
+                raise SystemExit(f'--dump-outputs: output {j} of image {i} is a {type(t).__name__}, not a tensor')
+            np.save(os.path.join(out_dir, f'img{i}_{j}.npy'), t.detach().float().cpu().numpy())
+
+
 def main():
     global T_MAIN
     T_MAIN = time.perf_counter()
@@ -348,8 +360,12 @@ def main():
     ap.add_argument('--no-extra', action='store_true')
     ap.add_argument('--p2p-train', action='store_true', help='also time a P2PHead training step (its two narrow output convs run on cuDNN under '
                     'autograd: the first cuDNN use pages the library in, minutes on a cold box)')
-    ap.add_argument('--profile', action='store_true', help='for runs under ncu: no load-holding steps, no e2e, no extras')
+    ap.add_argument('--profile', action='store_true', help='for runs under a profiler: no load-holding steps, no e2e, no extras')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step returned (per image: detections, float32) as DIR/<name>.npy')
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != 'ours' or args.steps < 1):
+        ap.error('--dump-outputs needs --impl ours and --steps >= 1 (it writes what the last timed step computed)')
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     rank = int(os.environ.get('RANK', 0))
     world = int(os.environ.get('WORLD_SIZE', 1))
@@ -376,7 +392,7 @@ def main():
     head.load_state_dict(sd)
 
     B = CFG['B']
-    # two rotating input sets (2 x 137.6 MB > 126 MB L2) so no step finds its input in L2
+    # two rotating input sets (each 137.6 MB, larger than the 50 MB L2) so no step finds its input in L2
     host = []
     for i in range(2):
         x, gtb, gtl, aid, metas = synth_batch(B, 1234 + rank * 10 + i)
@@ -445,14 +461,18 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
+    last_out = []
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         l0 = ops.launch_count()
         e0.record()
+        out = None
         for i in range(steps):
-            fn(i)
+            out = fn(i)
         e1.record()
+        last_out[:] = [out]
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1)
         launches = ops.launch_count() - l0
@@ -476,6 +496,8 @@ def main():
     t_end = time.perf_counter()
     clocks = sampler.stop(t_begin, t_end) if rank == 0 else None
     value = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out[0])
 
     if args.profile:
         if rank == 0:
@@ -528,33 +550,27 @@ def main():
         alg = Bq * H * W * C * 4 + G * K * 8 + G * K * C * 4 + G * K       # SURVEY.md §8d: 166.5 MB/img x 8
         t_g = ktime(lambda: ops.bag_gather(fmap, gt.centers, gt.bag_img, off, CFG['stride'], gt.pad_hw))
         ach = alg / (t_g * 1e-3) / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, 'profiles', 'r01_gather_traffic.json')
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get('dram_bytes_per_launch')
+        traffic = None                    # DRAM bytes per launch are not measured here (no hardware-counter profiler in the run)
         roofline_gather = dict(kernel='ptb_cpr_bag_gather<C=256> (neighbor gather, reference data flow)', bound='hbm', achieved=ach,
                         peak=peak, unit='GB/s', frac=ach / peak, traffic=traffic, peak_source=peak_src,
                         algorithmic_bytes_per_launch=alg, ms_per_launch=t_g, units_per_launch=f'{Bq} images x {CFG["n"]} bags x {K} samples',
                         timing='CUDA events on the launching stream, kernel alone, L2 flushed between launches')
-        # dominant kernel of the step (~70 % of the device time, profiles/r01_step_launches_v*.json): the tcgen05 conv
+        # dominant kernel of the step (the four tower launches: extra.share_of_step.towers_wgmma): the wgmma conv
         conv_traffic = None
-        ctp = os.path.join(ROOT, 'profiles', 'r01_conv_traffic.json')
-        if os.path.exists(ctp):
-            conv_traffic = json.load(open(ctp)).get('dram_bytes_per_launch')       # DRAM bytes per launch from the ncu --set full capture
         from pointtinybenchmark_b200.layers import _packed_weight, _packed_weight_f16
         flops = 2.0 * 9 * C * 256 * Bq * H * W                                   # algorithmic (fp32 semantics), 158.5 GFLOP
         tpeak, tsrc = measured_tensor_peak()
         xin = ops.to_nhwc(x).contiguous()
-        if head.last_tower_backend == 'tcgen05-f16x2':
+        if head.last_tower_backend == 'wgmma-f16x2':
             h16, l16, dinv = ops.split_f16(xin, auto_scale=True)
             wh, wl, invw = _packed_weight_f16(head.cls_convs[0])
             t_c = ktime(lambda: ops.conv3x3_c256_f16(h16, l16, wh, wl, invw, dinv))
-            kname, mma_peak, mma_kind = 'ptb::conv_tc_kernel<3,true> (CTA-pair tcgen05.mma.cta_group::2, fp16 two-term split, kind::f16)', tpeak, 'fp16'
+            kname, mma_peak, mma_kind = 'ptb::conv_tc_kernel<true,128> (wgmma m64n128k16, fp16 two-term split)', tpeak, 'fp16'
         else:
             xh, xl = ops.split_tf32(xin)
             wh, wl = _packed_weight(head.cls_convs[0])
             t_c = ktime(lambda: ops.conv3x3_c256(xh, xl, wh, wl))
-            kname, mma_peak, mma_kind = 'ptb::conv_tc_kernel<1,false> (3xTF32, kind::tf32)', tpeak / 2, 'tf32'
+            kname, mma_peak, mma_kind = 'ptb::conv_tc_kernel<false,128> (3xTF32, wgmma m64n128k8 tf32)', tpeak / 2, 'tf32'
         ach_t = flops / (t_c * 1e-3) / 1e12
         roofline = dict(kernel=kname + ': conv3x3 256->256 of the head towers, 4 launches per step', bound='tensor',
                         achieved=ach_t, peak=tpeak, unit='TFLOP/s', frac=ach_t / tpeak, traffic=conv_traffic, peak_source=tsrc,
@@ -583,9 +599,9 @@ def main():
             extra['nchw_to_nhwc_ms'] = t_tr       # NOT inside the timed step: the step takes the FPN tensor channels_last (config.fpn_layout)
             step_ms = ms / args.steps
             extra['kernels_ms_per_batch'] = dict(
-                towers_tcgen05=t_tow, linear_rows_256x80=t_lin, refine_fused=t_ref, bag_gather_c256=t_g, bag_gather_c80=t_g80,
+                towers_wgmma=t_tow, linear_rows_256x80=t_lin, refine_fused=t_ref, bag_gather_c256=t_g, bag_gather_c80=t_g80,
                 neg_mask=t_neg)
-            extra['share_of_step'] = dict(towers_tcgen05=t_tow / step_ms, linear_rows=t_lin / step_ms, refine_fused=t_ref / step_ms)
+            extra['share_of_step'] = dict(towers_wgmma=t_tow / step_ms, linear_rows=t_lin / step_ms, refine_fused=t_ref / step_ms)
             extra['tower_backend'] = head.last_tower_backend
             extra['towers_effective_fp32_tflops'] = 4 * 2 * 9 * C * C * Bq * H * W / (t_tow * 1e-3) / 1e12
             extra['linear_rows_tflops'] = 2 * Bq * H * W * C * N / (t_lin * 1e-3) / 1e12
@@ -699,7 +715,7 @@ def main():
                 pass
             except Exception as ex:  # pragma: no cover
                 extra['config4_dense_anchor_error'] = repr(ex)[:300]
-            # P2PHead inference at BASELINE.json configs[2] shape (bs 16): two tcgen05 towers + output convs + decode/top-k/NMS
+            # P2PHead inference at BASELINE.json configs[2] shape (bs 16): two wgmma towers + output convs + decode/top-k/NMS
             try:
                 if world > 1:                 # side measurements are reported by the 1-GPU run only
                     raise _SkipP2PTrain()
@@ -806,8 +822,7 @@ def main():
                                                  what='gradients are views of one persistent flat fp32 buffer (no copy-in / copy-out, mean = NCCL AVG): '
                                                       'ONE all-reduce of the 9.6 MB after backward (allreduce_alone_ms, timed on its own). '
                                                       'PTB_GRAD_OVERLAP=1 selects per-bucket all-reduces from post-accumulate hooks on a side stream; '
-                                                      'measured on 2 x B200 it is slower (9.30 vs ~8.7 ms per step): the exchange takes 0.05 ms, the '
-                                                      'hooks cost more host time than that in a backward pass that is partly launch-bound')
+                                                      'the hooks cost host time in a backward pass that is partly launch-bound (not measured on H100)')
         bucket.close()
         del opt
         head.zero_grad(set_to_none=True)

@@ -1,4 +1,4 @@
-/* ptb_b200.h — C ABI of libptb_b200.so: the B200 (sm_100a) CPR / P2P point-localization hot path.
+/* ptb_b200.h — C ABI of libptb_b200.so: the H100 (sm_90a) CPR / P2P point-localization hot path.
  *
  * The reference (ucas-vg/PointTinyBenchmark, TOV_mmdetection) is pure Python: it has NO FFI for this path.  Its
  * "plugin boundary" is the mmdet dense-head protocol (HEADS registry).  This header is the C ABI that sits directly
@@ -356,7 +356,7 @@ int ptb_smooth_l1_fwd_bwd(const float* pred /*[M][2]*/, const float* target, con
 /* ------------------------------------------------------------------------------------------------------------------
  * Conv towers on the tensor cores — replace the cuDNN calls behind CPRHead.forward_single / P2PHead.forward_single
  * (cpr_head.py:983-995,1033-1043; p2p_head.py:82-97,113-123): ConvModule = conv3x3(256 out, no bias) + GroupNorm + ReLU.
- * fp32-accurate 3xTF32 implicit GEMM (tcgen05.mma kind::tf32, TMA-staged operands, TMEM accumulators).
+ * fp32-accurate 3xTF32 implicit GEMM (wgmma.mma_async tf32, TMA-staged operands, fp32 accumulators in registers).
  *   ptb_split_tf32           x -> hi (13 low mantissa bits cleared) + lo (= x - hi, exact)
  *   ptb_conv3x3_pack_weight  nn.Conv2d weight [Cout][Cin][3][3] -> [Cout][tap][Cin] as hi / lo
  *   ptb_conv3x3_c256_tf32x3  y[b][h][w][0..256) = sum_{tap,ci} x[b][h+kh-1][w+kw-1][ci] * w[co][tap][ci]  (zero padding);
@@ -372,7 +372,7 @@ int ptb_conv3x3_c256_tf32x3(const float* x_hi, const float* x_lo /*[B][H][W][Cin
 int ptb_gn_relu_apply(const float* y, const double* gn_stats, const float* gamma, const float* beta, int B, int HW, int C,
                       int groups, float eps, int relu, float* out_hi, float* out_lo, void* stream);
 /* Same tower at HALF the tensor-pipe time: two-term fp16 split  x*scale = h + l  (22 significant bits), three
- * tcgen05.mma.kind::f16 per k-step (h*h + l*h + h*l), fp32 accumulate.  Operands are IEEE fp16 arrays (void* = __half*).
+ * wgmma.mma_async f16 products per k-step (h*h + l*h + h*l), fp32 accumulate.  Operands are IEEE fp16 arrays (void* = __half*).
  *   ptb_split_f16: auto_scale != 0 picks a power-of-two scale from max|x| ON THE DEVICE (workspace: 4 bytes) and writes
  *                  its inverse to dev_inv_scale (a device float), else scale = 1.
  *   ptb_conv3x3_pack_weight_f16: weights * scale (a power of two chosen by the caller) as h / l.
@@ -421,7 +421,7 @@ int ptb_bbox_overlaps(const float* boxes1, int m, const float* boxes2, int n, in
  *                            max|dy| as float bits (device) for the operand scale.  Deterministic (no fp atomics).
  *   ptb_split_f16_amax       dy -> fp16 (h, l) pair with the power-of-two scale derived from that device max; 1/scale -> dev_inv_scale
  *   ptb_conv_tc_f16x2        dgrad: the forward kernel on (dy pair, weights transposed + flipped and packed by the host layer)
- *   ptb_conv3x3_wgrad_f16x2  dW[co][ci][3][3] (+)= scale * s_dy * s_x * sum_pixels dy (x) x_shifted  on tcgen05 with MN-major operands
+ *   ptb_conv3x3_wgrad_f16x2  dW[co][ci][3][3] (+)= scale * s_dy * s_x * sum_pixels dy (x) x_shifted  on wgmma with MN-major operands
  * All tensors channels-last; C = 256 for the tensor-core kernels.
  */
 uint64_t ptb_gn_relu_bwd_workspace(int B, int HW, int C, int groups);

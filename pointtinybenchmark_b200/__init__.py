@@ -1,4 +1,4 @@
-"""pointtinybenchmark_b200 — B200 (sm_100a) native CPR / P2P point-localization head path.
+"""pointtinybenchmark_b200 — H100 (sm_90a) native CPR / P2P point-localization head path.
 
 Python host layer that mirrors the reference's mmdet dense-head interface (CPRHead / P2PHead, HEADS registry,
 same ctor kwargs and state_dict keys) over the C-ABI CUDA library libptb_b200.so (include/ptb_b200.h).

@@ -102,7 +102,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f'{LIB_PATH} is missing: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            '(nvcc, sm_100a). pointtinybenchmark_b200 has no CPU or PyTorch fallback.')
+            '(nvcc, sm_90a). pointtinybenchmark_b200 has no CPU or PyTorch fallback.')
     lib = ctypes.CDLL(LIB_PATH)
     missing = []
     for name, (res, args) in SIGNATURES.items():

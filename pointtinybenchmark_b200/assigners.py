@@ -32,7 +32,7 @@ class MaxIoUAssigner:
 
     def assign(self, bboxes, gt_bboxes, gt_bboxes_ignore=None, gt_labels=None):
         if not bboxes.is_cuda:
-            raise RuntimeError('MaxIoUAssigner (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('MaxIoUAssigner runs on CUDA tensors only; there is no CPU fallback')
         b = bboxes[:, :4].float().contiguous()
         g = gt_bboxes[:, :4].float().contiguous()
         ign = gt_bboxes_ignore[:, :4].float().contiguous() if gt_bboxes_ignore is not None else None
@@ -53,7 +53,7 @@ class PointAssigner:
 
     def assign(self, points, gt_bboxes, gt_bboxes_ignore=None, gt_labels=None):
         if not points.is_cuda:
-            raise RuntimeError('PointAssigner (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('PointAssigner runs on CUDA tensors only; there is no CPU fallback')
         p = (points.reshape(-1, 3) if points.numel() == 0 else points[:, :3]).float().contiguous()      # the reference's tests pass 1-D empties
         g = (gt_bboxes.reshape(-1, 4) if gt_bboxes.numel() == 0 else gt_bboxes[:, :4]).float().contiguous()
         gt_inds = ops.point_assigner(p, g, self.scale, self.pos_num)
@@ -80,7 +80,7 @@ class HungarianAssignerV2:
         cc = cc[0] if isinstance(cc, (list, tuple)) and len(cc) == 1 else cc
         rc = rc[0] if isinstance(rc, (list, tuple)) and len(rc) == 1 else rc
         if not isinstance(cc, dict) or not isinstance(rc, dict) or cc.get('type') != 'FocalLossCost' or rc.get('type') != 'DisCostV2':
-            raise NotImplementedError('HungarianAssignerV2 (B200): one FocalLossCost + one DisCostV2 (the P2P configs) are implemented')
+            raise NotImplementedError('HungarianAssignerV2: one FocalLossCost + one DisCostV2 (the P2P configs) are implemented')
         if rc.get('p', 1) != 1:
             raise NotImplementedError('DisCostV2 p != 1')
         self.w_cls, self.alpha, self.gamma, self.eps = cc.get('weight', 1.0), cc.get('alpha', 0.25), cc.get('gamma', 2), cc.get('eps', 1e-12)
@@ -90,9 +90,9 @@ class HungarianAssignerV2:
     def assign(self, bbox_pred, cls_pred, gt_bboxes, gt_labels, img_meta, gt_bboxes_ignore=None, eps=1e-7):
         assert gt_bboxes_ignore is None, 'Only case when gt_bboxes_ignore is None is supported.'
         if not bbox_pred.is_cuda:
-            raise RuntimeError('HungarianAssignerV2 (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('HungarianAssignerV2 runs on CUDA tensors only; there is no CPU fallback')
         if bbox_pred.shape[-1] != 2 or (gt_bboxes.numel() > 0 and gt_bboxes.shape[-1] != 2):
-            raise NotImplementedError('HungarianAssignerV2 (B200): (x, y) points only (DisCostV2 with k*2 = 2 coordinates, as P2PHead uses it)')
+            raise NotImplementedError('HungarianAssignerV2: (x, y) points only (DisCostV2 with k*2 = 2 coordinates, as P2PHead uses it)')
         N, n = bbox_pred.shape[0], gt_bboxes.shape[0]
         dev = bbox_pred.device
         gt_inds = torch.zeros((N,), dtype=torch.long, device=dev)

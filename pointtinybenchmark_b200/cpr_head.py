@@ -1,4 +1,4 @@
-"""CPRHead — host-side mirror of the reference's Coarse-Point-Refine head over the sm_100a kernels.
+"""CPRHead — host-side mirror of the reference's Coarse-Point-Refine head over the sm_90a kernels.
 
 Interface (same names / argument meaning / output structure as the reference, SURVEY.md §8b):
   reference: TOV_mmdetection/mmdet/models/point/dense_heads/cpr_head.py:898-1309 (CPRHead), registered in HEADS.
@@ -6,8 +6,8 @@ Interface (same names / argument meaning / output structure as the reference, SU
   get_bboxes(...) -> [(det (n,6) [x1,y1,x2,y2,score,ann_id], labels (n,))];  forward_train / simple_test as mmdet.
   state_dict keys: cls_convs.{i}.conv.weight, cls_convs.{i}.gn.{weight,bias}, cls_out.*, ins_out.*.
 
-Data flow (B200-first, see DESIGN.md): the per-point Linear(256->C) of the reference commutes with bilinear sampling,
-so the head computes ONE class/instance logit map (a 1-tap tcgen05 convolution, `ptb_conv_tc_f16x2`; `ptb_linear_rows` is the
+Data flow (GPU-first, see DESIGN.md): the per-point Linear(256->C) of the reference commutes with bilinear sampling,
+so the head computes ONE class/instance logit map (a 1-tap wgmma convolution, `ptb_conv_tc_f16x2`; `ptb_linear_rows` is the
 fp32 FFMA alternative) and samples that (C channels instead of 256); the (G,K,256) gathered-feature tensor of the reference is
 never built, and at inference not even the (G,K,C) probability tensor is (ptb_cpr_refine_fused).  All images of the batch go
 through each kernel in one launch.  Positive bags: ring bags (CirclePtFeatGenerator) or grid-cell bags (GridCirclesPtFeatGenerator);
@@ -100,7 +100,7 @@ class _GridCircleBags:
 
 
 def _loss_gemm_on_tc(C, LD):
-    """the two GEMMs of the loss that are plain 1x1 convolutions (logit map forward, its input gradient) run on the tcgen05 kernel
+    """the two GEMMs of the loss that are plain 1x1 convolutions (logit map forward, its input gradient) run on the wgmma kernel
     when the channel counts fit it (Cin % 32 == 0, N <= 256); PTB_LOSS_GEMM=ffma keeps the fp32 FFMA kernels."""
     import os
     return os.environ.get('PTB_LOSS_GEMM', 'tc') == 'tc' and C % 32 == 0 and LD % 32 == 0 and C <= 256 and LD <= 256
@@ -338,7 +338,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
     def _check_supported(self):
         def need(cond, what):
             if not cond:
-                raise NotImplementedError(f'CPRHead (B200): {what} is not supported by the CUDA path')
+                raise NotImplementedError(f'CPRHead: {what} is not supported by the CUDA path')
         need(len(self.strides) == 1, 'more than one FPN level (the reference asserts a single level too, cpr_head.py:799,1152)')
         need(self.ins_share_head_feat, 'ins_share_head_feat=False')
         need(self.loss_mil_cfg.get('type', 'MILLoss') == 'MILLoss', 'loss_mil.type != MILLoss')
@@ -495,7 +495,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
 
     def simple_test(self, feats, img_metas, rescale=False, **kwargs):
         """dense_test_mixins.py:15-36 (forward -> get_bboxes).  Inference fast path: the towers hand their output over
-        as the fp16 operand pair and the class-logit map comes from the same tcgen05 kernel (1 tap, N = num_classes),
+        as the fp16 operand pair and the class-logit map comes from the same wgmma kernel (1 tap, N = num_classes),
         so neither the fp32 feature map nor an FFMA GEMM appears in the step; results are identical within 1e-4."""
         x = feats[0]
         if len(feats) == 1 and self._default_variant() and tc_enabled(x, self.cls_convs, self.cls_out) and not torch.is_grad_enabled() \
@@ -519,7 +519,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         assert len(gt_labels) > 0
         feat = cls_feat[0]
         if not feat.is_cuda:
-            raise RuntimeError('CPRHead (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('CPRHead runs on CUDA tensors only; there is no CPU fallback')
         gt = _BatchGT(gt_bboxes, gt_labels, img_metas, feat.device)
         pos, neg = self.train_pts_extractor['pos_generator'], self.train_pts_extractor['neg_generator']
         hp = dict(num_classes=self.num_classes, stride=float(self.strides[0]), eps=float(self.loss_mil_cfg.get('eps', 1e-6)),
@@ -600,7 +600,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         assert gt_labels is not None and len(gt_labels) > 0
         feat = cls_feat[0]
         if not feat.is_cuda:
-            raise RuntimeError('CPRHead (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('CPRHead runs on CUDA tensors only; there is no CPU fallback')
         gt = _BatchGT(gt_bboxes, gt_labels, img_metas, feat.device)
         nr_in = torch.cat(list(not_refine)).to(feat.device) if not_refine is not None else None
         geo = bool(self.other_info.get('out_geo', False))

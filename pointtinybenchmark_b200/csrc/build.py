@@ -1,4 +1,4 @@
-"""Builds libptb_b200.so (sm_100a only) in-tree with nvcc.  Used by __graft_entry__.build() and by hand:
+"""Builds libptb_b200.so (sm_90a only) in-tree with nvcc.  Used by __graft_entry__.build() and by hand:
     python pointtinybenchmark_b200/csrc/build.py [--force] [--verbose]
 """
 import os
@@ -9,7 +9,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(os.path.dirname(HERE), 'libptb_b200.so')
 SOURCES = ['capi.cu', 'gather.cu', 'linear.cu', 'negmask.cu', 'refine.cu', 'gridbag.cu', 'mil.cu', 'p2p.cu', 'nms.cu', 'conv_tc.cu', 'tower_bwd.cu', 'wgrad_tc.cu', 'assign.cu', 'lsap.cu', 'rpn.cu', 'loss_bwd.cu']
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-Xptxas', '-v']
 
 

@@ -1,4 +1,4 @@
-// Dense convolutions of the head on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), fp32-accurate by operand splitting:
+// Dense convolutions of the head on the Hopper tensor cores (wgmma + TMA + mbarrier), fp32-accurate by operand splitting:
 // conv3x3 (stride 1, pad 1) and conv1x1 / per-cell Linear, Cin % 32 == 0 (fp16 mode) or Cin % 16 == 0 (TF32 mode), up to 256
 // output channels, optional bias, optional GroupNorm statistics in the epilogue; GroupNorm-apply + ReLU + operand split is a
 // second, HBM-bound kernel.  Replaces the cuDNN / cuBLAS calls behind CPRHead.forward_single / P2PHead.forward_single
@@ -6,78 +6,49 @@
 // per-sample cls_out / ins_out Linear of CPRHead.get_pts_outs (cpr_head.py:1045-1078, applied once per map cell here) and
 // P2PHead's cls_out / reg_out conv3x3.
 //
-// Implicit GEMM:  M = output pixels (tile = 8 rows x 16 cols = 128 pixels of one image), N = n_mma <= 256 output channels,
+// Implicit GEMM:  M = output pixels (tile = 128 pixels of one image), N = output channels in slices of NT <= 128,
 //                 K = taps x Cin.  One K-block = (tap, 64 B of input channels) = one SWIZZLE_64B row.
-//   * A operand: 4-D TMA box {64 B ch, 16 w, 8 h, 1 img} of the channels-last activation at the tap-shifted origin;
+//   * A operand: 4-D TMA box {64 B ch, tile w, tile h, 1 img} of the channels-last activation at the tap-shifted origin;
 //     out-of-bounds (the zero padding of the conv and partial edge tiles) is zero-filled by the TMA unit.
-//   * B operand: 2-D TMA box {64 B k, n_mma co} of the packed weights W2[co][tap*Cin + ci].
+//   * B operand: 2-D TMA box {64 B k, NT co} of the packed weights W2[co][tap*Cin + ci]; rows beyond n_mma are zero-filled.
 //   * fp32 accuracy (the head's logits must match the fp32 reference to 1e-4).  Every operand is split x = hi + lo and three
 //     MMAs per k-step accumulate hi*hi + lo*hi + hi*lo (the lo*lo term is below 2^-22 |a||b|):
 //       F16 = true  (default): hi = fp16(x*s), lo = fp16(x*s - hi) with one power-of-two scale s per tensor (undone exactly in
-//                    the epilogue), kind::f16, 32 channels per K-block  -> 0.37 ms per 256->256 layer at the headline shape;
-//       F16 = false: hi = x with the 13 low mantissa bits cleared (exact TF32), lo = x - hi (exact), kind::tf32, 16 channels
-//                    per K-block (half the MMA rate)                    -> 0.62 ms per layer.
-//   * TMEM: the tensor core adds into the fp32 accumulator with truncation, i.e. every accumulate step costs ~0.5 ulp of
-//     the accumulator (measured with one accumulator: 2-5e-5 relative).  The two small correction products therefore go to
-//     their OWN 256-column accumulator (their truncation is 2^-11 smaller in absolute terms); the epilogue adds the two in
-//     fp32 (round-to-nearest).  512 columns = whole TMEM, so the epilogue of a tile cannot overlap the next tile's MMAs
-//     beyond the early release below — measured cost 0.05 ms of 0.37 ms per layer.
-//   * warp roles (192 threads, 1 CTA / SM, persistent over tiles): warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM
-//     allocator), warps 2-5 = epilogue.  Four 48 KB smem stages (mbarrier full/empty ring): with two 96 KB stages the tensor
-//     pipe was only 62 % busy (ncu) because one K-block of loads could not hide behind one K-block of MMAs.
-//   * epilogue: per 32-column chunk tcgen05.ld (main + correction) -> one tcgen05.wait::ld -> add, scale, bias -> staged in a
-//     double-buffered SWIZZLE_128B smem tile -> cp.async.bulk.tensor.4d store (the TMA unit clips partial edge tiles);
-//     GroupNorm sum / sum of squares per (image, group) by a halving butterfly over the 32 lanes + fp64 atomics; the TMEM
-//     "empty" barrier is arrived right after the last tcgen05.ld so the next tile's MMAs start while the tail is stored.
+//                    the epilogue), m64nNk16, 32 channels per K-block;
+//       F16 = false: hi = x with the 13 low mantissa bits cleared (exact TF32), lo = x - hi (exact), m64n128k8 tf32, 16 channels
+//                    per K-block (half the MMA rate).
+//   * The tensor core adds into its fp32 accumulator without round-to-nearest, i.e. every accumulate step costs up to ~0.5 ulp of
+//     the accumulator.  The two small correction products therefore go to their OWN accumulator (their error is 2^-11 smaller in
+//     absolute terms); the epilogue adds the two in fp32 (round-to-nearest).
+//   * warp roles (384 threads, 1 CTA / SM, persistent over (tile, channel slice) items): warpgroup 0 = TMA producer (one thread),
+//     warpgroups 1 and 2 = MMA + epilogue for pixel rows 0-63 / 64-127 of the tile, each holding two 64 x NT fp32 accumulators in
+//     registers (128 per thread at NT = 128).  Six 32 KB shared-memory stages (mbarrier full / empty ring): the producer runs ahead
+//     into the next item while the MMA warpgroups store the previous one.
+//   * epilogue: straight from the accumulator registers (add, scale, bias) to global memory (8-byte stores, 32 contiguous bytes per
+//     row and quad); GroupNorm sum / sum of squares per (image, group of 8 channels) by a halving butterfly over the 32 lanes of a
+//     warp + one fp64 atomic per lane.
 #include "tc_ptx.cuh"
 #include <stdlib.h>
+#include <type_traits>
 
 namespace ptb {
 
-constexpr int CV_TH = 8, CV_TW = 16;            // output tile (pixels)
-constexpr int CV_BM = CV_TH * CV_TW;            // 128
-constexpr int CV_N = 256;                       // output channels
+constexpr int CV_N = 256;                       // output channels of the tower convolutions
+constexpr int CV_BM = 128;                      // output pixels per tile
+constexpr int CV_NT = 128;                      // widest output-channel slice of one item
 constexpr int CV_KB = 16;                       // fp32/TF32 input channels per K-block (64 B = one SWIZZLE_64B row)
 constexpr int CV_KB_F16 = 32;                   // fp16 input channels per K-block (also 64 B)
-constexpr int CV_STAGES = 4;                    // 4 x 48 KB ring: 3 K-blocks of loads in flight behind the MMA
-constexpr uint32_t CV_A_BYTES = CV_BM * CV_KB * 4;          // 8 KB
-constexpr uint32_t CV_B_BYTES = CV_N * CV_KB * 4;           // 16 KB
-constexpr uint32_t CV_STAGE_BYTES = 2 * CV_A_BYTES + 2 * CV_B_BYTES;   // 48 KB
-constexpr uint32_t CV_OUT_BYTES = CV_BM * 32 * 4;              // one 128-row x 32-column fp32 output chunk (16 KB)
-constexpr uint32_t CV_SMEM_BYTES = CV_STAGES * CV_STAGE_BYTES + 2 * CV_OUT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int CV_THREADS = 192;
-// CTA-pair mode (CL = 3): each CTA stages half of the weight tile -> 32 KB stages, five of them, and the freed shared memory holds a
-// second pair of output staging buffers for a second group of four epilogue warps (columns 128..255): the accumulators are read out
-// twice as fast, and it is this read-out — not the stores — that keeps the tensor pipe waiting between tiles (TMEM is full).
-constexpr int CV_STAGES_PAIR = 5;
-constexpr uint32_t CV_STAGE_BYTES_PAIR = 2 * CV_A_BYTES + CV_B_BYTES;                                  // 32 KB
-constexpr int CV_THREADS_PAIR = 64 + 8 * 32;                                                           // TMA + MMA + 8 epilogue warps
-constexpr uint32_t CV_SMEM_BYTES_PAIR = CV_STAGES_PAIR * CV_STAGE_BYTES_PAIR + 4 * CV_OUT_BYTES + 1024 + 256;
+constexpr int CV_STAGES = 6;                    // 6 x 32 KB ring
+constexpr uint32_t CV_A_BYTES = CV_BM * 64;                 // 8 KB
+constexpr uint32_t CV_B_BYTES = CV_NT * 64;                 // 8 KB (a narrower slice uses the front of it)
+constexpr uint32_t CV_STAGE_BYTES = 2 * CV_A_BYTES + 2 * CV_B_BYTES;   // 32 KB
+constexpr uint32_t CV_SMEM_BYTES = CV_STAGES * CV_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int CV_THREADS = 384;
 
-// K-major, SWIZZLE_64B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): 8-row atoms of 64 B rows,
-// atoms 512 B apart (SBO), version 1 (sm_100), layout type 4 (SWIZZLE_64B)
-__device__ __forceinline__ uint64_t umma_desc_sw(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);            // start address  [0,14)
-  d |= (uint64_t)1 << 16;                                  // leading byte offset (unused for swizzled K-major) = 1
-  d |= (uint64_t)((8 * CV_KB * 4) >> 4) << 32;             // stride byte offset  [32,46): 8 rows x 64 B
-  d |= (uint64_t)1 << 46;                                  // version = 1
-  d |= (uint64_t)4 << 61;                                  // SWIZZLE_64B
-  return d;
-}
-// cute::UMMA::InstrDescriptor for kind::tf32: D=f32, A=B=tf32, both K-major, M=128, N=256, dense, no negate
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_m128_n256() {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(CV_N >> 3) << 17) | ((uint32_t)(CV_BM >> 4) << 24);
-}
-// same for kind::f16 with fp16 operands (a_format = b_format = F16 = 0), fp32 accumulate
-__host__ __device__ constexpr uint32_t umma_idesc_f16_m128_n256() {
-  return (1u << 4) | ((uint32_t)(CV_N >> 3) << 17) | ((uint32_t)(CV_BM >> 4) << 24);
-}
-
-// Output tiling (round 2).  A tile is always 128 pixels (the UMMA M of one CTA); the main region uses 8 x 16 tiles and the two edge
-// strips that 8 x 16 tiles would cover half-empty get their own shapes: a bottom strip of <= 4 rows is covered by 4 x 32 tiles, a right
-// strip of <= 8 columns by 16 x 8 tiles.  At the headline 100 x 168 map that is 132 tiles per image instead of 143 (13 x 11 with the
-// last tile row and column half outside the image): 7.7 % fewer MMAs, loads and epilogues for the same output.
+// Output tiling.  A tile is always 128 pixels; the main region uses 8 x 16 tiles and the two edge strips that 8 x 16 tiles would
+// cover half-empty get their own shapes: a bottom strip of <= 4 rows is covered by 4 x 32 tiles, a right strip of <= 8 columns by
+// 16 x 8 tiles.  At the 100 x 168 map that is 132 tiles per image instead of 143 (13 x 11 with the last tile row and column half
+// outside the image): 7.7 % fewer MMAs and loads for the same output.
 //   shape 0: 8 h x 16 w (main)     shape 1: 4 h x 32 w (bottom strip, all columns)     shape 2: 16 h x 8 w (right strip, rows above the bottom strip)
 struct ConvShape {
   int B, H, W, Cin;
@@ -85,21 +56,15 @@ struct ConvShape {
   int n_main, n_right, n_bottom, per_img, n_tiles;
   int right_w0, right_h;  // right strip: first column, number of rows it covers (rows below belong to the bottom strip)
   int bottom_h0;          // bottom strip: first row
-  // Tail wave (pair mode): the n_groups tile pairs are dealt round-robin to the n_units CTA pairs, `q_full` full rounds and a last round
-  // of `rem` pairs that used to leave most SMs idle for a whole tile time (528 = 7 x 74 + 10 at the headline shape).  The tail tiles are
-  // therefore split into `tail_s` column slices (N = 256 / tail_s output channels each, independent outputs: no reduction), one slice per
-  // unit: the last round takes ~1/tail_s of a tile time.  tail_s = 1: no split.
-  int q_full, rem, tail_s;
+  int n_slices;           // output-channel slices of NT channels per tile: item = tile * n_slices + slice
   int taps;       // 9: conv3x3 (pad 1), 1: conv1x1 / per-cell Linear
-  int n_mma;      // MMA N (multiple of 16, <= 256): output channels rounded up; weight rows beyond n_out are zero
   int n_out;      // output channels actually stored
   int ldy;        // floats per output pixel row
 };
 
-struct ConvMaps {          // by-value __grid_constant__ kernel argument (15 x 128 B)
+struct ConvMaps {          // by-value __grid_constant__ kernel argument
   CUtensorMap x[3][2];     // activations (hi, lo) with the box of tile shape 0 / 1 / 2
-  CUtensorMap y[3];        // output, same boxes (the right strip's map is clipped to right_h rows)
-  CUtensorMap w[3][2];     // packed weights (hi, lo); box rows = n_mma/2, n_mma/4, n_mma/8 (full tile, half- and quarter-width tail slices)
+  CUtensorMap w[2];        // packed weights (hi, lo); box rows = NT
 };
 struct TileAt {
   int b, h0, w0, shape, twl;     // image, origin, shape id, log2(tile width)
@@ -118,369 +83,162 @@ __device__ __forceinline__ TileAt tile_at(const ConvShape& cs, int tile) {
   return t;
 }
 
-struct WorkItem {
-  int grp;        // tile group (pair of tiles in cluster modes)
-  int n0, nn;     // output-channel slice [n0, n0 + nn) this unit computes for the group
-  int kind;       // 0: full width, 1: half, 2: quarter (selects the weight map)
-};
-// k-th work item of `unit`; false when the unit is done.  Rounds 0 .. q_full-1: group unit + k*n_units, full width; round q_full: the
-// tail (see ConvShape).  Every role of the CTA (producer, MMA issuer, epilogue) walks the same list.
-__device__ __forceinline__ bool work_item(const ConvShape& cs, int unit, int n_units, int k, WorkItem& wi) {
-  if (k < cs.q_full) { wi.grp = unit + k * n_units; wi.n0 = 0; wi.nn = cs.n_mma; wi.kind = 0; return true; }
-  if (k > cs.q_full || unit >= cs.rem * cs.tail_s) return false;
-  const int sl = unit / cs.rem;
-  wi.grp = cs.q_full * n_units + (unit - sl * cs.rem);
-  wi.nn = cs.n_mma / cs.tail_s;
-  wi.n0 = sl * wi.nn;
-  wi.kind = cs.tail_s == 4 ? 2 : (cs.tail_s == 2 ? 1 : 0);
-  return true;
-}
-
-// CL = 3 (round 2, default for 256-channel outputs): CTA PAIRS issuing ONE tcgen05.mma.cta_group::2 per product over both SMs
-// (M = 256 = the pair's two pixel tiles, N = 256): each CTA stages its own activation tile and only HALF of the weight tile, the
-// tensor cores exchange the halves.  Per CTA and K-step the shared-memory traffic drops from 36 KB of MMA operand reads + 24 KB of TMA
-// fill (160 B/clk at full tensor rate, above the 128 B/clk the SM has: ncu showed the tensor pipe 63 % active, l1tex 78 % busy) to
-// 24 KB + 16 KB (107 B/clk).  The leader CTA's MMA thread issues for both; its "full" barrier collects both CTAs' TMA bytes
-// (cp.async.bulk.tensor.cta_group::2 with the leader's barrier as completion target), tcgen05.commit.cta_group::2 multicasts the
-// "stage free" / "accumulator ready" arrivals to both CTAs, and the peer's epilogue warps release the accumulators with remote
-// mbarrier arrives.  Every CTA still stores its own 128-pixel tile and adds its own GroupNorm partial sums.
-// CL = 1: independent CTAs.  CL = 2: clusters of two CTAs working on neighbouring tiles in lock-step; each CTA fetches
-// its own activation tile and HALF of the weight tile, TMA-multicast into both CTAs' shared memory.  The weights are
-// 2/3 of the operand bytes, and the kernel is bound by the L2->SM operand stream (41 B/clk/SM measured), so this cuts
-// the stream per SM from 48 KB to 32 KB per K-block.
-// F16 = false: 3xTF32 (operands fp32 hi/lo).  F16 = true: 2-term fp16 split (x = h + l, 22 significant bits):
-// h*h + l*h + h*l with kind::f16 — the same three MMAs per k-step but K = 16 per MMA, i.e. HALF the tensor-pipe time
-// (the 3xTF32 kernel is tensor bound) and half the operand bytes.  out_scale undoes the power-of-two scaling of the
-// fp16 operands (exact).
-template <int CL, bool F16>
-__global__ void __launch_bounds__(CL == 3 ? CV_THREADS_PAIR : CV_THREADS, 1)
+// F16 = false: 3xTF32 (operands fp32 hi/lo).  F16 = true: 2-term fp16 split (x = h + l, 22 significant bits): h*h + l*h + h*l,
+// the same three MMAs per k-step but K = 16 per MMA, i.e. half the tensor-pipe time and half the operand bytes.  out_scale undoes
+// the power-of-two scaling of the fp16 operands (exact).  NT: output channels per item (16, 32, 64 or 128; 128 in TF32 mode).
+template <bool F16, int NT>
+__global__ void __launch_bounds__(CV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restrict__ y, double* __restrict__ stats /*[B][32][2] or NULL*/,
-                      float out_scale, const float* __restrict__ dev_out_scale, const float* __restrict__ bias) {
+               float out_scale, const float* __restrict__ dev_out_scale, const float* __restrict__ bias) {
+  static_assert(F16 || NT == 128, "the TF32 mode runs 128-channel slices");
   constexpr int KBC = F16 ? CV_KB_F16 : CV_KB;      // channels per K-block
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B atoms need 1024 B alignment
-  constexpr int NST = CL == 3 ? CV_STAGES_PAIR : CV_STAGES;              // smem ring depth
-  constexpr uint32_t STB = CL == 3 ? CV_STAGE_BYTES_PAIR : CV_STAGE_BYTES;
-  constexpr uint32_t BLO = CL == 3 ? CV_B_BYTES / 2 : CV_B_BYTES;        // offset of the weight lo tile behind the hi tile
-  constexpr int NEG = CL == 3 ? 2 : 1;                                   // epilogue warp groups (4 warps each, 128 / 256 columns each)
-  const uint32_t out_base = smem_base + NST * STB;                       // NEG x 2 x 16 KB output staging (SWIZZLE_128B rows)
-  const uint32_t bar_base = out_base + NEG * 2 * CV_OUT_BYTES;
-  // barriers: full[4] | empty[4] | tmem_full | tmem_empty | tmem_ptr
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // swizzle atoms need (at least) 512 B alignment
+  const uint32_t bar_base = smem_base + CV_STAGES * CV_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
-  auto tfull_bar = [&](int s) { return bar_base + 128u + 8u * s; };
-  auto tempty_bar = [&](int s) { return bar_base + 144u + 8u * s; };
-  const uint32_t tmem_slot = bar_base + 160u;
-  uint8_t* smem_aligned = smem_raw + (smem_base - smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_aligned + NST * STB + NEG * 2 * CV_OUT_BYTES + 160);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int kblocks_per_tap = cs.Cin / KBC;
   const int n_kb = cs.taps * kblocks_per_tap;
-  // work distribution: unit u = blockIdx.x / CL owns tile groups u, u + n_units, ...; CTA `rank` of the cluster takes
-  // tile CL*group + rank (a group's missing last tile is a dummy: loads + MMAs run, nothing is stored)
-  constexpr int CSZ = CL >= 2 ? 2 : 1;   // CTAs per cluster
-  const uint32_t rank = (CL >= 2) ? cluster_ctarank() : 0u;
-  const int unit = blockIdx.x / CSZ, n_units = gridDim.x / CSZ;
-  const int n_groups = (cs.n_tiles + CSZ - 1) / CSZ;
+  const int n_items = cs.n_tiles * cs.n_slices;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NST; ++s) {
+    for (int s = 0; s < CV_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), CL == 2 ? 2 : 1);       // CL 2: one tcgen05.commit per CTA of the cluster; CL 3: the leader's commit, multicast
+      mbar_init(empty_bar(s), 8);                    // one arrive per MMA warp
     }
-    mbar_init(tfull_bar(0), 1);
-    mbar_init(tempty_bar(0), CL == 3 ? 16 : 4);       // one arrive per epilogue warp (CL 3: 8 warps of BOTH CTAs, on the leader's barrier)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {     // TMEM: 512 columns = 2 accumulators of 128 lanes x 256 fp32 columns
-    if (CL == 3) {     // pair allocation: one warp of EACH CTA
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CL >= 2) cluster_sync_all();       // the peer's barriers exist before any multicast / remote arrive can land
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // =============================== TMA producer ===============================
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      WorkItem wi;
-      for (int k = 0; work_item(cs, unit, n_units, k, wi); ++k) {
-        const int grp = wi.grp;
-        const uint32_t b_bytes = (uint32_t)wi.nn * 64u;            // one weight operand tile of this item: nn rows x 64 B
-        const uint32_t stage_tx = 2 * CV_A_BYTES + 2 * b_bytes;
-        const int w_half = wi.nn / 2;
-        int tile = CSZ * grp + (int)rank;
-        if (tile >= cs.n_tiles) tile = cs.n_tiles - 1;              // dummy: re-load a valid tile, never stored
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int tile = item / cs.n_slices, n0 = (item - tile * cs.n_slices) * NT;
         const TileAt ta = tile_at(cs, tile);
-        const int b = ta.b, h0 = ta.h0, w0 = ta.w0;
-        const CUtensorMap* tm_xhi_p = &mp.x[ta.shape][0];
-        const CUtensorMap* tm_xlo_p = &mp.x[ta.shape][1];
         for (int kb = 0; kb < n_kb; ++kb) {
           const int tap = kb / kblocks_per_tap, cblk = kb - tap * kblocks_per_tap;
           const int kh = cs.taps == 9 ? tap / 3 : 1, kw = cs.taps == 9 ? tap - (tap / 3) * 3 : 1;
           mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sA_hi = smem_base + stage * STB;
+          const uint32_t sA_hi = smem_base + stage * CV_STAGE_BYTES;
           const uint32_t sA_lo = sA_hi + CV_A_BYTES;
           const uint32_t sB_hi = sA_lo + CV_A_BYTES;
-          const uint32_t sB_lo = sB_hi + BLO;
+          const uint32_t sB_lo = sB_hi + CV_B_BYTES;
           const int kcol = tap * cs.Cin + cblk * KBC;
-          if (CL == 3) {
-            // pair mode: my activation tile + MY half of the weight tile into my shared memory; all bytes are counted on the LEADER's barrier
-            const uint32_t lead_full = mapa_rank(full_bar(stage), 0u);
-            if (rank == 0) mbar_expect_tx(full_bar(stage), 2u * (2 * CV_A_BYTES + b_bytes));      // both CTAs: 2 x (A hi + lo + half B hi + lo)
-            tma_load_4d_pair(tm_xhi_p, lead_full, sA_hi, cblk * KBC, w0 + kw - 1, h0 + kh - 1, b);
-            tma_load_4d_pair(tm_xlo_p, lead_full, sA_lo, cblk * KBC, w0 + kw - 1, h0 + kh - 1, b);
-            tma_load_2d_pair(&mp.w[wi.kind][0], lead_full, sB_hi, kcol, wi.n0 + (int)rank * w_half);
-            tma_load_2d_pair(&mp.w[wi.kind][1], lead_full, sB_lo, kcol, wi.n0 + (int)rank * w_half);
-            if (++stage == NST) { stage = 0; phase ^= 1u; }
-            continue;
-          }
-          mbar_expect_tx(full_bar(stage), stage_tx);
-          tma_load_4d(tm_xhi_p, full_bar(stage), sA_hi, cblk * KBC, w0 + kw - 1, h0 + kh - 1, b);
-          tma_load_4d(tm_xlo_p, full_bar(stage), sA_lo, cblk * KBC, w0 + kw - 1, h0 + kh - 1, b);
-          if (CL == 2) {     // my 128-row half of the weight tile, delivered to both CTAs (and both full barriers)
-            const uint32_t half = rank * (b_bytes / 2);
-            tma_load_2d_mc(&mp.w[0][0], full_bar(stage), sB_hi + half, kcol, (int)rank * (cs.n_mma / 2), (uint16_t)0x3);
-            tma_load_2d_mc(&mp.w[0][1], full_bar(stage), sB_lo + half, kcol, (int)rank * (cs.n_mma / 2), (uint16_t)0x3);
-          } else {
-            tma_load_2d(&mp.w[0][0], full_bar(stage), sB_hi, kcol, 0);
-            tma_load_2d(&mp.w[0][0], full_bar(stage), sB_hi + b_bytes / 2, kcol, cs.n_mma / 2);
-            tma_load_2d(&mp.w[0][1], full_bar(stage), sB_lo, kcol, 0);
-            tma_load_2d(&mp.w[0][1], full_bar(stage), sB_lo + b_bytes / 2, kcol, cs.n_mma / 2);
-          }
-          if (++stage == NST) { stage = 0; phase ^= 1u; }
+          mbar_expect_tx(full_bar(stage), 2 * CV_A_BYTES + 2 * NT * 64);
+          tma_load_4d(&mp.x[ta.shape][0], full_bar(stage), sA_hi, cblk * KBC, ta.w0 + kw - 1, ta.h0 + kh - 1, ta.b);
+          tma_load_4d(&mp.x[ta.shape][1], full_bar(stage), sA_lo, cblk * KBC, ta.w0 + kw - 1, ta.h0 + kh - 1, ta.b);
+          tma_load_2d(&mp.w[0], full_bar(stage), sB_hi, kcol, n0);
+          tma_load_2d(&mp.w[1], full_bar(stage), sB_lo, kcol, n0);
+          if (++stage == CV_STAGES) { stage = 0; phase ^= 1u; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (lane == 0 && (CL != 3 || rank == 0)) {          // pair mode: the leader's thread issues for both CTAs
-      uint32_t idesc0 = (F16 ? umma_idesc_f16_m128_n256() : umma_idesc_tf32_m128_n256()) & ~(0x3Fu << 17);
-      if (CL == 3) idesc0 = (idesc0 & ~(0x1Fu << 24)) | ((uint32_t)(256 >> 4) << 24);      // M = 256 across the pair
-      int stage = 0;
-      uint32_t phase = 0;
-      WorkItem wi;
-      for (int it = 0; work_item(cs, unit, n_units, it, wi); ++it) {
-        const uint32_t idesc = idesc0 | ((uint32_t)(wi.nn >> 3) << 17);                      // N = this item's channel slice
-        const int acc = 0;
-        const uint32_t acc_phase = (uint32_t)it & 1u;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);          // epilogue has drained the accumulators
-        tc_fence_after();
-        const uint32_t d_main = tmem_base, d_corr = tmem_base + CV_N;
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sA_hi = smem_base + stage * STB;
-          const uint32_t sA_lo = sA_hi + CV_A_BYTES;
-          const uint32_t sB_hi = sA_lo + CV_A_BYTES;
-          const uint32_t sB_lo = sB_hi + BLO;
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {                       // UMMA_K = 32 B (8 tf32 / 16 fp16) inside the 64 B swizzle row
-            const uint64_t a_hi = umma_desc_sw(sA_hi + 32u * k), a_lo = umma_desc_sw(sA_lo + 32u * k);
-            const uint64_t b_hi = umma_desc_sw(sB_hi + 32u * k), b_lo = umma_desc_sw(sB_lo + 32u * k);
-            if (CL == 3) {
-              umma_ss_pair<F16>(d_main, a_hi, b_hi, idesc, (kb | k) != 0);
-              umma_ss_pair<F16>(d_corr, a_lo, b_hi, idesc, (kb | k) != 0);
-              umma_ss_pair<F16>(d_corr, a_hi, b_lo, idesc, 1u);
-            } else {
-              umma_ss<F16>(d_main, a_hi, b_hi, idesc, (kb | k) != 0);
-              umma_ss<F16>(d_corr, a_lo, b_hi, idesc, (kb | k) != 0);
-              umma_ss<F16>(d_corr, a_hi, b_lo, idesc, 1u);
-            }
-          }
-          if (CL == 3) umma_commit_pair(empty_bar(stage), (uint16_t)0x3);      // stage free in both CTAs
-          else if (CL == 2) umma_commit_mc(empty_bar(stage), (uint16_t)0x3);   // stage free in BOTH CTAs' books
-          else umma_commit(empty_bar(stage));                  // smem stage free once these MMAs have read it
-          if (++stage == NST) { stage = 0; phase ^= 1u; }
-        }
-        if (CL == 3) umma_commit_pair(tfull_bar(acc), (uint16_t)0x3);          // both CTAs' halves of the accumulators are complete
-        else umma_commit(tfull_bar(acc));                      // accumulator complete
       }
     }
   } else {
-    // =============================== epilogue (warps 2..5) ===============================
-    const int q = warp & 3;                                    // TMEM lane quarter this warp may access
-    const int eg = NEG == 2 ? (warp - 2) >> 2 : 0;             // epilogue group: columns [eg * 256 / NEG, (eg + 1) * 256 / NEG)
-    constexpr int CPG = (CV_N / 32) / NEG;                     // 32-column chunks per group
-    WorkItem wi;
-    for (int it = 0; work_item(cs, unit, n_units, it, wi); ++it) {
-      const int grp = wi.grp;
-      const int acc = 0;
-      const uint32_t acc_phase = (uint32_t)it & 1u;
-      const int tile_raw = CSZ * grp + (int)rank;
-      const bool dummy = tile_raw >= cs.n_tiles;
-      const int tile = dummy ? cs.n_tiles - 1 : tile_raw;
-      const TileAt ta = tile_at(cs, tile);
-      const int b = ta.b, h0 = ta.h0, w0 = ta.w0;
-      const CUtensorMap* tm_y_p = &mp.y[ta.shape];
-      const int row = q * 32 + lane;                           // GEMM row = pixel inside the tile (h-major, tile-width pixels per row)
-      const int h = h0 + (row >> ta.twl), w = w0 + (row & ((1 << ta.twl) - 1));
-      const bool valid = !dummy && (h < (ta.shape == 2 ? cs.right_h : cs.H)) && (w < cs.W);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      // TMEM chunk c of this item holds output columns 32 * (oc0 + c) ..; a tail slice has nn / 32 chunks, split between the groups
-      const int oc0 = wi.n0 >> 5;
-      const int n_chunks = min((cs.n_out + 31) / 32 - oc0, (wi.nn + 31) >> 5);
-      const int cpg_item = NEG == 2 ? max(1, (wi.nn >> 5) / NEG) : CPG;
-      const int c_lo = eg * cpg_item;
-      const float sc = F16 ? (dev_out_scale ? __fmul_rn(out_scale, *dev_out_scale) : out_scale) : 1.f;   // powers of two: exact
-      const bool issuer = (warp == 2 + 4 * eg) && (lane == 0);  // owns the bulk-store groups of its epilogue group
-      const int c_end = min(n_chunks, c_lo + cpg_item);        // this group's chunks: [c_lo, c_end)
-      auto grp_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + eg) : "memory"); };
-      // Chunk pipeline (8 x 32 columns, fully unrolled so every array index is static): the TMEM loads of chunk c+1 are in
-      // flight while chunk c is scaled, staged and stored; the GroupNorm partial sums stay in registers until the accumulators
-      // have been handed back to the MMA warp, so neither the TMEM latency nor the statistics sit in the exposed path.
-      uint32_t bx[32], by[32], bz[32];       // main accumulator chunks alternate between bx / bz, by takes the correction
-      float part[8 * CPG];                   // per-row (sum, sum of squares) of the 4 groups of each chunk
-      const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-      if (c_lo < c_end) {
-        tmem_ld32_nowait(t_lane + (uint32_t)(c_lo * 32), bx);
-        tmem_ld32_nowait(t_lane + (uint32_t)(CV_N + c_lo * 32), by);
+    // =============================== MMA + epilogue (warpgroups 1, 2) ===============================
+    regs_alloc<232>();
+    const int cw = wg - 1;                                   // pixel rows 64 cw .. 64 cw + 63 of the tile
+    const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+    const float sc = F16 ? (dev_out_scale ? __fmul_rn(out_scale, *dev_out_scale) : out_scale) : 1.f;   // powers of two: exact
+    float acc[NT / 2], cor[NT / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int tile = item / cs.n_slices, n0 = (item - tile * cs.n_slices) * NT;
+      int prev = 0;
+      for (int kb = 0; kb < n_kb; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t sA_hi = smem_base + stage * CV_STAGE_BYTES + (uint32_t)cw * (CV_A_BYTES / 2);
+        const uint32_t sA_lo = sA_hi + CV_A_BYTES;
+        const uint32_t sB_hi = smem_base + stage * CV_STAGE_BYTES + 2 * CV_A_BYTES;
+        const uint32_t sB_lo = sB_hi + CV_B_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {                        // 32 B (16 fp16 / 8 tf32) of K per MMA inside the 64 B swizzle row
+          const uint64_t a_hi = gmma_desc(sA_hi + 32u * k, 16u, 512u, GMMA_SW64), a_lo = gmma_desc(sA_lo + 32u * k, 16u, 512u, GMMA_SW64);
+          const uint64_t b_hi = gmma_desc(sB_hi + 32u * k, 16u, 512u, GMMA_SW64), b_lo = gmma_desc(sB_lo + 32u * k, 16u, 512u, GMMA_SW64);
+          const uint32_t first = (kb | k) != 0;
+          if constexpr (F16) {
+            wgmma_f16<0, 0>(acc, a_hi, b_hi, first);
+            wgmma_f16<0, 0>(cor, a_lo, b_hi, first);
+            wgmma_f16<0, 0>(cor, a_hi, b_lo, 1u);
+          } else {
+            wgmma_tf32(acc, a_hi, b_hi, first);
+            wgmma_tf32(cor, a_lo, b_hi, first);
+            wgmma_tf32(cor, a_hi, b_lo, 1u);
+          }
+        }
+        wgmma_commit();
+        if (kb > 0) {                                        // the previous K-block's MMAs have read their stage: hand it back
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(empty_bar(prev));
+        }
+        prev = stage;
+        if (++stage == CV_STAGES) { stage = 0; phase ^= 1u; }
       }
-      auto chunk = [&](const int j_, const int c, uint32_t (&cur)[32], uint32_t (&nxt)[32]) {
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float f = __fadd_rn(__uint_as_float(cur[j]), __uint_as_float(by[j]));
-          if (F16) f = __fmul_rn(f, sc);
-          cur[j] = __float_as_uint(f);
-        }
-        if (c + 1 < c_end) {
-          tmem_ld32_nowait(t_lane + (uint32_t)((c + 1) * 32), nxt);
-          tmem_ld32_nowait(t_lane + (uint32_t)(CV_N + (c + 1) * 32), by);
-        } else {                       // accumulators fully read: the MMA warp may start the next tile under the stores
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (CL == 3) mbar_arrive_cluster(mapa_rank(tempty_bar(acc), 0u));      // the leader's MMA thread waits for all 8 warps
-            else mbar_arrive(tempty_bar(acc));
-          }
-        }
-        if (bias) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int col = (oc0 + c) * 32 + j;
-            if (col < cs.n_out) cur[j] = __float_as_uint(__uint_as_float(cur[j]) + __ldg(bias + col));
-          }
-        }
-        // ---- stage the 128 x 32 chunk in shared memory (SWIZZLE_128B: 16-byte slot j of row r lives at slot j ^ (r & 7),
-        //      so the 32 lanes of a warp, one row each, write conflict-free) and hand it to the TMA unit: one bulk tensor
-        //      store per chunk, fully coalesced, and the tile's out-of-range rows / columns are clipped by the hardware.
-        const uint32_t buf = out_base + (uint32_t)(2 * eg + (j_ & 1)) * CV_OUT_BYTES;
-        if (issuer) tma_store_wait_read<1>();                    // the store issued two chunks ago has drained this buffer
-        grp_bar();
-        {
-          const uint32_t row_addr = buf + (uint32_t)row * 128u;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint32_t slot = (uint32_t)(j ^ (row & 7));
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row_addr + slot * 16u), "r"(cur[4 * j]), "r"(cur[4 * j + 1]),
-                         "r"(cur[4 * j + 2]), "r"(cur[4 * j + 3])
-                         : "memory");
-          }
-        }
-        fence_async_smem();
-        grp_bar();
-        if (issuer && !dummy) {
-          tma_store_4d(tm_y_p, buf, (oc0 + c) * 32, w0, h0, b);
-          tma_store_commit();
-        }
-        if (stats) {
-          // GroupNorm(32 groups of 8 channels): this chunk covers groups 4c .. 4c+3; per-row partials only, reduced below
-#pragma unroll
-          for (int gq = 0; gq < 4; ++gq) {
-            float s = 0.f, ss = 0.f;
-            if (valid) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float f = __uint_as_float(cur[8 * gq + j]);
-                s += f;
-                ss = fmaf(f, f, ss);
-              }
-            }
-            part[8 * j_ + 2 * gq] = s;
-            part[8 * j_ + 2 * gq + 1] = ss;
-          }
-        }
-      };
-#pragma unroll
-      for (int j_ = 0; j_ < CPG; ++j_) {
-        const int c = c_lo + j_;
-        if (c < c_end) {
-          if (j_ & 1) chunk(j_, c, bz, bx);
-          else chunk(j_, c, bx, bz);
-        }
-      }
-      if (stats) {
-        // halving butterfly over the 32 rows of the warp per chunk: 9 shuffles instead of 40, the 8 totals end up on lanes
-        // 0,4,..,28 which issue one fp64 atomic each.  Runs while the MMA warp is already working on the next tile.
-#pragma unroll
-        for (int j_ = 0; j_ < CPG; ++j_) {
-          const int c = c_lo + j_;
-          if (c < c_end) {
-            float t[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) t[i] = part[8 * j_ + i];
-            {
-              const bool up = (lane & 16) != 0;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float send = up ? t[i] : t[i + 4];
-                const float recv = __shfl_xor_sync(0xffffffffu, send, 16);
-                t[i] = (up ? t[i + 4] : t[i]) + recv;
-              }
-            }
-            {
-              const bool up = (lane & 8) != 0;
-#pragma unroll
-              for (int i = 0; i < 2; ++i) {
-                const float send = up ? t[i] : t[i + 2];
-                const float recv = __shfl_xor_sync(0xffffffffu, send, 8);
-                t[i] = (up ? t[i + 2] : t[i]) + recv;
-              }
-            }
-            {
-              const bool up = (lane & 4) != 0;
-              const float send = up ? t[0] : t[1];
-              const float recv = __shfl_xor_sync(0xffffffffu, send, 4);
-              t[0] = (up ? t[1] : t[0]) + recv;
-            }
-            t[0] += __shfl_xor_sync(0xffffffffu, t[0], 2);
-            t[0] += __shfl_xor_sync(0xffffffffu, t[0], 1);
-            if ((lane & 3) == 0) {
-              const int idx = ((lane & 16) ? 4 : 0) + ((lane & 8) ? 2 : 0) + ((lane & 4) ? 1 : 0);   // = 2*gq + {0: sum, 1: sumsq}
-              atomicAdd(stats + ((size_t)b * 32 + (4 * (oc0 + c) + (idx >> 1))) * 2 + (idx & 1), (double)t[0]);
-            }
-          }
-        }
-      }
-      if (c_lo >= c_end) {                   // nothing to read for this group (narrow outputs): release the accumulators right away
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (CL == 3) mbar_arrive_cluster(mapa_rank(tempty_bar(acc), 0u));
-          else mbar_arrive(tempty_bar(acc));
-        }
-      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
 
+      // ---- epilogue: rows r0 and r0 + 8, columns n0 + 8 i + 2 (lane % 4) (+1) ----
+      const TileAt ta = tile_at(cs, tile);
+      const int h_end = ta.shape == 2 ? cs.right_h : cs.H;   // the right strip stops where the bottom strip begins
+      float* row_ptr[2];
+      bool valid[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int r = 64 * cw + 16 * warp + (lane >> 2) + 8 * j;
+        const int h = ta.h0 + (r >> ta.twl), w = ta.w0 + (r & ((1 << ta.twl) - 1));
+        valid[j] = h < h_end && w < cs.W;
+        row_ptr[j] = y + (((size_t)ta.b * cs.H + h) * cs.W + w) * cs.ldy;
+      }
+      float part[NT == 128 ? 32 : 1];                        // per group of 8 channels: (sum, sum of squares) of this thread's values
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int col = n0 + 8 * i + 2 * (lane & 3);
+        float s = 0.f, ss = 0.f;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          float v0 = __fadd_rn(acc[4 * i + 2 * j], cor[4 * i + 2 * j]);
+          float v1 = __fadd_rn(acc[4 * i + 2 * j + 1], cor[4 * i + 2 * j + 1]);
+          if (F16) { v0 = __fmul_rn(v0, sc); v1 = __fmul_rn(v1, sc); }
+          if (bias) {
+            if (col < cs.n_out) v0 = v0 + __ldg(bias + col);
+            if (col + 1 < cs.n_out) v1 = v1 + __ldg(bias + col + 1);
+          }
+          if (valid[j]) {
+            if (col + 1 < cs.n_out) *reinterpret_cast<float2*>(row_ptr[j] + col) = make_float2(v0, v1);
+            else if (col < cs.n_out) row_ptr[j][col] = v0;
+            s += v0 + v1;
+            ss = fmaf(v0, v0, ss);
+            ss = fmaf(v1, v1, ss);
+          }
+        }
+        if constexpr (NT == 128) { part[2 * i] = s; part[2 * i + 1] = ss; }
+      }
+      if constexpr (NT == 128) {
+        if (stats) {
+          // halving butterfly: 32 values (16 groups x {sum, sumsq}) over 32 lanes in 31 shuffles; lane L ends with value L
+          auto level = [&](auto o_) {
+            constexpr int o = decltype(o_)::value;
+            const bool up = (lane & o) != 0;
+#pragma unroll
+            for (int i = 0; i < o; ++i) {
+              const float send = up ? part[i] : part[i + o];
+              const float recv = __shfl_xor_sync(0xffffffffu, send, o);
+              part[i] = (up ? part[i + o] : part[i]) + recv;
+            }
+          };
+          level(std::integral_constant<int, 16>{}); level(std::integral_constant<int, 8>{}); level(std::integral_constant<int, 4>{});
+          level(std::integral_constant<int, 2>{}); level(std::integral_constant<int, 1>{});
+          atomicAdd(stats + ((size_t)ta.b * 32 + (n0 >> 3) + (lane >> 1)) * 2 + (lane & 1), (double)part[0]);
+        }
+      }
     }
-  }
-  if (warp >= 2 && ((warp - 2) & 3) == 0 && lane == 0) tma_store_wait_all();     // every bulk tensor store of this CTA has landed
-  __syncthreads();
-  if (CL >= 2) cluster_sync_all();       // no CTA exits while the peer can still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    if (CL == 3) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
   }
 }
 
@@ -550,7 +308,7 @@ __device__ __forceinline__ float amax4(float m, const float4 v) {
   return fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
 }
 
-// pure HBM read: four independent 16-byte loads in flight per thread (B200 needs ~40 KB in flight per SM to saturate HBM)
+// pure HBM read: four independent 16-byte loads in flight per thread (tens of KB in flight per SM are needed to saturate HBM)
 __global__ void __launch_bounds__(256) amax_abs_kernel(const float4* __restrict__ x, long long n4, unsigned int* __restrict__ out_bits) {
   float m = 0.f;
   const long long step = (long long)gridDim.x * 256;
@@ -765,25 +523,12 @@ static int make_act_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, i
   if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(activation) failed: %s%lld", "", (long long)r);
   return 0;
 }
-static int make_out_map(CUtensorMap* tm, float* y, int B, int H, int W, int n_out, int ldy, int shape, int h_clip) {
-  EncodeTiledFn enc = tc_get_encode();
-  if (!enc) return fail("%s", "cuTensorMapEncodeTiled is unavailable (driver too old?)");
-  // columns >= n_out and rows >= h_clip (<= H: the right strip stops where the bottom strip begins) are clipped by the TMA unit
-  cuuint64_t dims[4] = {(cuuint64_t)n_out, (cuuint64_t)W, (cuuint64_t)h_clip, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)ldy * 4, (cuuint64_t)W * ldy * 4, (cuuint64_t)H * W * ldy * 4};
-  cuuint32_t box[4] = {32, (cuuint32_t)CV_SHAPE_TW[shape], (cuuint32_t)CV_SHAPE_TH[shape], 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(output) failed: %s%lld", "", (long long)r);
-  return 0;
-}
 static int make_w_map(CUtensorMap* tm, const void* ptr, int n_mma, int Ktot, bool f16, int box_rows) {
   EncodeTiledFn enc = tc_get_encode();
   if (!enc) return fail("%s", "cuTensorMapEncodeTiled is unavailable (driver too old?)");
   cuuint64_t dims[2] = {(cuuint64_t)Ktot, (cuuint64_t)n_mma};
   cuuint64_t strides[1] = {(cuuint64_t)Ktot * (f16 ? 2 : 4)};
-  cuuint32_t box[2] = {(cuuint32_t)(f16 ? CV_KB_F16 : CV_KB), (cuuint32_t)box_rows};   // half a weight tile (or tail slice) per TMA request
+  cuuint32_t box[2] = {(cuuint32_t)(f16 ? CV_KB_F16 : CV_KB), (cuuint32_t)box_rows};   // one channel slice per TMA request
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(tm, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -815,6 +560,18 @@ extern "C" int ptb_conv3x3_pack_weight(const float* w_oihw, int Cout, int Cin, f
   return check_launch("ptb_conv3x3_pack_weight");
 }
 
+template <bool F16, int NT>
+static int conv_launch_nt(const ConvMaps& mp, const ConvShape& cs, float* y, double* gn_stats, float out_scale, const float* dev_out_scale,
+                          const float* bias, void* stream) {
+  // a function attribute is per DEVICE and a process may drive several: set it on every call (a few hundred ns)
+  if (cudaFuncSetAttribute(conv_tc_kernel<F16, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess)
+    return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the conv kernel");
+  int grid = sm_count();                                     // persistent: one CTA per SM
+  if (grid > cs.n_tiles * cs.n_slices) grid = cs.n_tiles * cs.n_slices;
+  conv_tc_kernel<F16, NT><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias);
+  return 0;
+}
+
 template <bool F16>
 static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, int H, int W, int Cin, int taps,
                        int n_out, int n_mma, float* y, int ldy, const float* bias, double* gn_stats, float out_scale,
@@ -836,68 +593,26 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
     cs.per_img = cs.n_main + cs.n_right + cs.n_bottom;
     cs.n_tiles = B * cs.per_img;
   }
+  // narrowest slice width that covers the output channels (the MMA N); 256-channel outputs run as two 128-channel slices
+  const int nt = (!F16 || n_mma > 64) ? CV_NT : n_mma > 32 ? 64 : n_mma > 16 ? 32 : 16;
+  // the epilogue's statistics index [B][32][2] as (slice start / 8 + group in slice): 256 channels = 32 groups of 8, 128-channel slices
+  PTB_REQUIRE(!gn_stats || (n_out == CV_N && n_mma == CV_N && nt == CV_NT), "GroupNorm statistics need 256 output channels (32 groups of 8)");
+  cs.n_slices = (n_mma + nt - 1) / nt;
+  cs.taps = taps; cs.n_out = n_out; cs.ldy = ldy;
   ConvMaps mp;
   int rc;
   for (int sh = 0; sh < 3; ++sh) {
-    if ((rc = make_out_map(&mp.y[sh], y, B, H, W, n_out, ldy, sh, sh == 2 && cs.n_right > 0 ? cs.right_h : H))) return rc;
     if ((rc = make_act_map(&mp.x[sh][0], x_hi, B, H, W, Cin, F16, sh))) return rc;
     if ((rc = make_act_map(&mp.x[sh][1], x_lo, B, H, W, Cin, F16, sh))) return rc;
   }
-  for (int kd = 0; kd < 3; ++kd) {     // box rows n_mma/2 (full tile), /4 and /8 (tail slices; only used when n_mma == 256)
-    const int rows = (n_mma == CV_N) ? (n_mma / 2) >> kd : n_mma / 2;
-    if ((rc = make_w_map(&mp.w[kd][0], w_hi, n_mma, taps * Cin, F16, rows))) return rc;
-    if ((rc = make_w_map(&mp.w[kd][1], w_lo, n_mma, taps * Cin, F16, rows))) return rc;
-  }
-  cs.taps = taps; cs.n_mma = n_mma; cs.n_out = n_out; cs.ldy = ldy;
-  // a function attribute is per DEVICE and a process may drive several: set it on every call (a few hundred ns)
-  if (cudaFuncSetAttribute(conv_tc_kernel<1, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_tc_kernel<2, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_tc_kernel<3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES_PAIR) != cudaSuccess)
-    return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the conv kernel");
-  const int sms = sm_count();
-  // PTB_CONV_CLUSTER=2 selects the 2-CTA weight-multicast variant.  Measured on B200 it is exactly as fast as independent
-  // CTAs (0.648 vs 0.656 ms per 3xTF32 layer): that kernel is tensor-pipe bound (730 TFLOP/s of TF32 MMA work = what
-  // cuDNN's TF32 conv reaches on the same part), not operand-stream bound, so the simpler mode is the default.
-  // PTB_CONV_CLUSTER: 1 = independent CTAs, 2 = weight multicast between two cta_group::1 CTAs, 3 = CTA-pair MMA (cta_group::2).
-  // Default: 3 for the 256-channel 3x3 convolutions of the towers (the shapes it was validated on), 1 otherwise.
-  const char* e_cl = getenv("PTB_CONV_CLUSTER");
-  int cluster_mode = (n_mma == CV_N && taps == 9 && F16) ? 3 : 1;
-  if (e_cl && e_cl[0] >= '1' && e_cl[0] <= '3') cluster_mode = e_cl[0] - '0';
-  if (cluster_mode == 3 && (n_mma % 32 != 0 || !F16)) cluster_mode = 1;
-  if (cluster_mode >= 2 && cs.n_tiles >= 2 && sms >= 2) {
-    int grid = (sms / 2) * 2;
-    const int groups = (cs.n_tiles + 1) / 2;
-    if (grid > 2 * groups) grid = 2 * groups;
-    const int n_units = grid / 2;
-    cs.q_full = groups / n_units; cs.rem = groups % n_units; cs.tail_s = 1;
-    const char* e_ts = getenv("PTB_CONV_TAIL_SPLIT");          // "0": no tail split (A-B timing)
-    if (cluster_mode == 3 && n_mma == CV_N && cs.rem > 0 && !(e_ts && e_ts[0] == '0')) {
-      if (cs.rem * 4 <= n_units) cs.tail_s = 4;
-      else if (cs.rem * 2 <= n_units) cs.tail_s = 2;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(cluster_mode == 3 ? CV_THREADS_PAIR : CV_THREADS);
-    cfg.dynamicSmemBytes = cluster_mode == 3 ? CV_SMEM_BYTES_PAIR : CV_SMEM_BYTES;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cluster_mode == 3
-                        ? cudaLaunchKernelEx(&cfg, conv_tc_kernel<3, F16>, mp, cs, y, gn_stats, out_scale,
-                                             dev_out_scale, bias)
-                        : cudaLaunchKernelEx(&cfg, conv_tc_kernel<2, F16>, mp, cs, y, gn_stats, out_scale,
-                                             dev_out_scale, bias);
-    if (e != cudaSuccess) return fail("conv: cluster launch failed: %s", cudaGetErrorString(e));
-  } else {
-    int grid = sms;
-    if (grid > cs.n_tiles) grid = cs.n_tiles;
-    cs.q_full = cs.n_tiles / grid; cs.rem = cs.n_tiles % grid; cs.tail_s = 1;
-    conv_tc_kernel<1, F16><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y,
-                                                                                             gn_stats, out_scale, dev_out_scale, bias);
-  }
+  if ((rc = make_w_map(&mp.w[0], w_hi, n_mma, taps * Cin, F16, nt))) return rc;
+  if ((rc = make_w_map(&mp.w[1], w_lo, n_mma, taps * Cin, F16, nt))) return rc;
+  if (!F16) rc = conv_launch_nt<false, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if (nt == 128) rc = conv_launch_nt<true, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if (nt == 64) rc = conv_launch_nt<true, 64>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if (nt == 32) rc = conv_launch_nt<true, 32>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else rc = conv_launch_nt<true, 16>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  if (rc) return rc;
   return check_launch(what);
 }
 

@@ -7,8 +7,8 @@
 //     sample j ONCE (fp32 coordinate pipeline identical to ATen's), writes pts/valid for it;
 //   * the warp then walks the flattened (sample, float4-channel-group) space 32 lanes at a time, fetching the
 //     sample's taps from a per-warp shared-memory table (3 broadcast reads; the first version pulled them from the
-//     owning lane with 10 shuffles per step, and ncu showed the L1 data pipe — which also executes shuffles — 88 % busy
-//     with a quarter of its wavefronts spent on them): every 128-bit load reads a contiguous channels-last run
+//     owning lane with 10 shuffles per step, and the L1 data pipe — which also executes shuffles — spent a large share of
+//     its wavefronts on them): every 128-bit load reads a contiguous channels-last run
 //     (1 KB per tap at C=256) and every 128-bit store lands in a contiguous output row -> fully coalesced both ways;
 //   * map reads go through the read-only path (L1-cached: neighbouring samples of a bag share taps, the map of one
 //     image (17 MB) stays L2 resident); output uses streaming stores.
@@ -142,8 +142,7 @@ bag_gather_kernel(const float* __restrict__ map, int H, int W, int C, int ld,
 // ---------------------------------------------------------------------------------------------------------------------------------
 // TMA-staged variant (round 2).  Work item = (bag, channel chunk of CC = 64 or 32 channels): ONE cp.async.bulk.tensor box
 // {CC channels, WS, WS, 1 image} brings the bag's (2r+2)^2-cell window of the chunk into shared memory (83 KB at CC = 64, r = 8); the
-// 289 x 4 tap reads are then shared-memory reads.  Why: ncu (round 1) showed the LDG version limited by the L1 data pipe (88 % busy:
-// a warp-wide LDG.128 that touches 4 lines costs ~2 cycles per line, ~62 B/clk, while this kernel needs 4 tap bytes per output byte);
+// 289 x 4 tap reads are then shared-memory reads.  Why: the LDG version is limited by the L1 data pipe (a warp-wide LDG.128 that touches 4 lines costs ~2 cycles per line, ~62 B/clk, while this kernel needs 4 tap bytes per output byte);
 // LDS serves 128 B/clk and the window moves 1.33 GB through L2 instead of the ~2.4 GB of L1 misses.  Two CTAs per SM overlap one's
 // box load with the other's interpolation.  Bags whose window does not fit (rounding straddle) read global memory in the same code.
 // Outputs are bit-identical to bag_gather_kernel (same tap arithmetic, same FMA chain).
@@ -319,10 +318,9 @@ extern "C" int ptb_cpr_bag_gather(const float* map, int B, int H, int W, int C, 
   int CCk = (C % 64 == 0) ? 64 : ((C % 32 == 0) ? 32 : 0);
   if (e_cc && e_cc[0] == '3' && C % 32 == 0) CCk = 32;
   if (!e_cc && C % 32 == 0 && C < 256) CCk = 32;            // small windows: 4 CTAs per SM
-  // Measured at the headline batch (tools/profile_gather2.py, B200): C = 256: LDG kernel 0.317 ms vs TMA 0.365 (64-channel chunks) / 0.326
-  // (32-channel chunks); C = 160 (training logits): TMA 0.213 vs 0.223 ms; C = 80: equal.  The kernel is bound by the L1 / shared-memory
-  // data pipe either way (4 tap bytes read per byte written: ncu shows 69 % of the pipe's wavefronts busy at 0.36 ms with only 16 warps
-  // resident per SM beside two 92 KB windows), so the staged form only pays where its windows are small.  Default: TMA for C <= 192.
+  // The kernel is bound by the L1 / shared-memory data pipe either way (4 tap bytes read per byte written), and at C = 256 the two
+  // 92 KB staging windows leave few warps resident per SM, so the staged form only pays where its windows are small.  Default: TMA for
+  // C <= 192; tools/profile_gather2.py times both forms.
   const bool want_tma = e_tma ? (e_tma[0] != '0') : (C <= 192);
   if (want_tma && out_feats && reach_px > 0.f && CCk && (long long)G * (C / CCk) < (1ll << 31)) {
     const int WS = 2 * (int)ceilf(reach_px / stride) + 2;

@@ -1,6 +1,6 @@
 // Row-wise linear classifier over channels-last maps (the 1x1-conv form of CPRHead.cls_out / ins_out,
 // cpr_head.py:1008-1014, 1045-1078) and its two backward products.  fp32 FFMA ("parity mode", no TF32):
-// logits must match the reference CPU head to 1e-4, see DESIGN.md for the tcgen05 plan.
+// logits must match the reference CPU head to 1e-4, see DESIGN.md for the tensor-core plan.
 //
 // forward  Y[M][N]   = X[M][Cin] * Wt[N][Cin]^T + b       128x80 output tile / CTA, 8x5 micro-tile / thread
 // bwd_x    dX[M][Cin] = dY[M][N] * W[N][Cin]              same kernel with operand roles swapped (B given as [K][N])

@@ -15,9 +15,9 @@
 //      row staged in shared memory; (2) the <= 256 (record, tap) hits of the round are counting-sorted by cell (stable); (3) every
 //      (cell, channel group) thread walks its cell's hits in order: acc += w * staged row.
 // No atomics anywhere and every sum is evaluated by ONE thread in a FIXED order: bit-identical run to run, no zero-initialised gradient
-// map, no materialised (G,K,2N) gradient tensor (740 MB written and re-read in round 1).  ncu history: a first version (one warp per
-// (bag, chunk), per-(tap, channel) shared-memory atomics into 64-bit fixed point) took 3.1 ms with 64-bit CAS loops and 2.1 ms with
-// hi/lo 32-bit atomics — 680 M warp instructions, a third of the time at the block barrier; this layout needs ~2.5x fewer.
+// map, no materialised (G,K,2N) gradient tensor (740 MB written and re-read in round 1).  An earlier version (one warp per (bag, chunk),
+// per-(tap, channel) shared-memory atomics into 64-bit fixed point) spent its time in atomic loops and at the block barrier; this layout
+// issues about 2.5x fewer instructions.
 // Samples whose taps straddle a tile border are evaluated by each tile they touch (~1.25x).
 #include "ptb_common.cuh"
 #include <math_constants.h>

@@ -123,7 +123,7 @@ extern "C" int ptb_hungarian_v2_batch(const float* cost, const int64_t* desc, in
                              (int)ptb_lsap::cl_smem_bytes(ptb_lsap::CL_NMIN)) != cudaSuccess)
       return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for hungarian_v2_cluster_kernel");
     // cluster size: the largest of 8 / 6 / 5 CTAs per image with which every image of the batch is resident at once (a cluster lives
-    // inside one GPC: 15 clusters of 8 fit a B200, so 16 images at 8 CTAs would run as two waves); else the one with the most clusters
+    // inside one GPC, so fewer clusters of 8 than SMs / 8 may fit, and a batch that does not fit runs as two waves); else the one with the most clusters
     int ncta = 8, best_active = -1;
     const int cand[3] = {8, 6, 5};
     cudaLaunchAttribute attr[1];

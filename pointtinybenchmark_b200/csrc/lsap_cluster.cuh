@@ -1,8 +1,8 @@
 // HungarianAssignerV2's matching with the column scan of every Dijkstra step split over an 8-CTA thread-block cluster (round 2).
 //
-// Why: ncu of the one-CTA-per-image kernel (lsap_core.cuh, profiles/r02_ncu_hungarian_v2.json) shows ~980 instructions per thread and
-// Dijkstra step for the 17 columns a thread owns, issue slots 51 % busy on the ONE SM an image runs on and the rest of the time spent at
-// the block barrier: the step is bound by one SM's instruction issue, not by memory.  Here an image is solved by a cluster of CL_N CTAs:
+// Why: the one-CTA-per-image kernel (lsap_core.cuh) runs hundreds of instructions per thread and Dijkstra step for the columns a thread
+// owns, on the ONE SM an image runs on, and spends the rest of the time at the block barrier: the step is bound by one SM's instruction
+// issue, not by memory.  Here an image is solved by a cluster of CL_N CTAs:
 //   * CTA r owns the contiguous column range [r*Cc, (r+1)*Cc) and keeps ITS part of the per-step read-write column state (spc fp64,
 //     colstate int32, flags) in its own shared memory; a thread scans <= 5 columns, all global loads of a step in flight at once;
 //   * per step: block arg-best -> every CTA stores its candidate into the leader's shared memory (st.shared::cluster) -> cluster
@@ -34,8 +34,8 @@
 namespace ptb_lsap {
 
 constexpr int CL_N = 8;            // largest cluster (CTAs per image; the portable limit).  The host picks 8, 6 or 5 CTAs per image so that all
-                                   // images of a batch are resident at once: only 15 clusters of 8 fit a B200 (one GPC has < 16 SMs), 16 images
-                                   // at 8 CTAs ran as two waves (5.5 ms instead of 2.9 ms)
+                                   // images of a batch are resident at once (a cluster lives inside one GPC, so fewer clusters of 8 than SMs / 8
+                                   // may fit; a batch that does not fit runs as two waves)
 constexpr int CL_T = 512;          // threads per CTA
 constexpr int CL_MAXC = 17600;     // columns of a problem (= the single-CTA kernel's shared-memory limit)
 constexpr int CL_NMIN = 5;         // smallest cluster the shared-memory budget allows (3520 columns per CTA)

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libptb_b200.so.
+// Shared helpers for the sm_90a kernels of libptb_b200.so.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,7 +44,7 @@ inline int check_launch(const char* what) {
 // concurrent launches on different streams (round 1 kept them in file-scope __device__ globals).  Allocated lazily
 // (cudaMalloc + memset, once per stream) by capi.cu; ptb_reset_stream_state() zeroes it after an aborted launch.
 // ---------------------------------------------------------------------------------------------
-constexpr int SCRATCH_BLOCKS = 592;      // 4 x 148: grid of the fixed-order sum kernels
+constexpr int SCRATCH_BLOCKS = 528;      // 4 x 132 (H100 SMs): grid of the fixed-order sum kernels
 struct SumScratch {
   float partials[SCRATCH_BLOCKS];
   unsigned int done;
@@ -60,10 +60,10 @@ StreamScratch* stream_scratch(void* stream);     // NULL on failure (g_err set)
 inline int sm_count() {       // of the CURRENT device (cached per device: a process may drive several)
   static int n[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;  // B200
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;  // H100 SXM
   if (n[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     n[dev] = v;
   }
   return n[dev];
@@ -107,16 +107,14 @@ __device__ __forceinline__ Taps make_taps(float px, float py, float stride, int 
 }
 
 // bilinear combination of four 128-bit taps in ATen's operation order (nw*w + ne*w + sw*w + se*w as an FMA chain, bit-exact vs the
-// CPU grid_sample kernel) on packed fp32 pairs: FMUL2 / FFMA2 (sm_100) round every element exactly like FMUL / FFMA and halve
-// the instruction count of the hot loops (gather, fused refine: both issue / MIO limited, not FMA-pipe limited).
+// CPU grid_sample kernel).  __f*_rn intrinsics are never contracted or reassociated, so every element rounds exactly as ATen's does.
+__device__ __forceinline__ float bilerp1(float q0, float q1, float q2, float q3, float w00, float w01, float w10, float w11) {
+  return __fmaf_rn(q3, w11, __fmaf_rn(q2, w10, __fmaf_rn(q1, w01, __fmul_rn(q0, w00))));
+}
 __device__ __forceinline__ float4 bilerp4(const float4 q0, const float4 q1, const float4 q2, const float4 q3, float w00, float w01,
                                           float w10, float w11) {
-  const float2 a = make_float2(w00, w00), b = make_float2(w01, w01), c = make_float2(w10, w10), d = make_float2(w11, w11);
-  const float2 lo = __ffma2_rn(make_float2(q3.x, q3.y), d, __ffma2_rn(make_float2(q2.x, q2.y), c,
-                    __ffma2_rn(make_float2(q1.x, q1.y), b, __fmul2_rn(make_float2(q0.x, q0.y), a))));
-  const float2 hi = __ffma2_rn(make_float2(q3.z, q3.w), d, __ffma2_rn(make_float2(q2.z, q2.w), c,
-                    __ffma2_rn(make_float2(q1.z, q1.w), b, __fmul2_rn(make_float2(q0.z, q0.w), a))));
-  return make_float4(lo.x, lo.y, hi.x, hi.y);
+  return make_float4(bilerp1(q0.x, q1.x, q2.x, q3.x, w00, w01, w10, w11), bilerp1(q0.y, q1.y, q2.y, q3.y, w00, w01, w10, w11),
+                     bilerp1(q0.z, q1.z, q2.z, q3.z, w00, w01, w10, w11), bilerp1(q0.w, q1.w, q2.w, q3.w, w00, w01, w10, w11));
 }
 
 // torch.cdist(p=2) as ATen computes it.

@@ -240,9 +240,8 @@ struct RfTile {           // where the taps of this CTA live
 
 // class phase for the 32 samples a warp owns: returns (to the owner lane) max logit, max logit over classes < l, logit of class l.
 // NT = float4 class groups per lane (ceil(ceil(ncls/4) / 8)); requires ncls % 4 == 0 and (NT-1)*8 < cg4 (only the LAST trip is partial).
-// Shape of the code after two ncu passes (r02 v1: 56 SASS instructions per trip from per-trip branches; v2: 260 per round from
-// predicated -inf initialisation and select chains): trips 0..NT-2 are unconditional (all tap loads first, then the FMA chains), the
-// last trip sits under one branch, and the label's own group is loaded a second time as a broadcast (4 LDS + 8 FFMA2) instead of being
+// Shape of the code (per-trip branches and predicated -inf initialisation / select chains cost many SASS instructions per trip): trips 0..NT-2 are unconditional (all tap loads first, then the FMA chains), the
+// last trip sits under one branch, and the label's own group is loaded a second time as a broadcast (4 LDS + 16 FFMA) instead of being
 // picked out of the trips with selects.
 template <bool STAGED, int NT>
 __device__ __forceinline__ void rf_class_phase(const RfTile& tl, float ix, float iy, int H, int W, int ld, int cg4, int l4, int lq,

@@ -225,7 +225,7 @@ rpn_nms_level_kernel(const float4* __restrict__ cand_box, const float* __restric
 //   * the sorted, level-offset boxes go to shared memory (SoA),
 //   * every thread fills words of the suppression matrix  M[i][w] bit j = IoU(box_i, box_{64w+j}) > thr  for 64w+j > i  — n^2/2
 //     independent IoU tests spread over the CTA (the serial kernel above ran them on ONE warp, kept-list against candidates:
-//     3.55 ms per launch in ncu, the whole RPN path's critical kernel),
+//     the whole RPN path's critical kernel),
 //   * one warp walks the candidates in order: lane w holds word w of the "removed" set, the next survivor is a find-first-set on
 //     the current word, keeping it ORs its row of M into the set.  ~50 cycles per KEPT box instead of an IoU sweep per candidate.
 // The greedy order and the IoU predicate (argument order: earlier box first) are those of the serial kernel: identical keep lists.

@@ -1,5 +1,5 @@
 // Backward of the tower's GroupNorm + ReLU (mmcv ConvModule order conv -> GN -> ReLU; cpr_head.py:983-995, p2p_head.py:82-102) on the
-// channels-last layout of the tcgen05 convolution:  a = relu(z), z = gamma * yhat + beta, yhat = (y - mean) * rstd per (image, group).
+// channels-last layout of the tensor-core convolution:  a = relu(z), z = gamma * yhat + beta, yhat = (y - mean) * rstd per (image, group).
 //   dz        = da * [z > 0]
 //   dgamma_c  = sum_{b,p} dz * yhat,   dbeta_c = sum_{b,p} dz
 //   dy        = rstd * (gamma * dz - (s1 + yhat * s2) / n),   s1 = sum_{c in g, p} gamma * dz,  s2 = sum gamma * dz * yhat,  n = HW * C/groups
@@ -91,7 +91,7 @@ gn_bwd_finalize_kernel(const float* __restrict__ partial, const double* __restri
   const int cpg = C / groups;
   const double inv_n = 1.0 / ((double)HW * cpg);
   // 1024 / C threads share a channel (chunk k goes to part k % nparts): the loop over chunks is a chain of dependent-latency loads,
-  // with one thread per channel it cost 20 us per launch (ncu) for a few KB of data
+  // with one thread per channel that chain, not the few KB of data, set the launch time
   const int nparts = 1024 / C;                       // >= 1 (C <= 1024)
   const int c = threadIdx.x % C, part = threadIdx.x / C;
   double r1 = 0.0, r2 = 0.0;

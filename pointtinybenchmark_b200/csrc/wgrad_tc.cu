@@ -1,27 +1,23 @@
-// Weight gradient of the tower's conv3x3 (256 -> 256, stride 1, pad 1) on the 5th-gen tensor cores, fp32-accurate:
+// Weight gradient of the tower's conv3x3 (256 -> 256, stride 1, pad 1) on the Hopper tensor cores (wgmma), fp32-accurate:
 //     dW[co][ci][kh][kw] = sum_{b,h,w} dy[b][h][w][co] * x[b][h+kh-1][w+kw-1][ci]          (autograd of cpr_head.py:1033-1043's convs)
 // A GEMM with M = co, N = ci and K = PIXELS: both operands are channels-last activations, i.e. their contiguous dimension is
-// M / N, not K.  tcgen05 reads such "MN-major" operands directly (instruction-descriptor bits 15/16, canonical layout
-// ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units for SWIZZLE_128B, cute/atom/mma_traits_sm100.hpp), so no transpose pass:
+// M / N, not K.  wgmma reads such "MN-major" fp16 operands directly (the transpose immediates of wgmma.mma_async; canonical layout
+// of 64-element x 8-deep SWIZZLE_128B atoms), so no transpose pass:
 //   * a 4-D TMA box {64 channels, 16 w, 2 h, 1 image} of fp16 lands in shared memory as 32 pixel rows of 128 B with the
 //     SWIZZLE_128B XOR — exactly one MN-major atom column (64 channels) x 4 K-atoms (8 pixels each, SBO = 1024 B);
-//     co 0..127 = 2 such boxes (LBO = 4096 B), ci 0..255 = 4 boxes.  The x box is fetched at the tap-shifted origin; its
-//     out-of-bounds part (the conv's zero padding, partial edge tiles) is zero-filled by the TMA unit, and dy's out-of-image
-//     rows are zero too, so edge tiles need no masks.
+//     128 channels = 2 such boxes (LBO = 4096 B).  The x box is fetched at the tap-shifted origin; its out-of-bounds part (the
+//     conv's zero padding, partial edge tiles) is zero-filled by the TMA unit, and dy's out-of-image rows are zero too, so edge
+//     tiles need no masks.
 //   * fp32 accuracy as in conv_tc.cu: dy*s1 = h + l and x*s2 = h + l as fp16 pairs, h*h -> main accumulator, l*h + h*l ->
-//     correction accumulator (512 TMEM columns), summed in fp32 in the epilogue.
-//   * the tensor core adds into the fp32 accumulator with truncation (~0.5 ulp of the accumulator per step, see conv_tc.cu);
-//     over the 1100 accumulation steps of a pixel split that is a 3e-4 error on dW (measured vs fp64 at the headline shape).
-//     The main accumulator is therefore FLUSHED every WG_FLUSH pixel blocks: the epilogue warps store it as one more fp32
-//     partial (store-only: a read-modify-write of the previous partial cost 25 us per flush, ncu; re-measured in round 2 with
-//     L2-resident ld.cg/st.cg: +47 us on the kernel for -40 us on the reduction, no gain) and the MMA warp restarts it
-//     from zero; the correction accumulator is 2^-11 smaller and runs through.  The reduction kernel adds runs and splits with
-//     round-to-nearest fp32 adds in a fixed order.
-//   * work: 2 co-halves x 9 taps x S pixel splits = 18*S CTAs (S = 8 -> 144 of 148 SMs), the two co halves being the two CTAs of a
-//     tcgen05 cta_group::2 pair (see the kernel); a CTA streams its pixel blocks through a 6 x 32 KB mbarrier ring (4 x 48 KB in the
-//     single-CTA debug mode PTB_WGRAD_PAIR=0; warp 0 TMA producer, warp 1 MMA issuer, warps 2-5 epilogue) and writes
-//     128 x 256 fp32 partials; `wgrad_reduce_kernel` adds the S partials in a fixed order, applies the (power-of-two) inverse
-//     operand scales and writes OIHW.  Deterministic.
+//     correction accumulator, summed in fp32 at the end.
+//   * the tensor core adds into the fp32 accumulator without round-to-nearest (see conv_tc.cu); over the thousands of accumulation
+//     steps of a pixel split that would be a visible error on dW.  The main accumulator is therefore FLUSHED every WG_FLUSH pixel
+//     blocks: the MMA warpgroups store it as one more fp32 partial and restart it from zero; the correction accumulator is 2^-11
+//     smaller and runs through.  The reduction kernel adds runs and splits with round-to-nearest fp32 adds in a fixed order.
+//   * work: 2 co halves x 2 ci halves x 9 taps x S pixel splits = 36*S CTAs (S chosen so the CTAs fill whole waves of the SMs);
+//     a CTA streams its pixel blocks through a 6 x 32 KB mbarrier ring (warpgroup 0: TMA producer, warpgroups 1 and 2: 64 output
+//     channels each, two 64 x 128 fp32 accumulators in registers) and writes 128 x 128 fp32 partials; `wgrad_reduce_kernel` adds
+//     the partials in a fixed order, applies the (power-of-two) inverse operand scales and writes OIHW.  Deterministic.
 #include "tc_ptx.cuh"
 #include <stdlib.h>
 
@@ -29,40 +25,18 @@ namespace ptb {
 
 constexpr int WG_PX = 32;                         // pixels per K-block: box {64 ch, 16 w, 2 h}
 constexpr int WG_TW = 16, WG_TH = 2;
-constexpr int WG_STAGES = 4;
+constexpr int WG_STAGES = 6;
 constexpr uint32_t WG_BOX_BYTES = WG_PX * 128;    // 4 KB: 32 pixel rows x 64 fp16 channels
-constexpr uint32_t WG_A_BYTES = 2 * WG_BOX_BYTES; // 128 co
-constexpr uint32_t WG_B_BYTES = 4 * WG_BOX_BYTES; // 256 ci
-constexpr uint32_t WG_STAGE_BYTES = 2 * WG_A_BYTES + 2 * WG_B_BYTES;   // 48 KB
-constexpr int WG_STAGES_PAIR = 6;                 // CTA-pair mode stages only half of the x tile: 6 x 32 KB
-constexpr uint32_t WG_STAGE_BYTES_PAIR = 2 * WG_A_BYTES + WG_B_BYTES;  // 32 KB
-constexpr uint32_t WG_RING_BYTES = WG_STAGES * WG_STAGE_BYTES;          // = WG_STAGES_PAIR * WG_STAGE_BYTES_PAIR = 192 KB
-static_assert(WG_STAGES_PAIR * WG_STAGE_BYTES_PAIR == WG_RING_BYTES, "both modes share one ring size");
-constexpr uint32_t WG_SMEM_BYTES = WG_RING_BYTES + 1024 + 256;
-constexpr int WG_THREADS = 192;
+constexpr uint32_t WG_OP_BYTES = 2 * WG_BOX_BYTES;  // 128 channels of one operand half (hi or lo)
+constexpr uint32_t WG_STAGE_BYTES = 4 * WG_OP_BYTES;  // dy hi, dy lo, x hi, x lo: 32 KB
+constexpr uint32_t WG_SMEM_BYTES = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
+constexpr int WG_THREADS = 384;
 constexpr int WG_C = 256;                         // Cout = Cin = 256
 constexpr int WG_FLUSH = 128;                     // pixel blocks (256 accumulation steps) between two flushes of the main accumulator
 
-// MN-major, SWIZZLE_128B shared-memory matrix descriptor: atoms of 64 elements (128 B) x 8 K-rows = 1024 B;
-// LBO = byte distance between atoms along M/N, SBO = byte distance between atoms along K.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo >> 4) << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;                          // version = 1 (sm_100)
-  d |= (uint64_t)2 << 61;                          // SWIZZLE_128B
-  return d;
-}
-// kind::f16, fp16 operands, fp32 accumulate, A and B MN-major, M = 128, N = 256
-__host__ __device__ constexpr uint32_t umma_idesc_f16_mn_m128_n256() {
-  return (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
 // Accumulation runs of a pixel split: the FIRST run of split s is shortened to WG_FLUSH * (s + 1) / splits blocks, later runs have WG_FLUSH
-// blocks.  All CTAs stream at the same pace, so equal runs made all 144 of them flush their 128 KB accumulators in the same few
-// microseconds (an 18.9 MB store burst at the DRAM write rate, ~7 us with every tensor pipe idle, five times per launch); staggered, the
-// splits flush 1/8 of a run apart and the stores of one hide behind the MMAs of the others.
+// blocks.  All CTAs stream at the same pace, so equal runs would make them all flush their accumulators in the same few microseconds;
+// staggered, the splits flush 1/splits of a run apart and the stores of one hide behind the MMAs of the others.
 __host__ __device__ inline int wg_first_run(int split, int splits) {
   const int f = (int)(((long long)WG_FLUSH * (split + 1)) / splits);
   return f < 1 ? 1 : f;
@@ -81,75 +55,40 @@ struct WgradShape {
   int Cout;                          // rows of dW actually wanted (<= 256); rows beyond it are the TMA unit's zero fill of dy
 };
 
-// PAIR = true (round 2, default): the two co halves of a (tap, pixel split) form a CTA pair issuing ONE tcgen05.mma.cta_group::2 per
-// product (M = 256 = all output channels): each CTA stages its own dy half and only HALF of the x tile (128 input channels), i.e. 32 KB
-// instead of 48 KB per pixel block — the single-CTA kernel pulled its operands at the L2 -> SM ceiling (144 CTAs x 48 KB per 768 tensor
-// cycles = 11.5 TB/s; ncu: tensor pipe 45 %).  Protocol as in conv_tc.cu: the leader's "full" barrier collects both CTAs' TMA bytes,
-// tcgen05.commit.cta_group::2 multicasts "stage free" / "run complete", the peer's epilogue warps release TMEM with remote arrives.
-template <bool PAIR>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_dyh, const __grid_constant__ CUtensorMap tm_dyl,
                 const __grid_constant__ CUtensorMap tm_xh, const __grid_constant__ CUtensorMap tm_xl, WgradShape ws,
                 float* __restrict__ partial /*[splits][max_runs][taps][256 co][256 ci]*/) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  constexpr int NST = PAIR ? WG_STAGES_PAIR : WG_STAGES;
-  constexpr uint32_t STB = PAIR ? WG_STAGE_BYTES_PAIR : WG_STAGE_BYTES;
-  constexpr uint32_t BLO = PAIR ? WG_B_BYTES / 2 : WG_B_BYTES;      // offset of the x "lo" half behind the x "hi" half
-  const uint32_t bar_base = smem_base + WG_RING_BYTES;
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B atoms need 1024 B alignment
+  const uint32_t bar_base = smem_base + WG_STAGES * WG_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
-  const uint32_t tfull_bar = bar_base + 128u;
-  const uint32_t tempty_bar = bar_base + 136u;
-  const uint32_t tmem_slot = bar_base + 160u;
-  uint8_t* smem_aligned = smem_raw + (smem_base - smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_aligned + WG_RING_BYTES + 160);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // unit = (split, tap, co half)
+  const int wg = threadIdx.x >> 7;
+  // unit = (split, tap, ci half, co half)
   const int unit = blockIdx.x;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;          // PAIR: cluster = (unit 2u, 2u+1) = the two co halves; rank == m_half
-  const int m_half = unit & 1;
-  const int tap = (unit >> 1) % ws.taps;
-  const int split = unit / (2 * ws.taps);
+  const int m_half = unit & 1, n_half = (unit >> 1) & 1;
+  const int tap = (unit >> 2) % ws.taps;
+  const int split = unit / (4 * ws.taps);
   const int kh = ws.taps == 9 ? tap / 3 : 1, kw = ws.taps == 9 ? tap - (tap / 3) * 3 : 1;
   const int blk0 = (int)(((long long)ws.n_blocks * split) / ws.splits);
   const int blk1 = (int)(((long long)ws.n_blocks * (split + 1)) / ws.splits);
   const int n_my = blk1 - blk0;
-  const int first_run = wg_first_run(split, ws.splits);
-  const int n_flush = wg_runs(n_my, first_run);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NST; ++s) {
+    for (int s = 0; s < WG_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);                    // one arrive per MMA warp
     }
-    mbar_init(tfull_bar, 1);
-    mbar_init(tempty_bar, PAIR ? 8 : 4); // one arrive per epilogue warp (PAIR: of both CTAs, on the leader's barrier)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if (PAIR) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // =============================== TMA producer ===============================
-    // The WHOLE warp walks the block list with warp-uniform coordinates (advanced incrementally: no division per block) and lane 0
-    // issues: with the loop inside an `if (lane == 0)` the compiler cannot prove the operands uniform and wraps every UTMALDG in an
-    // ELECT / R2UR waterfall — ncu's source page showed this single thread ISSUE-bound (~1100 cycles per 32 KB stage, the MMA warp
-    // starving at 50 % tensor-pipe activity).
-    {
+    regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int per_img = ws.tiles_h * ws.tiles_w;
@@ -157,140 +96,78 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_dyh, const __grid_constan
       int th = (blk0 - b * per_img) / ws.tiles_w;
       int tw = (blk0 - b * per_img) - th * ws.tiles_w;
       for (int blk = blk0; blk < blk1; ++blk) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);               // all lanes wait (measured faster than lane 0 alone waiting inside the branch)
-        // shfl-broadcasts: the values are uniform anyway, this is what lets ptxas SEE it (uniform registers feed UTMALDG directly)
-        const int ust = __shfl_sync(0xffffffffu, stage, 0);
-        const int h0 = __shfl_sync(0xffffffffu, th, 0) * WG_TH, w0 = __shfl_sync(0xffffffffu, tw, 0) * WG_TW;
-        const int ub = __shfl_sync(0xffffffffu, b, 0);
-        const uint32_t sA_h = smem_base + ust * STB;
-        const uint32_t sA_l = sA_h + WG_A_BYTES;
-        const uint32_t sB_h = sA_l + WG_A_BYTES;
-        const uint32_t sB_l = sB_h + BLO;
-        if (PAIR) {
-          // my dy half (128 co) + MY half of the x tile (128 ci); every byte is counted on the LEADER's barrier
-          const uint32_t lead_full = mapa_rank(full_bar(ust), 0u);
-          if (lane == 0) {
-            if (rank == 0) mbar_expect_tx(full_bar(ust), 2u * (2 * WG_A_BYTES + WG_B_BYTES));
+        mbar_wait(empty_bar(stage), phase ^ 1u);
+        const int h0 = th * WG_TH, w0 = tw * WG_TW;
+        const uint32_t sA_h = smem_base + stage * WG_STAGE_BYTES;
+        const uint32_t sA_l = sA_h + WG_OP_BYTES;
+        const uint32_t sB_h = sA_l + WG_OP_BYTES;
+        const uint32_t sB_l = sB_h + WG_OP_BYTES;
+        mbar_expect_tx(full_bar(stage), WG_STAGE_BYTES);
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              tma_load_4d_pair(&tm_dyh, lead_full, sA_h + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, ub);
-              tma_load_4d_pair(&tm_dyl, lead_full, sA_l + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, ub);
-            }
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              tma_load_4d_pair(&tm_xh, lead_full, sB_h + j * WG_BOX_BYTES, 64 * (2 * (int)rank + j), w0 + kw - 1, h0 + kh - 1, ub);
-              tma_load_4d_pair(&tm_xl, lead_full, sB_l + j * WG_BOX_BYTES, 64 * (2 * (int)rank + j), w0 + kw - 1, h0 + kh - 1, ub);
-            }
-          }
-        } else if (lane == 0) {
-          mbar_expect_tx(full_bar(ust), WG_STAGE_BYTES);
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            tma_load_4d(&tm_dyh, full_bar(ust), sA_h + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, ub);
-            tma_load_4d(&tm_dyl, full_bar(ust), sA_l + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, ub);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            tma_load_4d(&tm_xh, full_bar(ust), sB_h + j * WG_BOX_BYTES, 64 * j, w0 + kw - 1, h0 + kh - 1, ub);
-            tma_load_4d(&tm_xl, full_bar(ust), sB_l + j * WG_BOX_BYTES, 64 * j, w0 + kw - 1, h0 + kh - 1, ub);
-          }
+        for (int i = 0; i < 2; ++i) {
+          tma_load_4d(&tm_dyh, full_bar(stage), sA_h + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, b);
+          tma_load_4d(&tm_dyl, full_bar(stage), sA_l + i * WG_BOX_BYTES, m_half * 128 + 64 * i, w0, h0, b);
+          tma_load_4d(&tm_xh, full_bar(stage), sB_h + i * WG_BOX_BYTES, n_half * 128 + 64 * i, w0 + kw - 1, h0 + kh - 1, b);
+          tma_load_4d(&tm_xl, full_bar(stage), sB_l + i * WG_BOX_BYTES, n_half * 128 + 64 * i, w0 + kw - 1, h0 + kh - 1, b);
         }
-        __syncwarp();
-        if (++stage == NST) { stage = 0; phase ^= 1u; }
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1u; }
         if (++tw == ws.tiles_w) { tw = 0; if (++th == ws.tiles_h) { th = 0; ++b; } }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (lane == 0 && n_my > 0 && (!PAIR || rank == 0)) {
-      const uint32_t idesc = PAIR ? ((umma_idesc_f16_mn_m128_n256() & ~(0x1Fu << 24)) | ((uint32_t)(256 >> 4) << 24))
-                                  : umma_idesc_f16_mn_m128_n256();
-      const uint32_t d_main = tmem_base, d_corr = tmem_base + 256u;
-      int stage = 0;
-      uint32_t phase = 0;
-      int in_run = 0, run_len = first_run, run_idx = 0;        // position inside / length / index of the current accumulation run
-      for (int it = 0; it < n_my; ++it) {
-        if (in_run == 0 && it > 0) {                           // the epilogue has stored the previous run
-          mbar_wait(tempty_bar, (uint32_t)((run_idx - 1) & 1));
-          tc_fence_after();
-        }
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t sA_h = smem_base + stage * STB;
-        const uint32_t sA_l = sA_h + WG_A_BYTES;
-        const uint32_t sB_h = sA_l + WG_A_BYTES;
-        const uint32_t sB_l = sB_h + BLO;
-#pragma unroll
-        for (int k = 0; k < WG_PX / 16; ++k) {                 // UMMA_K = 16 pixels = two 8-row atoms = 2048 B
-          const uint64_t a_h = umma_desc_mn_sw128(sA_h + 2048u * k, WG_BOX_BYTES, 1024u);
-          const uint64_t a_l = umma_desc_mn_sw128(sA_l + 2048u * k, WG_BOX_BYTES, 1024u);
-          const uint64_t b_h = umma_desc_mn_sw128(sB_h + 2048u * k, WG_BOX_BYTES, 1024u);
-          const uint64_t b_l = umma_desc_mn_sw128(sB_l + 2048u * k, WG_BOX_BYTES, 1024u);
-          if (PAIR) {
-            umma_ss_pair<true>(d_main, a_h, b_h, idesc, (in_run | k) != 0);
-            umma_ss_pair<true>(d_corr, a_l, b_h, idesc, (it | k) != 0);
-            umma_ss_pair<true>(d_corr, a_h, b_l, idesc, 1u);
-          } else {
-            umma_ss<true>(d_main, a_h, b_h, idesc, (in_run | k) != 0);
-            umma_ss<true>(d_corr, a_l, b_h, idesc, (it | k) != 0);
-            umma_ss<true>(d_corr, a_h, b_l, idesc, 1u);
-          }
-        }
-        if (PAIR) umma_commit_pair(empty_bar(stage), (uint16_t)0x3);
-        else umma_commit(empty_bar(stage));
-        if (++stage == NST) { stage = 0; phase ^= 1u; }
-        if (in_run == run_len - 1 || it == n_my - 1) {                              // run complete: hand it to the epilogue(s)
-          if (PAIR) umma_commit_pair(tfull_bar, (uint16_t)0x3);
-          else umma_commit(tfull_bar);
-          in_run = 0; run_len = WG_FLUSH; ++run_idx;
-        } else {
-          ++in_run;
-        }
-      }
-    }
   } else {
-    // =============================== epilogue (warps 2..5) ===============================
-    const int q = warp & 3;                                    // TMEM lane quarter this warp may access
-    const int co = m_half * 128 + q * 32 + lane;
-    float* out0 = partial + ((((size_t)split * ws.max_runs) * ws.taps + tap) * WG_C + co) * WG_C;       // run r: + r * taps*256*256
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    for (int f = 0; f < n_flush; ++f) {
-      mbar_wait(tfull_bar, (uint32_t)(f & 1));
-      tc_fence_after();
-      const bool last = f == n_flush - 1;
-      float* out = out0 + (size_t)f * ws.taps * WG_C * WG_C;
-#pragma unroll 1
-      for (int c = 0; c < WG_C / 32; ++c) {
-        uint32_t v[32], vc[32];
-        tmem_ld32_nowait(t_lane + (uint32_t)(c * 32), v);
-        if (last) tmem_ld32_nowait(t_lane + 256u + (uint32_t)(c * 32), vc);
-        tmem_ld_wait();
+    // =============================== MMA + flushes (warpgroups 1, 2) ===============================
+    regs_alloc<232>();
+    const int cw = wg - 1;                                   // output channels m_half * 128 + 64 cw .. + 63
+    const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+    float acc[64], cor[64];
+    int stage = 0;
+    uint32_t phase = 0;
+    const int co = m_half * 128 + cw * 64 + warp * 16 + (lane >> 2);
+    const int ci = n_half * 128 + 2 * (lane & 3);
+    int it = 0;
+    for (int run = 0; it < n_my; ++run) {
+      const int run_len = min(run == 0 ? wg_first_run(split, ws.splits) : WG_FLUSH, n_my - it);
+      int prev = 0;
+      for (int r = 0; r < run_len; ++r, ++it) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t sA_h = smem_base + stage * WG_STAGE_BYTES + (uint32_t)cw * WG_BOX_BYTES;
+        const uint32_t sA_l = sA_h + WG_OP_BYTES;
+        const uint32_t sB_h = smem_base + stage * WG_STAGE_BYTES + 2 * WG_OP_BYTES;
+        const uint32_t sB_l = sB_h + WG_OP_BYTES;
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                 __uint_as_float(v[4 * j + 3]));
-          if (last) {
-            o.x = __fadd_rn(o.x, __uint_as_float(vc[4 * j]));     o.y = __fadd_rn(o.y, __uint_as_float(vc[4 * j + 1]));
-            o.z = __fadd_rn(o.z, __uint_as_float(vc[4 * j + 2])); o.w = __fadd_rn(o.w, __uint_as_float(vc[4 * j + 3]));
-          }
-          __stcg(reinterpret_cast<float4*>(out + c * 32 + 4 * j), o);      // L2-resident: all CTAs flush at once (18.9 MB burst), the reduction re-reads it
+        for (int k = 0; k < WG_PX / 16; ++k) {               // 16 pixels per MMA = two 8-deep atoms = 2048 B
+          const uint64_t a_h = gmma_desc(sA_h + 2048u * k, WG_BOX_BYTES, 1024u, GMMA_SW128);
+          const uint64_t a_l = gmma_desc(sA_l + 2048u * k, WG_BOX_BYTES, 1024u, GMMA_SW128);
+          const uint64_t b_h = gmma_desc(sB_h + 2048u * k, WG_BOX_BYTES, 1024u, GMMA_SW128);
+          const uint64_t b_l = gmma_desc(sB_l + 2048u * k, WG_BOX_BYTES, 1024u, GMMA_SW128);
+          wgmma_f16<1, 1>(acc, a_h, b_h, (r | k) != 0);
+          wgmma_f16<1, 1>(cor, a_l, b_h, (it | k) != 0);
+          wgmma_f16<1, 1>(cor, a_h, b_l, 1u);
+        }
+        wgmma_commit();
+        if (r > 0) {                                         // the previous block's MMAs have read their stage: hand it back
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(empty_bar(prev));
+        }
+        prev = stage;
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      // run complete: store it as one partial (the last run adds the correction accumulator)
+      const bool last = it == n_my;
+      float* out = partial + ((((size_t)split * ws.max_runs + run) * ws.taps + tap) * WG_C + co) * WG_C + ci;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          float2 o = make_float2(acc[4 * i + 2 * j], acc[4 * i + 2 * j + 1]);
+          if (last) { o.x = __fadd_rn(o.x, cor[4 * i + 2 * j]); o.y = __fadd_rn(o.y, cor[4 * i + 2 * j + 1]); }
+          __stcg(reinterpret_cast<float2*>(out + (size_t)8 * j * WG_C + 8 * i), o);     // L2-resident: the reduction re-reads it
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (PAIR) mbar_arrive_cluster(mapa_rank(tempty_bar, 0u));
-        else mbar_arrive(tempty_bar);
-      }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (PAIR) cluster_sync_all();          // no CTA exits while the peer can still arrive on its barriers / read its operands
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
   }
 }
 
@@ -359,11 +236,15 @@ static int make_px_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, in
 
 using namespace ptb;
 
+// pixel splits: 4 * taps * S CTAs of one block each per SM; S is picked for the least wave-quantised time ceil(CTAs / SMs) / S
 static int wgrad_splits(int taps) {
-  int s = sm_count() / (2 * taps);
-  if (s < 1) s = 1;
-  if (s > 96) s = 96;
-  return s;
+  const int sms = sm_count(), units = 4 * taps;
+  int s_max = 4 * (sms / units > 1 ? sms / units : 1);
+  if (s_max > 96) s_max = 96;
+  int best = 1;
+  for (int s = 2; s <= s_max; ++s)
+    if ((long long)((units * s + sms - 1) / sms) * best < (long long)((units * best + sms - 1) / sms) * s) best = s;
+  return best;
 }
 
 static int wgrad_max_runs(int n_blocks, int splits) {
@@ -399,29 +280,11 @@ static int wgrad_run(const void* dy_h, const void* dy_l, const void* x_h, const 
   ws.max_runs = wgrad_max_runs(ws.n_blocks, ws.splits);
   ws.taps = taps; ws.Cout = Cout;
   // per-device function attribute: set on every call (a process may drive several devices)
-  if (cudaFuncSetAttribute(wgrad_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(wgrad_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES) != cudaSuccess)
+  if (cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES) != cudaSuccess)
     return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the wgrad kernel");
   cudaStream_t st = (cudaStream_t)stream;
   // CTAs of the upper co half have nothing to do when Cout <= 128: they still run (zero operands) to keep the unit decomposition uniform
-  const char* e_pair = getenv("PTB_WGRAD_PAIR");
-  if (e_pair && e_pair[0] == '0') {
-    wgrad_tc_kernel<false><<<2 * taps * ws.splits, WG_THREADS, WG_SMEM_BYTES, st>>>(tm_dyh, tm_dyl, tm_xh, tm_xl, ws,
-                                                                                   reinterpret_cast<float*>(workspace));
-  } else {      // CTA pairs: units (2u, 2u+1) = the two co halves of one (tap, split)
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * taps * ws.splits);
-    cfg.blockDim = dim3(WG_THREADS);
-    cfg.dynamicSmemBytes = WG_SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, wgrad_tc_kernel<true>, tm_dyh, tm_dyl, tm_xh, tm_xl, ws, reinterpret_cast<float*>(workspace));
-    if (e != cudaSuccess) return fail("wgrad: cluster launch failed: %s", cudaGetErrorString(e));
-  }
+  wgrad_tc_kernel<<<4 * taps * ws.splits, WG_THREADS, WG_SMEM_BYTES, st>>>(tm_dyh, tm_dyl, tm_xh, tm_xl, ws, reinterpret_cast<float*>(workspace));
   if ((rc = check_launch(what))) return rc;
   const int n = taps * WG_C * WG_C;
   wgrad_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const float*>(workspace), ws, scale, dev_scale_dy,
@@ -455,13 +318,13 @@ extern "C" int ptb_conv_tc_wgrad_f16x2(const void* dy_h, const void* dy_l, const
 
 extern "C" uint64_t ptb_col_sum_workspace(int64_t M, int N) {
   if (M <= 0 || N <= 0) return 0;
-  return (uint64_t)148 * 4 * N * sizeof(float);
+  return (uint64_t)SCRATCH_BLOCKS * N * sizeof(float);
 }
 
 extern "C" int ptb_col_sum(const float* y, int64_t M, int N, int ld, float* workspace, float* out, void* stream) {
   PTB_REQUIRE(M > 0 && N > 0 && ld >= N, "shape");
   PTB_REQUIRE(y && workspace && out, "NULL input");
-  int slices = 148 * 4;
+  int slices = SCRATCH_BLOCKS;
   if ((int64_t)slices > M) slices = (int)M;
   const int rps = (int)((M + slices - 1) / slices);
   slices = (int)((M + rps - 1) / rps);

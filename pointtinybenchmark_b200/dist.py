@@ -53,10 +53,10 @@ class GradBucket:
     The bucketed / hooked exchange is opt-in (overlap=True); the default is one all-reduce of the flat buffer (see __init__)."""
 
     def __init__(self, module, group=None, average=True, buckets=None, overlap=False):
-        # overlap=False (default): ONE all-reduce of the whole flat buffer, issued by wait() — measured on 2 x B200: the head's 9.6 MB take
-        # 0.05 ms on NVLink, less than the host time the per-bucket hooks add to a backward pass that is partly launch-bound
-        # (8.70 vs 9.30 ms per step).  overlap=True: per-bucket all-reduces from post-accumulate hooks on a side stream, for heads /
-        # links where the exchange is long enough to be worth hiding.
+        # overlap=False (default): ONE all-reduce of the whole flat buffer (the head's 9.6 MB), issued by wait(): on an NVLink-connected
+        # node that exchange is short, and per-bucket hooks add host work to a backward pass that is partly launch-bound.  overlap=True:
+        # per-bucket all-reduces from post-accumulate hooks on a side stream, for heads / links where the exchange is long enough to be
+        # worth hiding.
         self.group, self.average, self.overlap = group, average, overlap
         params = [(n, p) for n, p in module.named_parameters() if p.requires_grad]
         if buckets is None:

@@ -1,9 +1,9 @@
 """Host-side layer containers with the reference's parameter names (checkpoint compatibility, SURVEY.md §5).
 
-Conv towers (SURVEY.md §8f rank 1): at inference they run on the hand-written tcgen05 implicit-GEMM kernel of csrc/conv_tc.cu
+Conv towers (SURVEY.md §8f rank 1): at inference they run on the hand-written wgmma implicit-GEMM kernel of csrc/conv_tc.cu
 (fp16 two-term split by default, 3xTF32 with PTB_CONV_MODE=tf32x3; both fp32-accurate); under autograd (training) the shipped
 256 -> 256 geometry runs `_TowerTCFn`: the same forward kernel plus hand-written GroupNorm/ReLU backward, dgrad (the forward
-kernel on transposed, flipped weights) and a tcgen05 wgrad with MN-major operands.  Other geometries (or PTB_TOWER_TRAIN=cudnn)
+kernel on transposed, flipped weights) and a wgmma wgrad with MN-major operands.  Other geometries (or PTB_TOWER_TRAIN=cudnn)
 use cuDNN fp32 through torch with TF32 switched off locally (library path).
 """
 import math
@@ -81,7 +81,7 @@ class PackedWeightsMixin:
 
 
 def _tc_supported(convs, x):
-    """the tcgen05 path covers the shipped head geometry: conv3x3 s1 p1 without bias -> 256 channels, GroupNorm with
+    """the wgmma path covers the shipped head geometry: conv3x3 s1 p1 without bias -> 256 channels, GroupNorm with
     channels-per-group % 4 == 0, Cin % 32 == 0, fp32 CUDA input, inference (no autograd graph)."""
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in convs for p in m.parameters())):
         return False
@@ -224,7 +224,7 @@ class _TowerTCFn(torch.autograd.Function):
 
 
 def tower(convs, x, info=None, want='fp32'):
-    """4 x [conv3x3 + GN + ReLU].  Inference: hand-written tcgen05 implicit GEMM (fp16 two-term split or 3xTF32) with GroupNorm
+    """4 x [conv3x3 + GN + ReLU].  Inference: hand-written wgmma implicit GEMM (fp16 two-term split or 3xTF32) with GroupNorm
     statistics in the epilogue (csrc/conv_tc.cu).  Training (autograd): _TowerTCFn for the shipped 256 -> 256 geometry (same forward
     kernel + hand-written backward), else cuDNN fp32 through torch."""
     import os
@@ -247,7 +247,7 @@ def tower(convs, x, info=None, want='fp32'):
             else:
                 h, l = ops.gn_relu_apply_f16(y, stats, m.gn.weight.detach(), m.gn.bias.detach(), m.gn.num_groups, m.gn.eps, True, flag)
         if info is not None:
-            info['backend'] = 'tcgen05-f16x2'
+            info['backend'] = 'wgmma-f16x2'
             info['overflow_flag'] = flag
         if want == 'f16pair':
             return h, l              # (B,H,W,C) fp16 operand pair of the tower output: feeds ptb_conv_tc_f16x2 directly
@@ -268,7 +268,7 @@ def tower(convs, x, info=None, want='fp32'):
             else:
                 hi, lo = res
         if info is not None:
-            info['backend'] = 'tcgen05-3xtf32'
+            info['backend'] = 'wgmma-3xtf32'
         return out.permute(0, 3, 1, 2)          # (B,C,H,W) view with channels_last strides
     if want == 'fp32' and torch.is_grad_enabled() and _tc_train_supported(convs, x):
         from . import ops
@@ -277,7 +277,7 @@ def tower(convs, x, info=None, want='fp32'):
             params += [m.conv.weight, m.gn.weight, m.gn.bias]
         out = _TowerTCFn.apply(ops.to_nhwc(x).contiguous(), convs, *params)
         if info is not None:
-            info['backend'] = 'tcgen05-f16x2-train'
+            info['backend'] = 'wgmma-f16x2-train'
         return out.permute(0, 3, 1, 2)
     if info is not None:
         info['backend'] = 'cudnn'

@@ -836,7 +836,7 @@ def conv_tc_pack_weight_f16(w, taps):
 
 
 def conv_tc_f16(x_h, x_l, packed, taps, n_out, bias=None, dev_out_scale=None, ldy=None):
-    """general tcgen05 conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias)."""
+    """general wgmma conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias)."""
     lib = _lib.load()
     _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
     w_h, w_l, inv_w, n_mma = packed

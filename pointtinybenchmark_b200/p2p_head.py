@@ -1,11 +1,11 @@
-"""P2PHead — host-side mirror of the reference's P2PNet-style head over the sm_100a kernels.
+"""P2PHead — host-side mirror of the reference's P2PNet-style head over the sm_90a kernels.
 
 reference: TOV_mmdetection/mmdet/models/point/dense_heads/p2p_head.py:18-572 (P2PHead), HungarianAssignerV2
 (core/bbox/assigners/hungarian_assigner.py:149-270), FocalLossCost/DisCostV2 (core/bbox/match_costs/match_cost.py),
 multiclass_nms (core/post_processing/bbox_nms.py).  Same ctor kwargs / outputs / state_dict keys
 (cls_convs.*, reg_convs.*, cls_out (conv3x3), reg_out (conv3x3)).
 
-What runs where: towers and the two output convs = tcgen05 implicit GEMMs of libptb_b200.so at inference; under autograd the
+What runs where: towers and the two output convs = wgmma implicit GEMMs of libptb_b200.so at inference; under autograd the
 towers use the tensor-core autograd function of layers.py (dgrad / wgrad / GroupNorm backward kernels) and the two narrow output
 convs cuDNN fp32; decode, top-k, NMS / soft-NMS, cost matrix, the Hungarian matching (scipy's shortest-augmenting-path algorithm
 restated as a one-CTA-per-image kernel, bit-identical assignments incl. ties: csrc/lsap_core.cuh; SURVEY.md §8f rank 2) and the
@@ -85,9 +85,9 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         self.train_cfg = CfgNode(train_cfg) if train_cfg is not None else None
         self.test_cfg = CfgNode(test_cfg) if test_cfg is not None else None
         if len(self.strides) != 1:
-            raise NotImplementedError('P2PHead (B200): one FPN level only (all configs2/*/p2p configs use strides=[s])')
+            raise NotImplementedError('P2PHead: one FPN level only (all configs2/*/p2p configs use strides=[s])')
         if not self.loss_cls_cfg.get('use_sigmoid', False):
-            raise NotImplementedError('P2PHead (B200): softmax classification')
+            raise NotImplementedError('P2PHead: softmax classification')
         self.num_cls_out = num_classes
         self.cls_convs, self.reg_convs = nn.ModuleList(), nn.ModuleList()
         for i in range(stacked_convs):
@@ -119,7 +119,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
 
     # ------------------------------------------------------------------------------------------------
     def forward(self, feats):
-        """p2p_head.py:104-123.  Inference: towers AND the two conv3x3 output layers run on the tcgen05 kernel (fp16 two-term
+        """p2p_head.py:104-123.  Inference: towers AND the two conv3x3 output layers run on the wgmma kernel (fp16 two-term
         split, fp32-level accuracy); with autograd recording the towers use the tensor-core autograd function of layers.py and the
         two output convs cuDNN fp32."""
         cls_outs, pts_outs = [], []
@@ -189,7 +189,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         """p2p_head.py:172-248 -> dict(loss_cls=[B], loss_pts=[B])."""
         cls_out, pts_out = cls_outs[0], pts_outs[0]
         if not cls_out.is_cuda:
-            raise RuntimeError('P2PHead (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('P2PHead runs on CUDA tensors only; there is no CPU fallback')
         for gb in gt_bboxes:                       # p2p_head.py:183-184: the reference refuses images without a GT point
             assert len(gb) > 0, gt_bboxes
         dev = cls_out.device
@@ -252,7 +252,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         num_total_pos = sum([(p[:, 0] > 0).sum() for p in pw_l]).float()
         gamma, alpha = self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25)
         if self.loss_cls_cfg['type'] != 'FocalLoss' or self.loss_reg_cfg['type'] != 'SmoothL1Loss':
-            raise NotImplementedError('P2PHead (B200): loss_cls must be FocalLoss and loss_reg SmoothL1Loss')
+            raise NotImplementedError('P2PHead: loss_cls must be FocalLoss and loss_reg SmoothL1Loss')
         loss_cls, loss_pts = [], []
         for b in range(B):
             lc = _FocalSumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], gamma, alpha)
@@ -270,7 +270,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         cfg = CfgNode(cfg) if cfg is not None else self.test_cfg
         cls_out, pts_out = cls_outs[0], pts_outs[0]
         if not cls_out.is_cuda:
-            raise RuntimeError('P2PHead (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('P2PHead runs on CUDA tensors only; there is no CPU fallback')
         if not with_nms:
             raise NotImplementedError('with_nms=False')
         dev = cls_out.device

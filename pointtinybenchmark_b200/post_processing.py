@@ -13,7 +13,7 @@ def multiclass_nms(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num=-1, s
     (n, #class*4) and `class_agnostic` NMS (both through one kernel candidate per (box, class): n * #class <= 4096), `max_num=-1`
     (exact while at most 1024 detections survive, else NotImplementedError)."""
     if not multi_bboxes.is_cuda:
-        raise RuntimeError('multiclass_nms (B200) runs on CUDA tensors only; there is no CPU fallback')
+        raise RuntimeError('multiclass_nms runs on CUDA tensors only; there is no CPU fallback')
     n, C = multi_scores.shape[0], multi_scores.shape[1] - 1
     class_specific = multi_bboxes.shape[1] > 4
     if class_specific and multi_bboxes.shape[1] != 4 * C:

@@ -145,7 +145,7 @@ class RPNProposals:
         if not with_nms:
             raise NotImplementedError('with_nms=False')
         if not cls_scores[0].is_cuda:
-            raise RuntimeError('RPNProposals (B200) runs on CUDA tensors only; there is no CPU fallback')
+            raise RuntimeError('RPNProposals runs on CUDA tensors only; there is no CPU fallback')
         cfg = CfgNode(cfg) if cfg is not None else self.test_cfg
         nms = dict(cfg.get('nms', dict(type='nms', iou_threshold=cfg.get('nms_thr', 0.7))))
         if nms.get('type', 'nms') != 'nms':

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads without a GPU, and exports every symbol include/ptb_b200.h declares."""
+"""CPU: the C-ABI library builds for sm_90a, loads without a GPU, and exports every symbol include/ptb_b200.h declares."""
 import ctypes
 import os
 import re
@@ -48,12 +48,12 @@ def test_ctypes_binding_covers_the_header(lib_path):
     assert sorted(_lib.SIGNATURES) == declared_symbols()
 
 
-def test_sass_is_sm100a_only(lib_path):
+def test_sass_is_sm90a_only(lib_path):
     r = subprocess.run(['cuobjdump', '--list-elf', lib_path], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip('cuobjdump unavailable')
     archs = set(re.findall(r'sm_\d+a?', r.stdout))
-    assert archs == {'sm_100a'}, archs
+    assert archs == {'sm_90a'}, archs
 
 
 def test_argument_validation_errors_are_reported_without_a_gpu(lib_path):

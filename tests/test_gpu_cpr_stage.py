@@ -82,7 +82,7 @@ def test_linear_and_bag_logits(ops, golden_dir, name, seed):
     ref = torch.nn.functional.linear(feats.cpu(), inp['weights']['cls_out.weight'], inp['weights']['cls_out.bias'])
     e1 = assert_close(lg, ref, 1e-4, 'linear_rows vs F.linear')
     assert np.abs(lg.cpu().flatten()[::101].numpy() - gold['pos_cls_sub']).max() <= 1e-4 * np.abs(gold['pos_cls_sub']).max()
-    # B200 dataflow: logit map first, then gather 80 channels (linearity of bilinear sampling)
+    # product dataflow: logit map first, then gather 80 channels (linearity of bilinear sampling)
     B, H, W, _ = fmap.shape
     wcat = torch.cat([w['cls_out.weight'], w['ins_out.weight']])
     bcat = torch.cat([w['cls_out.bias'], w['ins_out.bias']])

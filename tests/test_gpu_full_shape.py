@@ -1,7 +1,7 @@
 """Parity on the EXACT shapes the metric is quoted on (VERDICT r1 item 1; BASELINE.json configs[1], [2], [4]) plus
 P2PHead.aug_test_bboxes.
 
-* config 2 (B=8, 100x168x256 map, 500 points / image, r=8): the PRODUCT step the bench times — tcgen05 towers -> 1-tap logit conv ->
+* config 2 (B=8, 100x168x256 map, 500 points / image, r=8): the PRODUCT step the bench times — wgmma towers -> 1-tap logit conv ->
   ptb_cpr_refine_fused — for all 8 images against oracle tower_forward + cpr_get_bboxes, through the float64 decision-margin harness
   of tests/helpers.py (SURVEY.md §7.1): every chosen-mask / not_refine decision with margin > bound is bit-equal, floats 1e-4.
 * config 5 shard shape (2000 points / image): same harness on image 0 (replaces round 1's "<= 3 rows may differ" allowance).
@@ -77,7 +77,7 @@ def test_config2_full_shape_product_step_vs_oracle(config2, variant):
     # ---- the product call (what bench.py times)
     with torch.no_grad():
         res = head.simple_test((x,), metas, gt_bboxes=gtb, gt_labels=gtl, gt_anns_id=aid)
-        assert head.last_tower_backend == 'tcgen05-f16x2'
+        assert head.last_tower_backend == 'wgmma-f16x2'
         # the same step in pieces, to look inside: fp16 pair of the tower output -> logit map -> fused refine with the chosen mask
         info = {}
         h, l = tower(head.cls_convs, x, info, want='f16pair')
@@ -88,7 +88,7 @@ def test_config2_full_shape_product_step_vs_oracle(config2, variant):
     det_pieces = torch.cat([got[0] - 8.0, got[0] + 8.0, got[1][:, None]], 1)
     assert torch.equal(torch.cat([r[0] for r in res])[:, :5], det_pieces), 'simple_test == its pieces (deterministic)'
     # ---- oracle: reference data flow on the host (gather 256 channels, Linear per sample)
-    e_t = assert_close(feat_g, feat_o, 1e-4, 'tcgen05 towers vs oracle tower_forward at 8x256x100x168')
+    e_t = assert_close(feat_g, feat_o, 1e-4, 'wgmma towers vs oracle tower_forward at 8x256x100x168')
     with torch.no_grad():
         ores, allo = ocpr.cpr_get_bboxes(feat_o, w, inp['gt_bboxes'], inp['gt_labels'], inp['gt_anns_id'], metas, cfg, return_all=True)
     ora = _cat_refine(allo)
@@ -228,7 +228,7 @@ def test_config3_full_shape_topk_and_nms_bit_exact(iou):
 
 
 def test_config3_simple_test_through_the_towers():
-    """P2PHead.simple_test at 16 x (256,100,168): forward (two tcgen05 towers + conv3x3 outputs) within 1e-4 of the oracle on two
+    """P2PHead.simple_test at 16 x (256,100,168): forward (two wgmma towers + conv3x3 outputs) within 1e-4 of the oracle on two
     images; post-processing bit-exact on the head's OWN outputs for all 16 (top-k) / 2 images (full oracle NMS)."""
     _need_cuda()
     dev = torch.device('cuda:0')

@@ -1,4 +1,4 @@
-"""GPU: the tower's training path on the tensor cores — GroupNorm/ReLU backward, dgrad, tcgen05 wgrad (MN-major operands) and the
+"""GPU: the tower's training path on the tensor cores — GroupNorm/ReLU backward, dgrad, wgmma wgrad (MN-major operands) and the
 autograd function that chains them — against fp64 autograd on the same device and against the CPU oracle (oracle.cpr.tower_forward,
 = the reference's ConvModule stack, cpr_head.py:983-995, 1033-1043)."""
 import pytest
@@ -75,7 +75,7 @@ def test_wgrad_and_dgrad_match_fp64(ops, B, H, W):
         wf = w.clone().requires_grad_(True)
         F.conv2d(xf, wf, None, 1, 1).backward(dy.permute(0, 3, 1, 2))
         print(f'    cuDNN fp32: wgrad err {scale_rel_err(wf.grad, ref_dw):.2e}, dgrad err {scale_rel_err(xf.grad.permute(0, 2, 3, 1), ref_dx):.2e}')
-    e1 = assert_close(dw, ref_dw, 5e-5, 'dW (tcgen05 wgrad, MN-major operands)')
+    e1 = assert_close(dw, ref_dw, 5e-5, 'dW (wgmma wgrad, MN-major operands)')
     e2 = assert_close(dx, ref_dx, 2e-5, 'dX (forward kernel on W^T flipped)')
     dw2 = ops.conv3x3_wgrad_f16(dh, dl, xh, xl, 1.0, inv_dy, inv_x, out=dw.clone(), accumulate=True)
     assert_close(dw2, 2 * ref_dw, 5e-5, 'accumulate')
@@ -115,7 +115,7 @@ def test_tower_training_path_vs_fp64_and_oracle(ops):
     x = x0.to(dev).requires_grad_(True)
     info = {}
     out = tower(convs, x, info)
-    assert info['backend'] == 'tcgen05-f16x2-train', info
+    assert info['backend'] == 'wgmma-f16x2-train', info
     out.backward(dout.to(dev))
     # ReLU masks of our forward kernels (inference entry points, same arithmetic)
     masks = []

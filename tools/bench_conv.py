@@ -1,4 +1,4 @@
-"""timing of the tcgen05 3xTF32 conv3x3 + GN + ReLU layer vs cuDNN fp32 / TF32 at the headline shape (scratch tool)."""
+"""timing of the wgmma 3xTF32 conv3x3 + GN + ReLU layer vs cuDNN fp32 / TF32 at the headline shape (scratch tool)."""
 import os, sys, json
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

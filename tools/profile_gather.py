@@ -1,4 +1,4 @@
-"""runs the neighbor-gather (C=256), the fused refine, the tcgen05 conv / GroupNorm kernels and one layer of the training tower's
+"""runs the neighbor-gather (C=256), the fused refine, the wgmma conv / GroupNorm kernels and one layer of the training tower's
 backward (GroupNorm backward, split, wgrad, dgrad) a few times at the headline config: target for `ncu --set full`."""
 import os, sys
 import torch
