@@ -352,6 +352,17 @@ int ptb_sigmoid_focal_fwd_bwd(const float* logits /*[M][C]*/, const int64_t* lab
 int ptb_smooth_l1_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2]*/, int64_t M,
                           float inv_norm /* 1/(stride*reg_norm) */, float beta,
                           float* loss_sum, const float* scale, float* grad /*[M][2] or NULL*/, void* stream);
+/* the reference P2PHead's default losses (p2p_head.py:37-45), same conventions as the pair above (loss_sum += the weighted,
+ * un-normalised sum, deterministic; with grad != NULL the gradient scale * d sum / d input is written instead):
+ *   ptb_sigmoid_bce_fwd_bwd  CrossEntropyLoss(use_sigmoid=True, class_weight=None) (cross_entropy_loss.py:42-89):
+ *                            sum_m,c [(1 - t) x - log_sigmoid(x)] * weight[m], t = one-hot(labels[m]) (label outside [0, C): 0)
+ *   ptb_mse_fwd_bwd          MSELoss (mse_loss.py:9-48): sum ((pred - target) * inv_norm)^2 * weight */
+int ptb_sigmoid_bce_fwd_bwd(const float* logits /*[M][C]*/, const int64_t* labels /*[M], ==C: background*/,
+                            const float* weight /*[M] or NULL*/, int64_t M, int num_classes, float* loss_sum /*[1]*/,
+                            const float* scale /*[1] or NULL*/, float* grad /*[M][C] or NULL*/, void* stream);
+int ptb_mse_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
+                    float inv_norm /* 1/(stride*reg_norm) */, float* loss_sum, const float* scale, float* grad /*[M][2] or NULL*/,
+                    void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Conv towers on the tensor cores — replace the cuDNN calls behind CPRHead.forward_single / P2PHead.forward_single
@@ -385,9 +396,12 @@ int ptb_conv3x3_pack_weight_f16(const float* w_oihw, int Cout, int Cin, float sc
 int ptb_conv3x3_c256_f16x2(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin,
                            float out_scale, const float* dev_out_scale, float* y, double* gn_stats, void* stream);
 /* General form of the same kernel for the head's other GEMMs: taps = 1 (the per-cell Linear cls_out / ins_out of CPRHead,
- * cpr_head.py:1008-1014) or 9 (P2PHead's cls_out / reg_out conv3x3 WITH bias, p2p_head.py:98-102), n_out <= 256 output
- * channels, MMA N = n_mma (multiple of 16 >= n_out; the packed weight has zero rows beyond n_out), bias added in the
- * epilogue, output row stride ldy. */
+ * cpr_head.py:1008-1014) or 9 (P2PHead's cls_out / reg_out conv3x3 WITH bias, p2p_head.py:98-102), n_out <= 512 output
+ * channels (P2PHead at its default 4 anchors x 80 classes has 320), MMA N = n_mma (multiple of 16 in [n_out, 512]; the
+ * packed weight has zero rows beyond n_out), bias added in the epilogue, output row stride ldy (a multiple of 4, >= n_out).
+ * One launch at every width: outputs wider than 128 channels run as ceil(n_mma / 128) channel slices of 128 over the same
+ * persistent grid, so n_out <= 256 keeps its slicing (and its bits).  GroupNorm statistics stay with the 256-channel
+ * ptb_conv3x3_c256_* entry points. */
 int ptb_conv_tc_pack_weight_f16(const float* w /*[n_out][Cin][taps]*/, int n_out, int n_mma, int Cin, int taps, float scale,
                                 void* w_h, void* w_l, void* stream);
 int ptb_conv_tc_f16x2(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin, int taps,

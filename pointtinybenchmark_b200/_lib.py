@@ -68,6 +68,8 @@ SIGNATURES = {
     'ptb_point_assigner_workspace': (c_u64, [c_int, c_int]),
     'ptb_sigmoid_focal_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, c_float, c_float, P, P, P, P]),
     'ptb_smooth_l1_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, c_float, P, P, P, P]),
+    'ptb_sigmoid_bce_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
+    'ptb_mse_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, P, P, P, P]),
     'ptb_split_tf32': (c_int, [P, c_i64, P, P, P]),
     'ptb_conv3x3_pack_weight': (c_int, [P, c_int, c_int, P, P, P]),
     'ptb_conv3x3_c256_tf32x3': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P, P]),

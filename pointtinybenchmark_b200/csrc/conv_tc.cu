@@ -1,13 +1,16 @@
 // Dense convolutions of the head on the Hopper tensor cores (wgmma + TMA + mbarrier), fp32-accurate by operand splitting:
-// conv3x3 (stride 1, pad 1) and conv1x1 / per-cell Linear, Cin % 32 == 0 (fp16 mode) or Cin % 16 == 0 (TF32 mode), up to 256
-// output channels, optional bias, optional GroupNorm statistics in the epilogue; GroupNorm-apply + ReLU + operand split is a
+// conv3x3 (stride 1, pad 1) and conv1x1 / per-cell Linear, Cin % 32 == 0 (fp16 mode) or Cin % 16 == 0 (TF32 mode), up to 512
+// output channels (fp16 mode; 256 in TF32 mode and whenever GroupNorm statistics are requested), optional bias, optional
+// GroupNorm statistics in the epilogue; GroupNorm-apply + ReLU + operand split is a
 // second, HBM-bound kernel.  Replaces the cuDNN / cuBLAS calls behind CPRHead.forward_single / P2PHead.forward_single
 // (cpr_head.py:1033-1043, p2p_head.py:113-123: 4 x ConvModule(conv3x3 + GN(32) + ReLU), 79.3 GFLOP per image), the
 // per-sample cls_out / ins_out Linear of CPRHead.get_pts_outs (cpr_head.py:1045-1078, applied once per map cell here) and
-// P2PHead's cls_out / reg_out conv3x3.
+// P2PHead's cls_out / reg_out conv3x3 (k * num_classes channels: 320 at the reference's default 4 anchors x 80 classes).
 //
 // Implicit GEMM:  M = output pixels (tile = 128 pixels of one image), N = output channels in slices of NT <= 128,
 //                 K = taps x Cin.  One K-block = (tap, 64 B of input channels) = one SWIZZLE_64B row.
+//   Outputs wider than 128 channels run as ceil(n_mma / 128) slices of 128 in ONE launch (2 at 256, 3 at 320, 4 at 512); the
+//   persistent CTAs walk the (tile, slice) items, the weight TMA box of slice s starts at row 128 s (rows >= n_mma zero-filled).
 //   * A operand: 4-D TMA box {64 B ch, tile w, tile h, 1 img} of the channels-last activation at the tap-shifted origin;
 //     out-of-bounds (the zero padding of the conv and partial edge tiles) is zero-filled by the TMA unit.
 //   * B operand: 2-D TMA box {64 B k, NT co} of the packed weights W2[co][tap*Cin + ci]; rows beyond n_mma are zero-filled.
@@ -34,6 +37,7 @@
 namespace ptb {
 
 constexpr int CV_N = 256;                       // output channels of the tower convolutions
+constexpr int CV_N_MAX = 512;                   // widest output of ptb_conv_tc_f16x2 (4 slices of CV_NT)
 constexpr int CV_BM = 128;                      // output pixels per tile
 constexpr int CV_NT = 128;                      // widest output-channel slice of one item
 constexpr int CV_KB = 16;                       // fp32/TF32 input channels per K-block (64 B = one SWIZZLE_64B row)
@@ -593,7 +597,8 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
     cs.per_img = cs.n_main + cs.n_right + cs.n_bottom;
     cs.n_tiles = B * cs.per_img;
   }
-  // narrowest slice width that covers the output channels (the MMA N); 256-channel outputs run as two 128-channel slices
+  // narrowest slice width that covers the output channels (the MMA N); wider outputs run as ceil(n_mma / 128) slices of 128
+  // (two at 256 channels, up to four at CV_N_MAX)
   const int nt = (!F16 || n_mma > 64) ? CV_NT : n_mma > 32 ? 64 : n_mma > 16 ? 32 : 16;
   // the epilogue's statistics index [B][32][2] as (slice start / 8 + group in slice): 256 channels = 32 groups of 8, 128-channel slices
   PTB_REQUIRE(!gn_stats || (n_out == CV_N && n_mma == CV_N && nt == CV_NT), "GroupNorm statistics need 256 output channels (32 groups of 8)");
@@ -688,7 +693,7 @@ extern "C" int ptb_conv3x3_pack_weight_f16(const float* w_oihw, int Cout, int Ci
 extern "C" int ptb_conv_tc_pack_weight_f16(const float* w, int n_out, int n_mma, int Cin, int taps, float scale, void* w_h, void* w_l,
                                            void* stream) {
   PTB_REQUIRE(n_out > 0 && Cin > 0 && (taps == 1 || taps == 9) && w && w_h && w_l && scale > 0.f, "shape / NULL");
-  PTB_REQUIRE(n_mma >= n_out && n_mma % 16 == 0 && n_mma <= CV_N, "n_mma must be a multiple of 16 in [n_out, 256]");
+  PTB_REQUIRE(n_mma >= n_out && n_mma % 16 == 0 && n_mma <= CV_N_MAX, "n_mma must be a multiple of 16 in [n_out, 512]");
   const long long n = (long long)n_mma * Cin * taps;
   pack_conv_weight_f16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, n_out, n_mma, Cin, taps, scale,
                                                                                            reinterpret_cast<__half*>(w_h),
@@ -701,7 +706,7 @@ extern "C" int ptb_conv_tc_f16x2(const void* x_h, const void* x_l, const void* w
                                  float* y, int ldy, void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0 && (taps == 1 || taps == 9), "shape");
   PTB_REQUIRE(Cin % CV_KB_F16 == 0, "Cin must be a multiple of 32");
-  PTB_REQUIRE(n_out > 0 && n_mma >= n_out && n_mma % 16 == 0 && n_mma <= CV_N, "n_mma must be a multiple of 16 in [n_out, 256]");
+  PTB_REQUIRE(n_out > 0 && n_mma >= n_out && n_mma % 16 == 0 && n_mma <= CV_N_MAX, "n_mma must be a multiple of 16 in [n_out, 512]");
   PTB_REQUIRE(ldy >= n_out && ldy % 4 == 0, "ldy must be a multiple of 4 and >= n_out");
   PTB_REQUIRE(x_h && x_l && w_h && w_l && y, "NULL input");
   PTB_REQUIRE(((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) && ((uintptr_t)w_h % 16 == 0) && ((uintptr_t)w_l % 16 == 0) &&

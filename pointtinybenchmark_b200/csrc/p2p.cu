@@ -1,6 +1,6 @@
 // P2P head point path: decode + per-image top-k (p2p_head.py:125-170, 362-376), Hungarian cost matrix
 // (match_cost.py:94-99, 197-214), PointAssigner (point_assigner.py:23-133) and the elementwise losses
-// (focal_loss.py:11-56, smooth_l1_loss.py:25-31).  All HBM-bound scan / select work: coalesced channels-last
+// (focal_loss.py:11-56, smooth_l1_loss.py:25-31, cross_entropy_loss.py:42-89 with use_sigmoid, mse_loss.py:9-48).  All HBM-bound scan / select work: coalesced channels-last
 // reads, warp-shuffle reductions, radix select + bitonic sort in shared memory (no library sort).
 #include "ptb_common.cuh"
 #include "topk_select.cuh"
@@ -232,6 +232,47 @@ smooth_l1_kernel(const float* __restrict__ pred, const float* __restrict__ targe
   if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
 }
 
+// CrossEntropyLoss(use_sigmoid=True) = binary_cross_entropy (cross_entropy_loss.py:42-89): labels expanded to one-hot rows
+// (_expand_onehot_labels; a label outside [0, C), e.g. the background label C, is an all-zero row), the per-proposal weight
+// broadcast over the classes, F.binary_cross_entropy_with_logits(reduction='none') in ATen's CPU form
+//   (1 - t) * x - log_sigmoid(x),   log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|)),
+// then the weighted sum of weight_reduce_loss (the caller divides by avg_factor).  d/dx = sigmoid(x) - t.
+__global__ void __launch_bounds__(256)
+sigmoid_bce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight, long long M,
+                   int C, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad, SumScratch* __restrict__ scr) {
+  const long long total = M * C;
+  const float sc = (grad && scale) ? scale[0] : 1.f;
+  float acc = 0.f;
+  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256) {
+    const long long m = e / C;
+    const int c = (int)(e - m * C);
+    const float w = weight ? weight[m] : 1.f;
+    const float t = (labels[m] == c) ? 1.f : 0.f;
+    const float v = x[e];
+    if (loss_sum) {
+      const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
+      acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
+    }
+    if (grad) grad[e] = sc * w * (sigmoidf_acc(v) - t);
+  }
+  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
+}
+
+// MSELoss (mse_loss.py:9-48): sum ((pred - target) * inv_norm)^2 * weight on the normalised points; d/dpred = 2 diff inv_norm w
+__global__ void __launch_bounds__(256)
+mse_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ weight, long long n,
+           float inv_norm, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad, SumScratch* __restrict__ scr) {
+  const float sc = (grad && scale) ? scale[0] : 1.f;
+  float acc = 0.f;
+  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < n; e += (long long)gridDim.x * 256) {
+    const float w = weight ? weight[e] : 1.f;
+    const float diff = (pred[e] - target[e]) * inv_norm;
+    acc += __fmul_rn(__fmul_rn(diff, diff), w);
+    if (grad) grad[e] = sc * w * inv_norm * 2.f * diff;
+  }
+  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
+}
+
 }  // namespace ptb
 
 using namespace ptb;
@@ -335,4 +376,27 @@ extern "C" int ptb_smooth_l1_fwd_bwd(const float* pred, const float* target, con
   smooth_l1_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(pred, target, weight, M * 2, inv_norm, beta, loss_sum, scale, grad,
                                                                &scr->sl1);
   return check_launch("ptb_smooth_l1_fwd_bwd");
+}
+
+extern "C" int ptb_sigmoid_bce_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, int64_t M, int num_classes,
+                                       float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0 && num_classes > 0, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
+  StreamScratch* scr = stream_scratch(stream);
+  if (!scr) return 1;
+  sigmoid_bce_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, M, num_classes, loss_sum, scale, grad,
+                                                                   &scr->bce);
+  return check_launch("ptb_sigmoid_bce_fwd_bwd");
+}
+
+extern "C" int ptb_mse_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, float inv_norm,
+                               float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(pred && target && (loss_sum || grad), "NULL input");
+  StreamScratch* scr = stream_scratch(stream);
+  if (!scr) return 1;
+  mse_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(pred, target, weight, M * 2, inv_norm, loss_sum, scale, grad, &scr->mse);
+  return check_launch("ptb_mse_fwd_bwd");
 }

@@ -649,6 +649,31 @@ def smooth_l1(pred, target, weight, inv_norm, beta, scale=None, want_grad=False)
     return grad if want_grad else loss
 
 
+def sigmoid_bce(logits, labels, weight, scale=None, want_grad=False):
+    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels)) * weight[m] (labels == C: background row);
+    optional grad = scale * d/dlogits."""
+    lib = _lib.load()
+    _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels')
+    M, C = logits.shape
+    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
+    grad = torch.empty_like(logits) if want_grad else None
+    check(lib.ptb_sigmoid_bce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), M, C, _ptr(loss) if not want_grad else None,
+                                      _ptr(scale), _ptr(grad), _stream()), 'ptb_sigmoid_bce_fwd_bwd')
+    return grad if want_grad else loss
+
+
+def mse(pred, target, weight, inv_norm, scale=None, want_grad=False):
+    """sum ((pred - target) * inv_norm)^2 * weight over (M, 2) points; optional grad = scale * d/dpred."""
+    lib = _lib.load()
+    _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target')
+    M = pred.shape[0]
+    loss = torch.zeros(1, dtype=torch.float32, device=pred.device)
+    grad = torch.empty_like(pred) if want_grad else None
+    check(lib.ptb_mse_fwd_bwd(_ptr(pred), _ptr(target), _ptr(weight), M, float(inv_norm), _ptr(loss) if not want_grad else None,
+                              _ptr(scale), _ptr(grad), _stream()), 'ptb_mse_fwd_bwd')
+    return grad if want_grad else loss
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # conv towers on the tensor cores (3xTF32 implicit GEMM + GroupNorm + ReLU)
 # ----------------------------------------------------------------------------------------------------------------------

@@ -9,7 +9,8 @@ What runs where: towers and the two output convs = wgmma implicit GEMMs of libpt
 towers use the tensor-core autograd function of layers.py (dgrad / wgrad / GroupNorm backward kernels) and the two narrow output
 convs cuDNN fp32; decode, top-k, NMS / soft-NMS, cost matrix, the Hungarian matching (scipy's shortest-augmenting-path algorithm
 restated as a one-CTA-per-image kernel, bit-identical assignments incl. ties: csrc/lsap_core.cuh; SURVEY.md §8f rank 2) and the
-focal / smooth-L1 losses = libptb_b200.so.  Nothing of the training step returns to the host except one (B,) status read.
+losses = libptb_b200.so: FocalLoss or the reference's default CrossEntropyLoss(use_sigmoid=True) for classification,
+SmoothL1Loss or the default MSELoss for the points.  Nothing of the training step returns to the host except one (B,) status read.
 """
 import numpy as np
 import torch
@@ -45,6 +46,37 @@ class _FocalSumFn(torch.autograd.Function):
         return ops.sigmoid_focal(logits, labels, weight, ctx.ga[0], ctx.ga[1], scale=scale, want_grad=True), None, None, None, None
 
 
+class _SigmoidBCESumFn(torch.autograd.Function):
+    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels)) * weight[m]   (losses/cross_entropy_loss.py:42-89)"""
+
+    @staticmethod
+    def forward(ctx, logits, labels, weight):
+        ctx.save_for_backward(logits, labels, weight)
+        return ops.sigmoid_bce(logits, labels, weight)[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        logits, labels, weight = ctx.saved_tensors
+        scale = g.reshape(1).float().contiguous()
+        return ops.sigmoid_bce(logits, labels, weight, scale=scale, want_grad=True), None, None
+
+
+class _MSESumFn(torch.autograd.Function):
+    """sum ((pred - target) * inv_norm)^2 * weight   (losses/mse_loss.py:9-48)"""
+
+    @staticmethod
+    def forward(ctx, pred, target, weight, inv_norm):
+        ctx.save_for_backward(pred, target, weight)
+        ctx.inv_norm = inv_norm
+        return ops.mse(pred, target, weight, inv_norm)[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, target, weight = ctx.saved_tensors
+        scale = g.reshape(1).float().contiguous()
+        return ops.mse(pred, target, weight, ctx.inv_norm, scale=scale, want_grad=True), None, None, None
+
+
 class _SmoothL1SumFn(torch.autograd.Function):
     """sum smooth_l1((pred - target) * inv_norm, beta) * weight   (losses/smooth_l1_loss.py:25-31)"""
 
@@ -59,6 +91,11 @@ class _SmoothL1SumFn(torch.autograd.Function):
         pred, target, weight = ctx.saved_tensors
         scale = g.reshape(1).float().contiguous()
         return ops.smooth_l1(pred, target, weight, ctx.nb[0], ctx.nb[1], scale=scale, want_grad=True), None, None, None, None
+
+
+MAX_OUT_CHANNELS = 512     # widest output of the wgmma conv (ptb_conv_tc_f16x2): bounds num_points * num_classes
+LOSS_CLS_TYPES = ('FocalLoss', 'CrossEntropyLoss')
+LOSS_REG_TYPES = ('SmoothL1Loss', 'MSELoss')
 
 
 @register_head
@@ -89,6 +126,10 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         if not self.loss_cls_cfg.get('use_sigmoid', False):
             raise NotImplementedError('P2PHead: softmax classification')
         self.num_cls_out = num_classes
+        if max(self.num_cls_out * self.num_points, 2 * self.num_points) > MAX_OUT_CHANNELS:
+            raise NotImplementedError(
+                f'P2PHead: cls_out would have {self.num_cls_out} classes x {self.num_points} anchors = '
+                f'{self.num_cls_out * self.num_points} output channels; the output conv kernel supports at most {MAX_OUT_CHANNELS}')
         self.cls_convs, self.reg_convs = nn.ModuleList(), nn.ModuleList()
         for i in range(stacked_convs):
             chn = in_channels if i == 0 else feat_channels
@@ -120,8 +161,9 @@ class P2PHead(PackedWeightsMixin, nn.Module):
     # ------------------------------------------------------------------------------------------------
     def forward(self, feats):
         """p2p_head.py:104-123.  Inference: towers AND the two conv3x3 output layers run on the wgmma kernel (fp16 two-term
-        split, fp32-level accuracy); with autograd recording the towers use the tensor-core autograd function of layers.py and the
-        two output convs cuDNN fp32."""
+        split, fp32-level accuracy; cls_out has num_points * num_classes <= 512 channels, e.g. 320 at the reference's default 4
+        anchors x 80 classes, in one launch); with autograd recording the towers use the tensor-core autograd function of
+        layers.py and the two output convs cuDNN fp32."""
         cls_outs, pts_outs = [], []
         for x in feats:
             if tc_enabled(x, self.cls_convs, self.reg_convs, self.cls_out, self.reg_out) and self.feat_channels == 256 \
@@ -250,15 +292,26 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             pw = pos.float()[:, None].expand(Q, 2).contiguous()
             labels_l.append(labels); lw_l.append(lw.contiguous()); gp_l.append(gp.contiguous()); pw_l.append(pw)
         num_total_pos = sum([(p[:, 0] > 0).sum() for p in pw_l]).float()
+        cls_type, reg_type = self.loss_cls_cfg['type'], self.loss_reg_cfg['type']
+        if cls_type not in LOSS_CLS_TYPES or reg_type not in LOSS_REG_TYPES:
+            raise NotImplementedError(f'P2PHead: loss_cls must be one of {LOSS_CLS_TYPES} and loss_reg one of {LOSS_REG_TYPES}')
+        if cls_type == 'CrossEntropyLoss' and self.loss_cls_cfg.get('class_weight') is not None:
+            raise NotImplementedError('P2PHead: CrossEntropyLoss with class_weight')
         gamma, alpha = self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25)
-        if self.loss_cls_cfg['type'] != 'FocalLoss' or self.loss_reg_cfg['type'] != 'SmoothL1Loss':
-            raise NotImplementedError('P2PHead: loss_cls must be FocalLoss and loss_reg SmoothL1Loss')
+        # loss_single (p2p_head.py:220-231): CrossEntropyLoss averages over every proposal of the batch, FocalLoss over the positives
+        cls_avg = float(B * Q) if cls_type == 'CrossEntropyLoss' else num_total_pos
+        inv_norm = 1.0 / (s * self.reg_norm)
         loss_cls, loss_pts = [], []
         for b in range(B):
-            lc = _FocalSumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], gamma, alpha)
-            loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / num_total_pos)
-            lp = _SmoothL1SumFn.apply(pred[b].contiguous(), gp_l[b], pw_l[b], 1.0 / (s * self.reg_norm),
-                                      self.loss_reg_cfg.get('beta', 1.0))
+            if cls_type == 'CrossEntropyLoss':
+                lc = _SigmoidBCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b])
+            else:
+                lc = _FocalSumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], gamma, alpha)
+            loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / cls_avg)
+            if reg_type == 'MSELoss':
+                lp = _MSESumFn.apply(pred[b].contiguous(), gp_l[b], pw_l[b], inv_norm)
+            else:
+                lp = _SmoothL1SumFn.apply(pred[b].contiguous(), gp_l[b], pw_l[b], inv_norm, self.loss_reg_cfg.get('beta', 1.0))
             loss_pts.append(self.loss_reg_cfg.get('loss_weight', 1.0) * lp / num_total_pos)
         self._last_targets = dict(labels=labels_l, label_weights=lw_l, gt_pts=gp_l, pts_weights=pw_l)
         return dict(loss_cls=loss_cls, loss_pts=loss_pts)
