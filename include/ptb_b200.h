@@ -195,7 +195,9 @@ int ptb_cpr_bag_mil_fwd(const float* logit_map /*[B][H][W][ld]*/, int B, int H, 
  * with dLoss/d bag_logits from scale_mil (MIL term; needs bag_prob, mil_mt, label_weight = the trailing [G..2G) aux floats of
  * ptb_mil_loss_fwd's out_bag_prob buffer) and scale_gt * valid_center (gt term on the centre sample k = K-1).  Every element of
  * grad_map is written (no zero-init needed).  One CTA per 8x8-cell tile; every sum is formed by one thread in a fixed order, so the
- * result is bit-identical run to run.  ld must be a multiple of 32 and at most 160; K <= 320. */
+ * result is bit-identical run to run.  ld must be a multiple of 32 and at most 160 (every such ld, 32 to 160, is exact: narrow rows run
+ * smaller blocks and rounds of blockDim / 4 samples); K <= 320; reach_px must be at least the largest |offset| component, or samples
+ * outside the window are lost. */
 int ptb_cpr_loss_bwd_map(const float* bag_logits /*[G][K][ld]*/, const float* weight /*[G][K]*/, const float* mil_mt /*[G][N][2]*/,
                          const float* bag_prob /*[G][N]*/, const float* label_weight /*[G]*/, const int32_t* labels,
                          const float* centers /*[G][2]*/, const int32_t* img_ptr /*[B+1]*/, const float* offsets /*[K][2]*/,

@@ -14,6 +14,7 @@ through each kernel in one launch.  Positive bags: ring bags (CirclePtFeatGenera
 `other_info.out_geo` appends the chosen bag points to the output rows.
 """
 import os
+import warnings
 
 import numpy as np
 import torch
@@ -73,13 +74,16 @@ class _BatchGT:
 
 
 class _CircleBags:
-    """CirclePtFeatGenerator (cpr_head.py:447-497): ring offsets + centre, bilinear samples (ptb_cpr_bag_gather)."""
+    """CirclePtFeatGenerator (cpr_head.py:447-497): ring offsets + centre, bilinear samples (ptb_cpr_bag_gather).
+    `reach` = max |offset| in pixels, taken from the host copy of the table when it is built; it sizes the sample windows of the
+    gather, the fused refine and the deterministic loss backward (a reach that is too small loses samples)."""
 
-    def __init__(self, offsets, stride):
+    def __init__(self, offsets, stride, reach=None):
         self.offsets, self.stride = offsets, stride
+        self.reach = ops.offsets_reach(offsets) if reach is None else float(reach)
 
     def gather(self, lmap, gt, pts=False):
-        f, p, valid = ops.bag_gather(lmap, gt.centers, gt.bag_img, self.offsets, self.stride, gt.pad_hw, pts=pts)
+        f, p, valid = ops.bag_gather(lmap, gt.centers, gt.bag_img, self.offsets, self.stride, gt.pad_hw, pts=pts, reach_px=self.reach)
         return f, p, valid, None
 
     def gather_bwd(self, grad, map_shape, gt, aux):
@@ -122,6 +126,44 @@ class _BagGatherFn(torch.autograd.Function):
         return ctx.bags.gather_bwd(g.contiguous(), ctx.shape, ctx.gt, ctx.aux), None, None
 
 
+LB_MAX_LD = 160        # ptb_cpr_loss_bwd_map: logit rows of at most 160 columns (5 channel groups x 64 cells = 320 threads per tile)
+LB_MAX_K = 320         # ... and at most 320 samples per bag
+
+
+def loss_bwd_plan(N, K, circle_bags, with_mil_loss, env_mode=None, deterministic=False):
+    """Column padding and backward path of the fused CPR loss (_CPRLossFn).  A pure function of the configuration.
+
+    env_mode is PTB_LOSS_BWD (None when unset); deterministic is torch.are_deterministic_algorithms_enabled().  Returns
+    (NP, path, reason):
+      NP      ins column offset of the logit map, LD = 2 * NP.  ceil8(N) by default; ceil16(N) when bit-reproducible gradients are
+              asked for, so that LD is a multiple of 32 (the tile kernel's channel groups) for every N.
+      path    'tiles'   ptb_cpr_loss_bwd_map: deterministic, ring bags with the MIL loss, LD <= 160 (N <= 80), K <= 320
+              'scatter' ptb_cpr_loss_bwd_scatter: fp32 atomics, ring bags with the MIL loss (the default)
+              'staged'  mil_loss_bwd + gfocal_bwd + bag_gather_bwd / grid_bag_bwd: fp32 atomics, every configuration
+      reason  None, or why bit-reproducible gradients were asked for (PTB_LOSS_BWD=tiles or deterministic mode) but cannot be
+              given; `path` is then the atomic path that would run instead.  The caller raises, or warns in warn-only mode."""
+    want_tiles = env_mode == 'tiles' or (env_mode is None and deterministic)
+    NP = (N + 15) // 16 * 16 if want_tiles else (N + 7) // 8 * 8
+    LD = 2 * NP
+    circle = circle_bags and with_mil_loss
+    fallback = 'scatter' if circle and env_mode in (None, 'scatter', 'tiles') else 'staged'
+    if want_tiles:
+        if not circle_bags:
+            reason = 'grid-cell bags (GridCirclesPtFeatGenerator) have no deterministic loss backward'
+        elif not with_mil_loss:
+            reason = 'the deterministic loss backward needs with_mil_loss=True'
+        elif LD % 32 or LD > LB_MAX_LD:
+            reason = f'num_classes={N} gives logit rows of {LD} columns; the deterministic loss backward handles at most {LB_MAX_LD} (num_classes <= 80)'
+        elif K > LB_MAX_K:
+            reason = f'{K} samples per bag; the deterministic loss backward handles at most {LB_MAX_K}'
+        else:
+            return NP, 'tiles', None
+        return NP, fallback, reason
+    if deterministic:
+        return NP, fallback, f'PTB_LOSS_BWD={env_mode} selects a backward with fp32 atomics'
+    return NP, fallback, None
+
+
 def _gfocal(p, q, w, eps):
     """MILLoss.gfocal_loss (multi_instance_learning_loss.py:148-151)."""
     return -(((p - q) ** 2) * (q * (p + eps).log() + (1 - q) * (1 - p + eps).log()) * w).sum(dim=-1)
@@ -134,7 +176,11 @@ class _CPRLossFn(torch.autograd.Function):
     def forward(ctx, fmap, w_cls, b_cls, w_ins, b_ins, gt, bags, hp):
         B, H, W, C = fmap.shape
         N = hp['num_classes']
-        NP = (N + 7) // 8 * 8                  # column block per head (LD = 2*NP is a multiple of 16: GEMM K-tile)
+        K = bags.offsets.shape[0] if isinstance(bags, _CircleBags) else 0
+        env_mode = os.environ.get('PTB_LOSS_BWD')
+        NP, bwd_path, bwd_reason = loss_bwd_plan(N, K, isinstance(bags, _CircleBags), hp['with_mil_loss'], env_mode,
+                                                 torch.are_deterministic_algorithms_enabled())
+        ctx.bwd = (NP, bwd_path, bwd_reason, env_mode)
         LD = 2 * NP                            # logit row: [cls(0..N) pad | ins(NP..NP+N) pad]
         M = B * H * W
         dev = fmap.device
@@ -216,26 +262,31 @@ class _CPRLossFn(torch.autograd.Function):
         hp, gt, sv = ctx.hp, ctx.gt, ctx.saved
         B, H, W, C = fmap.shape
         N = hp['num_classes']
-        NP = (N + 7) // 8 * 8
+        NP, path, reason, env_mode = ctx.bwd
         LD = 2 * NP
         M = B * H * W
         G, K, _ = bl.shape
-        mode = os.environ.get('PTB_LOSS_BWD', 'tiles' if torch.are_deterministic_algorithms_enabled() else 'scatter')
+        if reason is not None:
+            # bit-reproducible gradients were asked for and the tile kernel cannot give them: torch's convention for an op without a
+            # deterministic implementation (raise; warn instead in warn-only mode, unless PTB_LOSS_BWD=tiles asks for it explicitly)
+            msg = f'CPRHead loss backward: no deterministic implementation here ({reason}); the {path} path uses fp32 atomics'
+            if env_mode == 'tiles' or not torch.is_deterministic_algorithms_warn_only_enabled():
+                raise RuntimeError(msg)
+            warnings.warn(msg)
         f1 = lambda t: t.reshape(1).float().contiguous()
-        circle = isinstance(ctx.bags, _CircleBags) and hp['with_mil_loss']
-        if circle and mode == 'tiles' and LD % 32 == 0 and LD <= 160 and K <= 320:
+        if path == 'tiles':
             # DETERMINISTIC mode (torch.use_deterministic_algorithms(True) or PTB_LOSS_BWD=tiles): MIL + gt + neg gfocal backward and the
             # grid_sample backward in one gather-formulated kernel, one CTA per 8x8 map tile, every sum formed by one thread in a fixed
             # order: bit-identical gradients run to run (2.2 ms at the headline batch)
             dlmap = ops.cpr_loss_bwd_map(
                 bl, weight, sv['mil_mt'], sv['bag_prob'], sv['mil_lw'], gt.labels, gt.centers, gt.img_ptr, ctx.bags.offsets, (B, H, W, LD), N, NP,
-                ctx.bags.stride, ops.offsets_reach(ctx.bags.offsets), hp['eps'],
+                ctx.bags.stride, ctx.bags.reach, hp['eps'],
                 scale_mil=f1(g_pos * hp['mil_loss_weight'] / sv['num_sample']),
                 scale_gt=f1(g_gt * hp['gt_loss_weight'] / sv['num_pos_gt']) if hp['with_gt_loss'] else None,
                 valid_center=sv['valid_center'] if hp['with_gt_loss'] else None,
                 logit_map=lmap if hp['with_neg'] else None, neg_mask=sv['neg_mask'] if hp['with_neg'] else None,
                 scale_neg=f1(g_neg * hp['neg_loss_weight'] / ctx.num_pos) if hp['with_neg'] else None)
-        elif circle and mode in ('scatter', 'tiles') and NP % 4 == 0:
+        elif path == 'scatter':
             # default: the neg term initialises the map (no memset + read-modify-write), then one kernel per batch computes the MIL + gt
             # gradient of every bag sample from the forward's per-(bag, class) statistics and scatters it with fp32 vector atomics; the
             # (G,K,LD) gradient tensor of round 1 (740 MB written and re-read) and mil_bwd's three passes are gone
@@ -363,16 +414,22 @@ class CPRHead(PackedWeightsMixin, nn.Module):
     def _bags(self, gen_cfg, device):
         if gen_cfg['type'] == 'GridCirclesPtFeatGenerator':
             return _GridCircleBags(gen_cfg['radius'], gen_cfg.get('max_pos_num', -1), float(self.strides[0]))
-        return _CircleBags(self._offsets(gen_cfg, device), float(self.strides[0]))
+        off, reach = self._offset_table(gen_cfg, device)
+        return _CircleBags(off, float(self.strides[0]), reach)
 
     def _offsets(self, gen_cfg, device):
+        return self._offset_table(gen_cfg, device)[0]
+
+    def _offset_table(self, gen_cfg, device):
+        """(device offset table, its reach in pixels); the reach comes from the host table when the table is built."""
         key = (gen_cfg.get('radius'), gen_cfg.get('start_angle', 0), gen_cfg.get('base_num_point', 8),
                gen_cfg.get('same_num_all_radius', False), gen_cfg.get('append_center', True), str(device))
         if key not in self._offset_cache:
             off = ops.circle_offsets(gen_cfg['radius'], self.strides[0], gen_cfg.get('start_angle', 0),
                                      gen_cfg.get('base_num_point', 8), gen_cfg.get('same_num_all_radius', False),
                                      gen_cfg.get('append_center', True))
-            self._offset_cache[key] = off.to(device)
+            reach = ops.offsets_reach(off)
+            self._offset_cache[key] = (ops.with_reach(off.to(device), reach), reach)
         return self._offset_cache[key]
 
     # ------------------------------------------------------------------------------------------------
@@ -577,9 +634,9 @@ class CPRHead(PackedWeightsMixin, nn.Module):
             o_pts, o_sc, o_nr, o_ch, _ = ops.refine(prob, pts, valid, pts.shape[1], gt.labels, gt.bag_img, gt.img_hw, groups, cfg,
                                                     not_refine=not_refine, want_masks=want_chosen)
             return (o_pts, o_sc, o_nr, o_ch, pts[..., :2]) if want_bag_pts else (o_pts, o_sc, o_nr, o_ch)
-        off = self._offsets(gen, dev)
+        off, reach = self._offset_table(gen, dev)
         out = ops.refine_fused(lmap, self.num_classes, gt.centers, gt.labels, gt.bag_img, off, self.strides[0], gt.pad_hw,
-                               gt.img_hw, groups, cfg, not_refine=not_refine, want_chosen=want_chosen)
+                               gt.img_hw, groups, cfg, not_refine=not_refine, want_chosen=want_chosen, reach_px=reach)
         if want_bag_pts:
             return out + (off[None, :, :] + gt.centers[:, None, :],)        # cpr_head.py:492-497 (same fp32 add as the kernel)
         return out

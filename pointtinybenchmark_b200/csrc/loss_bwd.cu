@@ -11,9 +11,11 @@
 //   A  the bags of the image whose sample window reaches the tile, in GT order (ordered ballot compaction);
 //   B  bag by bag, warp w evaluates samples 32w .. 32w+31 (lane = sample: tap geometry, which taps land in the tile) and the samples
 //      with a tap in the tile are appended to a record buffer in (bag, k) order;
-//   C  rounds of 64 records: (1) one warp per record, lanes = classes: two coalesced loads of the sampled logits, the per-sample gradient
-//      row staged in shared memory; (2) the <= 256 (record, tap) hits of the round are counting-sorted by cell (stable); (3) every
-//      (cell, channel group) thread walks its cell's hits in order: acc += w * staged row.
+//   C  rounds of min(64, blockDim.x / 4) records: (1) one warp per record, lanes = classes: two coalesced loads of the sampled logits,
+//      the per-sample gradient row staged in shared memory; (2) the (record, tap) hits of the round, one per thread, are counting-sorted
+//      by cell (stable); (3) every (cell, channel group) thread walks its cell's hits in order: acc += w * staged row.  A round never
+//      has more hits than the block has threads (LD = 32 runs 64 threads, 16 records per round); the rounds only split the record list,
+//      so every cell still adds its hits in record order whatever the round size.
 // No atomics anywhere and every sum is evaluated by ONE thread in a FIXED order: bit-identical run to run, no zero-initialised gradient
 // map, no materialised (G,K,2N) gradient tensor (740 MB written and re-read in round 1).  An earlier version (one warp per (bag, chunk),
 // per-(tap, channel) shared-memory atomics into 64-bit fixed point) spent its time in atomic loops and at the block barrier; this layout
@@ -96,8 +98,9 @@ cpr_loss_bwd_tile_kernel(const LossBwdArgs a) {
   // ---- C: consume the record buffer in rounds of LB_ROUND
   auto process = [&]() {
     const int nrec = s_nrec;                                               // (caller has synchronised)
-    for (int r0 = 0; r0 < nrec; r0 += LB_ROUND) {
-      const int nr = min(LB_ROUND, nrec - r0);
+    const int round = min(LB_ROUND, (int)blockDim.x >> 2);                 // 4 hits per record, one sorting thread per hit
+    for (int r0 = 0; r0 < nrec; r0 += round) {
+      const int nr = min(round, nrec - r0);
       // (1) gradient rows: one warp per record, lanes = classes
       for (int r = warp; r < nr; r += nwarps) {
         const LbRec rec = s_rec[r0 + r];
@@ -386,7 +389,11 @@ extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight
   const int threads = LB_CELLS * (ld / 32);
   PTB_REQUIRE(threads <= 320 || ld <= 512, "ld");
   if (threads > 320) return fail("%s", "ptb_cpr_loss_bwd_map: ld > 160 needs more than 320 threads per tile (not built)");
-  if (smem > 40 * 1024 &&
+  // the static arrays (record buffer, candidate list, hit list: ~21 KB) count against the 48 KB default too: ld = 128 needs the opt-in.
+  // Queried on every call (a host-side lookup, cheap next to the launch) so the value is that of the current device's image.
+  cudaFuncAttributes fa;
+  if (cudaFuncGetAttributes(&fa, cpr_loss_bwd_tile_kernel) != cudaSuccess) return fail("%s", "ptb_cpr_loss_bwd_map: cudaFuncGetAttributes failed");
+  if (smem + fa.sharedSizeBytes > 48 * 1024 &&
       cudaFuncSetAttribute(cpr_loss_bwd_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return fail("%s", "ptb_cpr_loss_bwd_map: shared memory opt-in failed");
   dim3 grid((W + LB_T - 1) / LB_T, (H + LB_T - 1) / LB_T, B);

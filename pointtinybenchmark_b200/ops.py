@@ -52,8 +52,9 @@ def circle_offsets(radius, stride, start_angle=0, base_num_point=8, same_num_all
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-def bag_gather(map_nhwc, centers, bag_img, offsets, stride, pad_hw, feats=True, pts=True, valid=True, C=None):
-    """ptb_cpr_bag_gather. map_nhwc (B,H,W,ld) fp32; centers (G,2); bag_img (G,) int32; offsets (K,2); pad_hw (B,2) int32.
+def bag_gather(map_nhwc, centers, bag_img, offsets, stride, pad_hw, feats=True, pts=True, valid=True, C=None, reach_px=None):
+    """ptb_cpr_bag_gather. map_nhwc (B,H,W,ld) fp32; centers (G,2); bag_img (G,) int32; offsets (K,2); pad_hw (B,2) int32;
+    reach_px: max |offset| (offsets_reach(offsets) when None).
     returns (feats (G,K,C) | None, pts (G,K,3) | None, valid (G,K) bool | None)."""
     lib = _lib.load()
     _chk(map_nhwc, torch.float32, 'map'); _chk(centers, torch.float32, 'centers'); _chk(bag_img, torch.int32, 'bag_img')
@@ -66,7 +67,8 @@ def bag_gather(map_nhwc, centers, bag_img, offsets, stride, pad_hw, feats=True, 
     o_p = torch.empty((G, K, 3), dtype=torch.float32, device=dev) if pts else None
     o_v = torch.empty((G, K), dtype=torch.uint8, device=dev) if valid else None
     check(lib.ptb_cpr_bag_gather(_ptr(map_nhwc), B, H, W, C, ld, _ptr(centers), _ptr(bag_img), G, _ptr(offsets), K,
-                                 float(stride), float(offsets_reach(offsets)) if feats else 0.0, _ptr(pad_hw), _ptr(o_f), _ptr(o_p), _ptr(o_v),
+                                 float(stride), (float(offsets_reach(offsets) if reach_px is None else reach_px)) if feats else 0.0,
+                                 _ptr(pad_hw), _ptr(o_f), _ptr(o_p), _ptr(o_v),
                                  _stream()),
           'ptb_cpr_bag_gather')
     return o_f, o_p, (o_v.bool() if o_v is not None else None)
@@ -242,19 +244,26 @@ def refine(bag_prob, bag_pts, bag_valid, K, labels, bag_img, img_hw, groups, cfg
     return o_pts, o_sc, o_nr.bool(), (o_ch.bool() if want_masks else None), (o_mv.bool() if want_masks else None)
 
 
-_REACH_CACHE = {}
+def with_reach(offsets, reach):
+    """attach the reach of a bag offset table to the tensor object (see offsets_reach); returns `offsets`.  Inference tensors have no
+    version counter, so nothing is attached to them (an in-place change could not be detected)."""
+    if not offsets.is_inference():
+        offsets._ptb_reach = (offsets._version, float(reach))
+    return offsets
 
 
 def offsets_reach(offsets):
-    """max |offset| of a bag offset table in pixels (= radius * stride for ring bags): sizes the shared-memory window the fused refine
-    kernel stages per GT.  Read back from the device ONCE per table (cached by storage), never on the steady-state path."""
-    key = (offsets.data_ptr(), offsets.numel(), str(offsets.device))
-    r = _REACH_CACHE.get(key)
-    if r is None:
-        r = float(offsets.detach().abs().max()) if offsets.numel() else 0.0
-        if len(_REACH_CACHE) > 64:
-            _REACH_CACHE.clear()
-        _REACH_CACHE[key] = r
+    """max |offset| of a bag offset table in pixels (= radius * stride for ring bags): sizes the shared-memory windows the gather, the
+    fused refine and the deterministic loss backward stage per GT.  Cached on the tensor object itself (valid while the tensor is not
+    modified in place), never by address: the caching allocator hands a freed table's address to the next allocation of that size.
+    A device table without a cached reach is read back (a host sync): once per table, or on every call for an inference tensor.
+    CPRHead keeps the reach of its host table beside the device table and passes it explicitly instead."""
+    if not offsets.is_inference():
+        cached = getattr(offsets, '_ptb_reach', None)
+        if cached is not None and cached[0] == offsets._version:
+            return cached[1]
+    r = float(offsets.detach().abs().max()) if offsets.numel() else 0.0
+    with_reach(offsets, r)
     return r
 
 

@@ -259,6 +259,103 @@ def test_training_gradients_are_deterministic(build):
         assert_close(other[3], grads[0][3], 2e-4, f'mode {mode}: dW ins')
 
 
+@pytest.mark.parametrize('deterministic', [False, True])
+@pytest.mark.parametrize('N', [1, 10, 33, 100])
+def test_loss_and_grads_class_counts(build, N, deterministic):
+    """CPRHead.loss + backward against the oracle at class counts other than 80, in the default mode and under
+    torch.use_deterministic_algorithms(True).  Deterministic mode pads the logit rows to NP = ceil16(N) (LD = 32, 32, 96 here, so the
+    1-tap wgmma GEMMs run with 32- and 96-column operands) and must give bit-identical gradients on two runs; at N = 100 it has no tile
+    kernel and must raise, or warn and run the atomic path in warn-only mode."""
+    dev = torch.device('cuda:0')
+    inp = synth.cpr_inputs('lite', 500 + N, num_classes=N)
+    cfg = oracle_cfg(inp['cfgd'])
+    head = build(inp)
+    gtb, gtl, _ = _to_dev(inp, dev)
+
+    def run():
+        head.zero_grad(set_to_none=True)
+        feat = inp['cls_feat'].to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+        losses = head.loss([feat], [feat], gtb, gtl, inp['img_metas'])
+        sum(v for k, v in losses.items() if 'loss' in k).backward()
+        return losses, [feat.grad.clone()] + [p.grad.clone() for p in (head.cls_out.weight, head.cls_out.bias, head.ins_out.weight)]
+
+    os.environ.pop('PTB_LOSS_BWD', None)
+    torch.use_deterministic_algorithms(deterministic)
+    try:
+        if deterministic and N > 80:
+            with pytest.raises(RuntimeError, match='no deterministic implementation'):
+                run()
+            torch.use_deterministic_algorithms(True, warn_only=True)
+            with pytest.warns(UserWarning, match='no deterministic implementation'):
+                losses, grads = run()
+        else:
+            losses, grads = run()
+            if deterministic:
+                _, again = run()
+                assert all(torch.equal(a, b) for a, b in zip(grads, again)), f'N={N}: deterministic mode gave different gradient bits'
+    finally:
+        torch.use_deterministic_algorithms(False)
+    fo = inp['cls_feat'].clone().requires_grad_(True)
+    wo = {k: v.clone().requires_grad_(True) for k, v in inp['weights'].items()}
+    ol = ocpr.cpr_loss(fo, wo, inp['gt_bboxes'], inp['gt_labels'], inp['img_metas'], cfg)
+    sum(v for k, v in ol.items() if 'loss' in k).backward()
+    errs = {k: assert_close(losses[k].reshape(-1), ol[k].detach().reshape(-1), 1e-4, f'N={N} {k}')
+            for k in ('gt_loss', 'pos_loss', 'neg_loss', 'bag_acc')}
+    errs['feat'] = assert_close(grads[0], fo.grad, 2e-4, f'N={N} d loss / d feature map')
+    errs['Wcls'] = assert_close(grads[1], wo['cls_out.weight'].grad, 2e-4, f'N={N} dW cls')
+    errs['bcls'] = assert_close(grads[2], wo['cls_out.bias'].grad, 2e-4, f'N={N} db cls')
+    errs['Wins'] = assert_close(grads[3], wo['ins_out.weight'].grad, 2e-4, f'N={N} dW ins')
+    print(f'[class counts] N={N} deterministic={deterministic}: ' + ', '.join(f'{k} {v:.1e}' for k, v in errs.items()))
+
+
+def test_deterministic_mode_refuses_atomics(build):
+    """an explicit PTB_LOSS_BWD=tiles that the tile kernel cannot serve raises even in warn-only mode, and PTB_LOSS_BWD=scatter under
+    torch.use_deterministic_algorithms(True) raises: neither may run fp32 atomics silently."""
+    dev = torch.device('cuda:0')
+    inp = synth.cpr_inputs('lite', 9, num_classes=100)
+    head = build(inp)
+    gtb, gtl, _ = _to_dev(inp, dev)
+
+    def run():
+        feat = inp['cls_feat'].to(dev).requires_grad_(True)
+        losses = head.loss([feat], [feat], gtb, gtl, inp['img_metas'])
+        sum(v for k, v in losses.items() if 'loss' in k).backward()
+
+    try:
+        os.environ['PTB_LOSS_BWD'] = 'tiles'
+        torch.use_deterministic_algorithms(True, warn_only=True)
+        with pytest.raises(RuntimeError, match='num_classes=100'):
+            run()
+        torch.use_deterministic_algorithms(False)
+        with pytest.raises(RuntimeError, match='num_classes=100'):
+            run()
+        os.environ['PTB_LOSS_BWD'] = 'scatter'
+        torch.use_deterministic_algorithms(True)
+        with pytest.raises(RuntimeError, match='PTB_LOSS_BWD=scatter'):
+            run()
+    finally:
+        os.environ.pop('PTB_LOSS_BWD', None)
+        torch.use_deterministic_algorithms(False)
+
+
+def test_offsets_reach_follows_the_table(build):
+    """the reach of an offset table belongs to the tensor, not to its address: a freed stride-4 table whose memory is handed to a
+    stride-8 table of the same size must not lend it its (smaller) reach."""
+    from pointtinybenchmark_b200 import ops
+    from pointtinybenchmark_b200.cpr_head import _CircleBags
+    dev = torch.device('cuda:0')
+    a = ops.circle_offsets(3, 4).to(dev)
+    ra = _CircleBags(a, 4.0).reach
+    ptr = a.data_ptr()
+    del a
+    b = ops.circle_offsets(3, 8).to(dev)
+    reused = b.data_ptr() == ptr
+    assert ra == 12.0
+    assert ops.offsets_reach(b) == 24.0 and _CircleBags(b, 8.0).reach == 24.0
+    if not reused:
+        pytest.skip('the caching allocator did not hand the freed table\'s address to the new one: the stale-reach case did not arise')
+
+
 @pytest.mark.parametrize('variant', ['softmax', 'normed_sigmoid', 'fcs_binary'])
 def test_head_variants_loss_grads_and_refine(golden_dir, variant):
     """the variants the reference class accepts beyond the shipped configs (cpr_head.py:1000-1008, 1055-1059, 1080-1099, 1108-1114;
