@@ -244,6 +244,18 @@ int ptb_p2p_decode_topk(const float* cls_map, const float* reg_map, int B, int H
                         int32_t* out_topk_idx /*[B][P]*/, float* out_pts /*[B][P][2]*/, float* out_scores /*[B][P][C]*/,
                         void* workspace, uint64_t workspace_bytes, void* stream);
 uint64_t ptb_p2p_decode_topk_workspace(int B, int H, int W, int k);
+/* Softmax classification (CrossEntropyLoss(use_sigmoid=False), p2p_head.py:63-67,363,370): the same arguments, workspace and outputs,
+ * but a cls row holds num_classes + 1 logits, background last (cls_map [B][H][W][k*(C+1)]):
+ *   key[q]              = max_{c<C} softmax(cls[q])[c] = exp(max_{c<C} x_c - m) / s,  m = max over the C+1 logits, s = sum exp(x - m)
+ *   out_topk_idx[b][r]  = index of the r-th largest key (ties: lower index first)
+ *   out_scores[b][r][c] = softmax(cls[topk])[c] for the C foreground classes (multiclass_nms drops the background column);
+ *                         max_c out_scores[b][r][c] equals that proposal's key bit for bit.
+ * Probabilities are within a few ulps of ATen's CPU softmax, not bit-identical to it. */
+int ptb_p2p_decode_topk_softmax(const float* cls_map, const float* reg_map, int B, int H, int W, int num_classes, int k,
+                                const float* point_anchor /*[k][2]*/, float stride, float pts_gamma,
+                                const int32_t* img_hw, const float* scale_xy /*[B][2] or NULL*/, int nms_pre,
+                                int32_t* out_topk_idx /*[B][P]*/, float* out_pts /*[B][P][2]*/, float* out_scores /*[B][P][C]*/,
+                                void* workspace, uint64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * multiclass NMS — replaces multiclass_nms (mmdet/core/post_processing/bbox_nms.py:7-94) and the third-party
@@ -365,6 +377,22 @@ int ptb_sigmoid_bce_fwd_bwd(const float* logits /*[M][C]*/, const int64_t* label
 int ptb_mse_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
                     float inv_norm /* 1/(stride*reg_norm) */, float* loss_sum, const float* scale, float* grad /*[M][2] or NULL*/,
                     void* stream);
+/* CrossEntropyLoss with its class_weight option and in softmax mode, same conventions:
+ *   ptb_sigmoid_bce_cw_fwd_bwd  use_sigmoid=True with class_weight, which mmdet passes as pos_weight of
+ *                               binary_cross_entropy_with_logits (cross_entropy_loss.py:85-86), in ATen's CPU order:
+ *                               sum_m,c [(1 - t) x - log_sigmoid(x) ((pw_c - 1) t + 1)] * weight[m];
+ *                               grad (pw_c t + 1 - t) sigmoid(x) - pw_c t.  pos_weight NULL: the bits of ptb_sigmoid_bce_fwd_bwd
+ *   ptb_softmax_ce_fwd_bwd      use_sigmoid=False (cross_entropy_loss.py:9-39): over rows of num_cols = C + 1 logits,
+ *                               sum_m weight[m] cw[y_m] (logsumexp(x_m) - x_m[y_m]); grad weight[m] cw[y_m] (softmax(x_m) - onehot(y_m)).
+ *                               Labels lie in [0, num_cols) (background = num_cols - 1); a row with a label outside it gets a NaN
+ *                               loss and gradient.  num_cols >= 2. */
+int ptb_sigmoid_bce_cw_fwd_bwd(const float* logits /*[M][C]*/, const int64_t* labels /*[M], ==C: background*/,
+                               const float* weight /*[M] or NULL*/, const float* pos_weight /*[C] or NULL*/, int64_t M,
+                               int num_classes, float* loss_sum /*[1]*/, const float* scale /*[1] or NULL*/,
+                               float* grad /*[M][C] or NULL*/, void* stream);
+int ptb_softmax_ce_fwd_bwd(const float* logits /*[M][num_cols]*/, const int64_t* labels /*[M]*/, const float* weight /*[M] or NULL*/,
+                           const float* class_weight /*[num_cols] or NULL*/, int64_t M, int num_cols, float* loss_sum /*[1]*/,
+                           const float* scale /*[1] or NULL*/, float* grad /*[M][num_cols] or NULL*/, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Conv towers on the tensor cores — replace the cuDNN calls behind CPRHead.forward_single / P2PHead.forward_single

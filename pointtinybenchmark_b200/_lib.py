@@ -51,6 +51,8 @@ SIGNATURES = {
     'ptb_p2p_decode_topk': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, c_float, c_float, P, P, c_int, P, P, P, P,
                                     c_u64, P]),
     'ptb_p2p_decode_topk_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
+    'ptb_p2p_decode_topk_softmax': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, c_float, c_float, P, P, c_int, P, P, P, P,
+                                            c_u64, P]),
     'ptb_multiclass_nms': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, P, P, P, P, P, P,
                                    c_u64, P]),
     'ptb_multiclass_nms_workspace': (c_u64, [c_int, c_int, c_int]),
@@ -70,6 +72,8 @@ SIGNATURES = {
     'ptb_smooth_l1_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, c_float, P, P, P, P]),
     'ptb_sigmoid_bce_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_mse_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, P, P, P, P]),
+    'ptb_sigmoid_bce_cw_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
+    'ptb_softmax_ce_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_split_tf32': (c_int, [P, c_i64, P, P, P]),
     'ptb_conv3x3_pack_weight': (c_int, [P, c_int, c_int, P, P, P]),
     'ptb_conv3x3_c256_tf32x3': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P, P]),

@@ -1,6 +1,7 @@
-// P2P head point path: decode + per-image top-k (p2p_head.py:125-170, 362-376), Hungarian cost matrix
-// (match_cost.py:94-99, 197-214), PointAssigner (point_assigner.py:23-133) and the elementwise losses
-// (focal_loss.py:11-56, smooth_l1_loss.py:25-31, cross_entropy_loss.py:42-89 with use_sigmoid, mse_loss.py:9-48).  All HBM-bound scan / select work: coalesced channels-last
+// P2P head point path: decode + per-image top-k with sigmoid or softmax scores (p2p_head.py:125-170, 362-376), Hungarian cost
+// matrix (match_cost.py:94-99, 197-214), PointAssigner (point_assigner.py:23-133) and the elementwise losses
+// (focal_loss.py:11-56, smooth_l1_loss.py:25-31, cross_entropy_loss.py:9-89 sigmoid with or without class_weight and softmax,
+// mse_loss.py:9-48).  All HBM-bound scan / select work: coalesced channels-last
 // reads, warp-shuffle reductions, radix select + bitonic sort in shared memory (no library sort).
 #include "ptb_common.cuh"
 #include "topk_select.cuh"
@@ -53,9 +54,42 @@ p2p_score_kernel(const float* __restrict__ cls_map, long long BQ, int k, int C, 
   (void)k;
 }
 
+// Softmax over one row of C1 logits (background last), by one warp: m = max_c x_c, s = sum_c exp(x_c - m) (lane-strided partial
+// sums, then the xor butterfly: a fixed order, the same bits in every lane and in every kernel that calls this), e_fg =
+// max_{c < C1-1} exp(x_c - m).  softmax(row)[c] = exp(x_c - m) / s; division by s > 0 is monotone, so the largest foreground
+// probability is exactly e_fg / s.
+__device__ __forceinline__ void softmax_row_stats(const float* __restrict__ row, int C1, int lane, float& m, float& s, float& e_fg) {
+  float mx = -CUDART_INF_F;
+  for (int c = lane; c < C1; c += 32) mx = fmaxf(mx, row[c]);
+  m = warp_max(mx);
+  float acc = 0.f, ef = 0.f;
+  for (int c = lane; c < C1; c += 32) {
+    const float e = sleef_expf_u10(__fsub_rn(row[c], m));
+    acc = __fadd_rn(acc, e);
+    if (c < C1 - 1) ef = fmaxf(ef, e);
+  }
+  s = warp_sum(acc);
+  e_fg = warp_max(ef);
+}
+
+// softmax classification (use_sigmoid=False, p2p_head.py:363,370): key[b][q] = max_{c<C} softmax(cls[b][q])[c] over a row of C+1
+// logits.  One warp per proposal.
+__global__ void __launch_bounds__(256)
+p2p_softmax_score_kernel(const float* __restrict__ cls_map, long long BQ, int C, float* __restrict__ key) {
+  const long long wq = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (wq >= BQ) return;
+  float m, s, e_fg;
+  softmax_row_stats(cls_map + wq * (C + 1), C + 1, lane, m, s, e_fg);
+  if (lane == 0) key[wq] = __fdiv_rn(e_fg, s);
+}
+
 // (radix select + bitonic sort: topk_select.cuh, shared with the RPN proposal path of rpn.cu)
 
-// gather: decode the selected proposals
+// gather: decode the selected proposals.  SOFTMAX: rows of C+1 logits, out_scores = the C foreground probabilities (the background
+// column is what multiclass_nms drops, bbox_nms.py:34,42), computed by softmax_row_stats like the key of p2p_softmax_score_kernel, so
+// max_c out_scores[r][c] equals the key bit for bit.
+template <bool SOFTMAX>
 __global__ void __launch_bounds__(256)
 p2p_gather_kernel(const float* __restrict__ cls_map, const float* __restrict__ reg_map, int H, int W, int C, int k,
                   const float* __restrict__ point_anchor, float stride, float gamma, const int32_t* __restrict__ img_hw,
@@ -83,9 +117,16 @@ p2p_gather_kernel(const float* __restrict__ cls_map, const float* __restrict__ r
     if (scale_xy) { x = __fdiv_rn(x, scale_xy[2 * b]); y = __fdiv_rn(y, scale_xy[2 * b + 1]); }
     out_pts[wr * 2] = x; out_pts[wr * 2 + 1] = y;
   }
-  const float* row = cls_map + ((size_t)b * Q + q) * C;
   float* orow = out_scores + wr * C;
-  for (int c = lane; c < C; c += 32) orow[c] = sigmoidf_acc(row[c]);
+  if constexpr (SOFTMAX) {
+    const float* row = cls_map + ((size_t)b * Q + q) * (C + 1);
+    float m, s, e_fg;
+    softmax_row_stats(row, C + 1, lane, m, s, e_fg);
+    for (int c = lane; c < C; c += 32) orow[c] = __fdiv_rn(sleef_expf_u10(__fsub_rn(row[c], m)), s);
+  } else {
+    const float* row = cls_map + ((size_t)b * Q + q) * C;
+    for (int c = lane; c < C; c += 32) orow[c] = sigmoidf_acc(row[c]);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -237,9 +278,14 @@ smooth_l1_kernel(const float* __restrict__ pred, const float* __restrict__ targe
 // broadcast over the classes, F.binary_cross_entropy_with_logits(reduction='none') in ATen's CPU form
 //   (1 - t) * x - log_sigmoid(x),   log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|)),
 // then the weighted sum of weight_reduce_loss (the caller divides by avg_factor).  d/dx = sigmoid(x) - t.
+// POS_WEIGHT: CrossEntropyLoss.class_weight, which binary_cross_entropy passes as pos_weight (cross_entropy_loss.py:85-86), in
+// ATen's CPU order: log_weight = (pw_c - 1) * t + 1, loss = (1 - t) * x - log_sigmoid(x) * log_weight; d/dx = (pw_c t + 1 - t)
+// sigmoid(x) - pw_c t (binary_cross_entropy_with_logits_backward).  Without it the kernel is the class_weight=None form above.
+template <bool POS_WEIGHT>
 __global__ void __launch_bounds__(256)
-sigmoid_bce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight, long long M,
-                   int C, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad, SumScratch* __restrict__ scr) {
+sigmoid_bce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight,
+                   const float* __restrict__ pos_weight, long long M, int C, float* loss_sum, const float* __restrict__ scale,
+                   float* __restrict__ grad, SumScratch* __restrict__ scr) {
   const long long total = M * C;
   const float sc = (grad && scale) ? scale[0] : 1.f;
   float acc = 0.f;
@@ -249,11 +295,59 @@ sigmoid_bce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labe
     const float w = weight ? weight[m] : 1.f;
     const float t = (labels[m] == c) ? 1.f : 0.f;
     const float v = x[e];
-    if (loss_sum) {
-      const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
-      acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
+    if constexpr (POS_WEIGHT) {
+      const float pw = pos_weight[c];
+      if (loss_sum) {
+        const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
+        const float log_w = __fadd_rn(__fmul_rn(__fsub_rn(pw, 1.f), t), 1.f);
+        acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), __fmul_rn(log_sig, log_w)), w);
+      }
+      if (grad) {
+        const float pt = __fmul_rn(pw, t);
+        grad[e] = sc * w * __fsub_rn(__fmul_rn(__fsub_rn(__fadd_rn(pt, 1.f), t), sigmoidf_acc(v)), pt);
+      }
+    } else {
+      if (loss_sum) {
+        const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
+        acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
+      }
+      if (grad) grad[e] = sc * w * (sigmoidf_acc(v) - t);
     }
-    if (grad) grad[e] = sc * w * (sigmoidf_acc(v) - t);
+  }
+  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
+}
+
+// CrossEntropyLoss(use_sigmoid=False) = cross_entropy (cross_entropy_loss.py:9-39): F.cross_entropy(x, y, weight=class_weight,
+// reduction='none') over rows of C1 logits (background label C1-1 is an ordinary column), times the per-proposal weight, summed
+// (the caller divides by avg_factor):  loss_m = w_m cw[y_m] (logsumexp(x_m) - x_m[y_m]),  d/dx = w_m cw[y_m] (softmax(x_m) - onehot(y_m)).
+// One warp per row (softmax_row_stats); lane 0 carries the row's loss into the ordered block-partial sum.  A label outside [0, C1)
+// makes its row's loss and gradient NaN: the library cannot report device data as an error code.
+__global__ void __launch_bounds__(256)
+softmax_ce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight,
+                  const float* __restrict__ class_weight, long long M, int C1, float* loss_sum, const float* __restrict__ scale,
+                  float* __restrict__ grad, SumScratch* __restrict__ scr) {
+  const int lane = threadIdx.x & 31;
+  const float sc = (grad && scale) ? scale[0] : 1.f;
+  float acc = 0.f;
+  for (long long r = (long long)blockIdx.x * 8 + (threadIdx.x >> 5); r < M; r += (long long)gridDim.x * 8) {
+    const float* row = x + r * C1;
+    const int64_t y = labels[r];
+    const bool ok = y >= 0 && y < C1;
+    float m, s, e_fg;
+    softmax_row_stats(row, C1, lane, m, s, e_fg);
+    const float w = !ok ? CUDART_NAN_F : __fmul_rn(weight ? weight[r] : 1.f, class_weight ? class_weight[y] : 1.f);
+    if (loss_sum && lane == 0) {
+      const float lse = __fadd_rn(m, logf(s));
+      acc += __fmul_rn(__fsub_rn(lse, ok ? row[y] : 0.f), w);
+    }
+    if (grad) {
+      const float g = sc * w;
+      float* grow = grad + r * C1;
+      for (int c = lane; c < C1; c += 32) {
+        const float p = __fdiv_rn(sleef_expf_u10(__fsub_rn(row[c], m)), s);
+        grow[c] = __fmul_rn(g, __fsub_rn(p, c == y ? 1.f : 0.f));
+      }
+    }
   }
   if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
 }
@@ -281,10 +375,14 @@ extern "C" uint64_t ptb_p2p_decode_topk_workspace(int B, int H, int W, int k) {
   return (uint64_t)B * H * W * k * sizeof(float) + (uint64_t)B * TOPK_MAX * sizeof(int32_t);
 }
 
-extern "C" int ptb_p2p_decode_topk(const float* cls_map, const float* reg_map, int B, int H, int W, int num_classes, int k,
-                                   const float* point_anchor, float stride, float pts_gamma, const int32_t* img_hw,
-                                   const float* scale_xy, int nms_pre, int32_t* out_topk_idx, float* out_pts, float* out_scores,
-                                   void* workspace, uint64_t workspace_bytes, void* stream) {
+// decode + top-k of both score forms: sigmoid over rows of C logits, or softmax over rows of C+1 (background last)
+template <bool SOFTMAX>
+static int p2p_decode_topk(const float* cls_map, const float* reg_map, int B, int H, int W, int num_classes, int k,
+                           const float* point_anchor, float stride, float pts_gamma, const int32_t* img_hw, const float* scale_xy,
+                           int nms_pre, int32_t* out_topk_idx, float* out_pts, float* out_scores, void* workspace,
+                           uint64_t workspace_bytes, void* stream) {
+  const char* name = SOFTMAX ? "ptb_p2p_decode_topk_softmax" : "ptb_p2p_decode_topk";
+  char what[64];
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && num_classes > 0 && k > 0, "shape");
   PTB_REQUIRE(cls_map && reg_map && point_anchor && img_hw && out_topk_idx && out_pts && out_scores, "NULL input");
   const int Q = H * W * k;
@@ -297,16 +395,39 @@ extern "C" int ptb_p2p_decode_topk(const float* cls_map, const float* reg_map, i
     PTB_REQUIRE(workspace && workspace_bytes >= ptb_p2p_decode_topk_workspace(B, H, W, k), "workspace too small");
     float* key = reinterpret_cast<float*>(workspace);
     const long long BQ = (long long)B * Q;
-    p2p_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, k, num_classes, key);
-    if ((rc = check_launch("ptb_p2p_decode_topk/score"))) return rc;
+    if (SOFTMAX)
+      p2p_softmax_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, num_classes, key);
+    else
+      p2p_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, k, num_classes, key);
+    snprintf(what, sizeof(what), "%s/score", name);
+    if ((rc = check_launch(what))) return rc;
     p2p_select_kernel<<<B, SEL_THREADS, 0, st>>>(key, Q, P, out_topk_idx, P);
-    if ((rc = check_launch("ptb_p2p_decode_topk/select"))) return rc;
+    snprintf(what, sizeof(what), "%s/select", name);
+    if ((rc = check_launch(what))) return rc;
   }
   const long long BP = (long long)B * P;
-  p2p_gather_kernel<<<(unsigned)((BP * 32 + 255) / 256), 256, 0, st>>>(cls_map, reg_map, H, W, num_classes, k, point_anchor,
-                                                                     stride, pts_gamma, img_hw, scale_xy, P, identity ? 1 : 0,
-                                                                     out_topk_idx, out_topk_idx, out_pts, out_scores, BP);
-  return check_launch("ptb_p2p_decode_topk/gather");
+  p2p_gather_kernel<SOFTMAX><<<(unsigned)((BP * 32 + 255) / 256), 256, 0, st>>>(cls_map, reg_map, H, W, num_classes, k,
+                                                                              point_anchor, stride, pts_gamma, img_hw, scale_xy, P,
+                                                                              identity ? 1 : 0, out_topk_idx, out_topk_idx, out_pts,
+                                                                              out_scores, BP);
+  snprintf(what, sizeof(what), "%s/gather", name);
+  return check_launch(what);
+}
+
+extern "C" int ptb_p2p_decode_topk(const float* cls_map, const float* reg_map, int B, int H, int W, int num_classes, int k,
+                                   const float* point_anchor, float stride, float pts_gamma, const int32_t* img_hw,
+                                   const float* scale_xy, int nms_pre, int32_t* out_topk_idx, float* out_pts, float* out_scores,
+                                   void* workspace, uint64_t workspace_bytes, void* stream) {
+  return p2p_decode_topk<false>(cls_map, reg_map, B, H, W, num_classes, k, point_anchor, stride, pts_gamma, img_hw, scale_xy,
+                                nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ptb_p2p_decode_topk_softmax(const float* cls_map, const float* reg_map, int B, int H, int W, int num_classes, int k,
+                                           const float* point_anchor, float stride, float pts_gamma, const int32_t* img_hw,
+                                           const float* scale_xy, int nms_pre, int32_t* out_topk_idx, float* out_pts,
+                                           float* out_scores, void* workspace, uint64_t workspace_bytes, void* stream) {
+  return p2p_decode_topk<true>(cls_map, reg_map, B, H, W, num_classes, k, point_anchor, stride, pts_gamma, img_hw, scale_xy,
+                               nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
 }
 
 extern "C" int ptb_p2p_cost_matrix(const float* cls_logits, const float* pts, int ldp, const int32_t* row_idx, int n_rows,
@@ -385,9 +506,37 @@ extern "C" int ptb_sigmoid_bce_fwd_bwd(const float* logits, const int64_t* label
   PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
   StreamScratch* scr = stream_scratch(stream);
   if (!scr) return 1;
-  sigmoid_bce_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, M, num_classes, loss_sum, scale, grad,
-                                                                   &scr->bce);
+  sigmoid_bce_kernel<false><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, nullptr, M, num_classes, loss_sum,
+                                                                          scale, grad, &scr->bce);
   return check_launch("ptb_sigmoid_bce_fwd_bwd");
+}
+
+extern "C" int ptb_sigmoid_bce_cw_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, const float* pos_weight,
+                                          int64_t M, int num_classes, float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0 && num_classes > 0, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
+  StreamScratch* scr = stream_scratch(stream);
+  if (!scr) return 1;
+  if (pos_weight)
+    sigmoid_bce_kernel<true><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, pos_weight, M, num_classes,
+                                                                           loss_sum, scale, grad, &scr->bce_pw);
+  else
+    sigmoid_bce_kernel<false><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, nullptr, M, num_classes,
+                                                                            loss_sum, scale, grad, &scr->bce_pw);
+  return check_launch("ptb_sigmoid_bce_cw_fwd_bwd");
+}
+
+extern "C" int ptb_softmax_ce_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, const float* class_weight,
+                                      int64_t M, int num_cols, float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0 && num_cols >= 2, "shape (softmax needs at least two columns)");
+  if (M == 0) return 0;
+  PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
+  StreamScratch* scr = stream_scratch(stream);
+  if (!scr) return 1;
+  softmax_ce_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, class_weight, M, num_cols, loss_sum, scale,
+                                                                  grad, &scr->ce);
+  return check_launch("ptb_softmax_ce_fwd_bwd");
 }
 
 extern "C" int ptb_mse_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, float inv_norm,

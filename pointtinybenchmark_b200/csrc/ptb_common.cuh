@@ -52,7 +52,7 @@ struct SumScratch {
 struct StreamScratch {
   unsigned int gather_ticket, gather_done;       // bag_gather chunk scheduler
   unsigned int ticket2, done2;                   // second scheduler (fused training gather)
-  SumScratch gfocal, focal, sl1, bce, mse;
+  SumScratch gfocal, focal, sl1, bce, mse, ce, bce_pw;
   unsigned int spare[60];
 };
 StreamScratch* stream_scratch(void* stream);     // NULL on failure (g_err set)

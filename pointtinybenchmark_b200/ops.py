@@ -424,6 +424,29 @@ def p2p_decode_topk(cls_map, reg_map, num_classes, k, point_anchor, stride, pts_
     return idx, pts, sc
 
 
+def p2p_decode_topk_softmax(cls_map, reg_map, num_classes, k, point_anchor, stride, pts_gamma, img_hw, nms_pre, scale_xy=None):
+    """ptb_p2p_decode_topk_softmax. cls_map (B,H,W,k*(C+1)) logits with the background column last, reg_map (B,H,W,2k).
+    returns topk_idx (B,P) int32, pts (B,P,2), scores (B,P,C) = the foreground softmax probabilities."""
+    lib = _lib.load()
+    _chk(cls_map, torch.float32, 'cls_map'); _chk(reg_map, torch.float32, 'reg_map'); _chk(point_anchor, torch.float32, 'anchor')
+    _chk(img_hw, torch.int32, 'img_hw')
+    B, H, W, ch = cls_map.shape
+    if ch != k * (num_classes + 1):
+        raise ValueError(f'cls_map has {ch} channels; softmax scores need k * (num_classes + 1) = {k * (num_classes + 1)}')
+    Q = H * W * k
+    P = nms_pre if 0 < nms_pre < Q else Q
+    dev = cls_map.device
+    idx = torch.empty((B, P), dtype=torch.int32, device=dev)
+    pts = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
+    sc = torch.empty((B, P, num_classes), dtype=torch.float32, device=dev)
+    nbytes = lib.ptb_p2p_decode_topk_workspace(B, H, W, k)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    check(lib.ptb_p2p_decode_topk_softmax(_ptr(cls_map), _ptr(reg_map), B, H, W, num_classes, k, _ptr(point_anchor), float(stride),
+                                          float(pts_gamma), _ptr(img_hw), _ptr(scale_xy), int(nms_pre), _ptr(idx), _ptr(pts), _ptr(sc),
+                                          _ptr(ws), nbytes, _stream()), 'ptb_p2p_decode_topk_softmax')
+    return idx, pts, sc
+
+
 def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img):
     """ptb_multiclass_nms. pts (B,P,2), scores (B,P,C) -> count (B,), det (B,max,5), label (B,max), keep (B,max), cand_count (B,)"""
     lib = _lib.load()
@@ -658,16 +681,42 @@ def smooth_l1(pred, target, weight, inv_norm, beta, scale=None, want_grad=False)
     return grad if want_grad else loss
 
 
-def sigmoid_bce(logits, labels, weight, scale=None, want_grad=False):
-    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels)) * weight[m] (labels == C: background row);
-    optional grad = scale * d/dlogits."""
+def sigmoid_bce(logits, labels, weight, scale=None, want_grad=False, pos_weight=None):
+    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels), pos_weight) * weight[m] (labels == C: background row);
+    optional grad = scale * d/dlogits.  pos_weight (C,) = CrossEntropyLoss.class_weight in sigmoid mode."""
     lib = _lib.load()
     _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels')
     M, C = logits.shape
     loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
     grad = torch.empty_like(logits) if want_grad else None
-    check(lib.ptb_sigmoid_bce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), M, C, _ptr(loss) if not want_grad else None,
-                                      _ptr(scale), _ptr(grad), _stream()), 'ptb_sigmoid_bce_fwd_bwd')
+    if pos_weight is None:
+        check(lib.ptb_sigmoid_bce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), M, C, _ptr(loss) if not want_grad else None,
+                                          _ptr(scale), _ptr(grad), _stream()), 'ptb_sigmoid_bce_fwd_bwd')
+        return grad if want_grad else loss
+    _chk(pos_weight, torch.float32, 'pos_weight')
+    if pos_weight.shape != (C,):
+        raise ValueError(f'pos_weight must have shape ({C},), got {tuple(pos_weight.shape)}')
+    check(lib.ptb_sigmoid_bce_cw_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), _ptr(pos_weight), M, C,
+                                         _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
+          'ptb_sigmoid_bce_cw_fwd_bwd')
+    return grad if want_grad else loss
+
+
+def softmax_ce(logits, labels, weight, class_weight=None, scale=None, want_grad=False):
+    """sum_m cross_entropy(logits[m], labels[m], weight=class_weight) * weight[m] over rows of C+1 logits (label C: background);
+    optional grad = scale * d/dlogits."""
+    lib = _lib.load()
+    _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels')
+    M, C1 = logits.shape
+    if class_weight is not None:
+        _chk(class_weight, torch.float32, 'class_weight')
+        if class_weight.shape != (C1,):
+            raise ValueError(f'class_weight must have shape ({C1},), got {tuple(class_weight.shape)}')
+    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
+    grad = torch.empty_like(logits) if want_grad else None
+    check(lib.ptb_softmax_ce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), _ptr(class_weight), M, C1,
+                                     _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
+          'ptb_softmax_ce_fwd_bwd')
     return grad if want_grad else loss
 
 

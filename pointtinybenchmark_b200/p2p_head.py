@@ -9,8 +9,10 @@ What runs where: towers and the two output convs = wgmma implicit GEMMs of libpt
 towers use the tensor-core autograd function of layers.py (dgrad / wgrad / GroupNorm backward kernels) and the two narrow output
 convs cuDNN fp32; decode, top-k, NMS / soft-NMS, cost matrix, the Hungarian matching (scipy's shortest-augmenting-path algorithm
 restated as a one-CTA-per-image kernel, bit-identical assignments incl. ties: csrc/lsap_core.cuh; SURVEY.md §8f rank 2) and the
-losses = libptb_b200.so: FocalLoss or the reference's default CrossEntropyLoss(use_sigmoid=True) for classification,
-SmoothL1Loss or the default MSELoss for the points.  Nothing of the training step returns to the host except one (B,) status read.
+losses = libptb_b200.so: FocalLoss or the reference's default CrossEntropyLoss(use_sigmoid=True) for classification, the latter
+also with class_weight (= pos_weight) or in softmax mode (use_sigmoid=False: C+1 outputs per anchor, background last, softmax decode
+and cross-entropy kernels), SmoothL1Loss or the default MSELoss for the points.  Nothing of the training step returns to the host
+except one (B,) status read.
 """
 import numpy as np
 import torch
@@ -47,18 +49,35 @@ class _FocalSumFn(torch.autograd.Function):
 
 
 class _SigmoidBCESumFn(torch.autograd.Function):
-    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels)) * weight[m]   (losses/cross_entropy_loss.py:42-89)"""
+    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels), pos_weight=class_weight) * weight[m]
+    (losses/cross_entropy_loss.py:42-89)"""
 
     @staticmethod
-    def forward(ctx, logits, labels, weight):
-        ctx.save_for_backward(logits, labels, weight)
-        return ops.sigmoid_bce(logits, labels, weight)[0]
+    def forward(ctx, logits, labels, weight, pos_weight=None):
+        ctx.save_for_backward(logits, labels, weight, pos_weight)
+        return ops.sigmoid_bce(logits, labels, weight, pos_weight=pos_weight)[0]
 
     @staticmethod
     def backward(ctx, g):
-        logits, labels, weight = ctx.saved_tensors
+        logits, labels, weight, pos_weight = ctx.saved_tensors
         scale = g.reshape(1).float().contiguous()
-        return ops.sigmoid_bce(logits, labels, weight, scale=scale, want_grad=True), None, None
+        return ops.sigmoid_bce(logits, labels, weight, scale=scale, want_grad=True, pos_weight=pos_weight), None, None, None
+
+
+class _SoftmaxCESumFn(torch.autograd.Function):
+    """sum_m cross_entropy(logits[m], labels[m], weight=class_weight) * weight[m] over C+1 columns
+    (losses/cross_entropy_loss.py:9-39, use_sigmoid=False)"""
+
+    @staticmethod
+    def forward(ctx, logits, labels, weight, class_weight=None):
+        ctx.save_for_backward(logits, labels, weight, class_weight)
+        return ops.softmax_ce(logits, labels, weight, class_weight)[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        logits, labels, weight, class_weight = ctx.saved_tensors
+        scale = g.reshape(1).float().contiguous()
+        return ops.softmax_ce(logits, labels, weight, class_weight, scale=scale, want_grad=True), None, None, None
 
 
 class _MSESumFn(torch.autograd.Function):
@@ -123,9 +142,16 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         self.test_cfg = CfgNode(test_cfg) if test_cfg is not None else None
         if len(self.strides) != 1:
             raise NotImplementedError('P2PHead: one FPN level only (all configs2/*/p2p configs use strides=[s])')
-        if not self.loss_cls_cfg.get('use_sigmoid', False):
-            raise NotImplementedError('P2PHead: softmax classification')
-        self.num_cls_out = num_classes
+        # p2p_head.py:63-67: sigmoid scores C classes, softmax C + 1 with the background column last
+        self.use_sigmoid_cls = bool(self.loss_cls_cfg.get('use_sigmoid', False))
+        if not self.use_sigmoid_cls and self.loss_cls_cfg['type'] == 'FocalLoss':
+            raise NotImplementedError('P2PHead: FocalLoss supports sigmoid classification only (use_sigmoid=True)')
+        self.num_cls_out = num_classes if self.use_sigmoid_cls else num_classes + 1
+        cw = self.loss_cls_cfg.get('class_weight') if self.loss_cls_cfg['type'] == 'CrossEntropyLoss' else None
+        if cw is not None and len(cw) != self.num_cls_out:
+            raise ValueError(f'P2PHead: CrossEntropyLoss.class_weight has {len(cw)} entries; '
+                             f'{"sigmoid" if self.use_sigmoid_cls else "softmax"} classification needs {self.num_cls_out}')
+        self.class_weight = None if cw is None else torch.tensor([float(v) for v in cw], dtype=torch.float32)
         if max(self.num_cls_out * self.num_points, 2 * self.num_points) > MAX_OUT_CHANNELS:
             raise NotImplementedError(
                 f'P2PHead: cls_out would have {self.num_cls_out} classes x {self.num_points} anchors = '
@@ -295,16 +321,17 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         cls_type, reg_type = self.loss_cls_cfg['type'], self.loss_reg_cfg['type']
         if cls_type not in LOSS_CLS_TYPES or reg_type not in LOSS_REG_TYPES:
             raise NotImplementedError(f'P2PHead: loss_cls must be one of {LOSS_CLS_TYPES} and loss_reg one of {LOSS_REG_TYPES}')
-        if cls_type == 'CrossEntropyLoss' and self.loss_cls_cfg.get('class_weight') is not None:
-            raise NotImplementedError('P2PHead: CrossEntropyLoss with class_weight')
         gamma, alpha = self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25)
         # loss_single (p2p_head.py:220-231): CrossEntropyLoss averages over every proposal of the batch, FocalLoss over the positives
         cls_avg = float(B * Q) if cls_type == 'CrossEntropyLoss' else num_total_pos
         inv_norm = 1.0 / (s * self.reg_norm)
+        cw = self.class_weight.to(dev) if self.class_weight is not None else None
         loss_cls, loss_pts = [], []
         for b in range(B):
-            if cls_type == 'CrossEntropyLoss':
-                lc = _SigmoidBCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b])
+            if cls_type == 'CrossEntropyLoss' and not self.use_sigmoid_cls:
+                lc = _SoftmaxCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], cw)
+            elif cls_type == 'CrossEntropyLoss':
+                lc = _SigmoidBCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], cw)
             else:
                 lc = _FocalSumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], gamma, alpha)
             loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / cls_avg)
@@ -333,8 +360,10 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         if rescale:
             scale_xy = torch.tensor(np.array([m['scale_factor'][:2] for m in img_metas], dtype=np.float32), device=dev)
         cmap, rmap = ops.to_nhwc(cls_out).contiguous(), ops.to_nhwc(pts_out).contiguous()
-        idx, pts, scores = ops.p2p_decode_topk(cmap, rmap, self.num_cls_out, self.num_points, self.point_anchor.to(dev),
-                                               self.strides[0], self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
+        # p2p_head.py:363-372: sigmoid scores, or the softmax over C+1 columns of which NMS sees the C foreground ones
+        decode = ops.p2p_decode_topk if self.use_sigmoid_cls else ops.p2p_decode_topk_softmax
+        idx, pts, scores = decode(cmap, rmap, self.num_classes, self.num_points, self.point_anchor.to(dev), self.strides[0],
+                                  self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
         wh = cfg.get('pseudo_wh', (16, 16))
         nms = cfg.get('nms')
         if nms.get('type', 'nms') == 'soft_nms':       # batched_nms dispatches on nms_cfg['type'] (mmcv/ops/nms.py)
@@ -395,8 +424,12 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             aug_scores.append(sc)
         boxes = torch.cat(aug_bboxes).contiguous()
         scores = torch.cat(aug_scores).contiguous()
+        if not self.use_sigmoid_cls:
+            # p2p_head.py:549-556: the reference pads a background column only in sigmoid mode, so in softmax mode
+            # multiclass_nms takes the last real class (C-1) for the background and drops it from the merged detections
+            scores = scores[:, :-1].contiguous()
         cfg = self.test_cfg
-        if boxes.shape[0] == 0:
+        if boxes.shape[0] == 0 or scores.shape[1] == 0:
             return [(boxes.new_zeros((0, 5)), boxes.new_zeros((0,), dtype=torch.long))]
         nms = cfg.get('nms')
         if nms.get('type', 'nms') == 'soft_nms':

@@ -5,9 +5,12 @@ CrossEntropyLoss(use_sigmoid=True) + MSELoss) at the BASELINE.json configs[2] sh
   p2p_defaults_train_ms   with --train: forward_train + backward per 16 images, 20 GT points per image, HungarianAssignerV2 topk_k 5.
                           At 67 200 rows the matching is past the cluster kernel's 17 600-column limit and runs its one-CTA
                           global-memory path (lsap.cu).
+  p2p_softmax_infer_ms    with --softmax: the same head with CrossEntropyLoss(use_sigmoid=False): 4 anchors x 81 outputs (80 classes +
+                          background) = 324-channel cls_out, softmax decode / top-k
+  p2p_softmax_train_ms    with --softmax --train: its training step (softmax cross-entropy kernel)
 CUDA events, L2 flushed (256 MB write) before every timed call, mean over the timed calls.  Writes nothing.
 
-    python tools/bench_p2p_defaults.py [--train] [--iters N]
+    python tools/bench_p2p_defaults.py [--train] [--softmax] [--iters N]
 """
 import argparse
 import json
@@ -34,6 +37,7 @@ TEST_CFG = dict(nms_pre=1000, min_bbox_size=0, score_thr=0.05, pseudo_wh=(32, 32
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--train', action='store_true', help='also time the training step')
+    ap.add_argument('--softmax', action='store_true', help='also time the head with softmax classification (4 anchors x 81 outputs)')
     ap.add_argument('--iters', type=int, default=5)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -59,26 +63,32 @@ def main():
     out = dict(workload=f'P2PHead reference defaults (4 anchors / cell, cls_out {4 * NCLS} ch), {B} x ({C}x{H}x{W}), '
                         f'{H * W * 4} proposals per image, random-init weights',
                device=torch.cuda.get_device_name(dev))
-    head = build_head(cfg).to(dev).eval()
-    with torch.no_grad():
-        out['p2p_defaults_infer_ms'] = ktime(lambda: head.simple_test((x,), metas), args.iters)
-    out['tower_backend'] = head.last_tower_backend
-    del head
-    if args.train:
-        head = build_head(dict(cfg, train_cfg=TRAIN_CFG)).to(dev).train()
-        g = torch.Generator().manual_seed(13)
-        gtb, gtl = [], []
-        for _ in range(B):
-            cxy = torch.rand(20, 2, generator=g) * torch.tensor([1300., 780.]) + 10
-            gtb.append(torch.cat([cxy - 8, cxy + 8], 1).to(dev))
-        gtl = [torch.randint(0, NCLS, (20,), generator=g).to(dev) for _ in range(B)]
-        xt = x.clone().requires_grad_(True)
+    g = torch.Generator().manual_seed(13)
+    gtb = []
+    for _ in range(B):
+        cxy = torch.rand(20, 2, generator=g) * torch.tensor([1300., 780.]) + 10
+        gtb.append(torch.cat([cxy - 8, cxy + 8], 1).to(dev))
+    gtl = [torch.randint(0, NCLS, (20,), generator=g).to(dev) for _ in range(B)]
 
-        def step():
-            head.zero_grad(set_to_none=True)
-            ls = head.forward_train((xt,), metas, gtb, gtl)
-            (sum(ls['loss_cls']) + sum(ls['loss_pts'])).backward()
-        out['p2p_defaults_train_ms'] = ktime(step, max(1, args.iters // 2 + 1))
+    def run(prefix, hcfg):
+        head = build_head(hcfg).to(dev).eval()
+        with torch.no_grad():
+            out[f'{prefix}_infer_ms'] = ktime(lambda: head.simple_test((x,), metas), args.iters)
+        out['tower_backend'] = head.last_tower_backend
+        del head
+        if args.train:
+            head = build_head(dict(hcfg, train_cfg=TRAIN_CFG)).to(dev).train()
+            xt = x.clone().requires_grad_(True)
+
+            def step():
+                head.zero_grad(set_to_none=True)
+                ls = head.forward_train((xt,), metas, gtb, gtl)
+                (sum(ls['loss_cls']) + sum(ls['loss_pts'])).backward()
+            out[f'{prefix}_train_ms'] = ktime(step, max(1, args.iters // 2 + 1))
+
+    run('p2p_defaults', cfg)
+    if args.softmax:
+        run('p2p_softmax', dict(cfg, loss_cls=dict(type='CrossEntropyLoss', use_sigmoid=False, loss_weight=1.0)))
     print(json.dumps(out))
 
 
