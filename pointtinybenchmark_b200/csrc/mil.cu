@@ -327,8 +327,6 @@ __global__ void __launch_bounds__(1024) mil_finish_kernel(const float* __restric
 // ------------------------------------------------------------------------------------------------
 // gfocal on sigmoid(logits) with weights; fixed grid + last-block reduction (deterministic sum)
 // ------------------------------------------------------------------------------------------------
-constexpr int GF_BLOCKS = SCRATCH_BLOCKS;   // 4 x 132; partials + "last block" counter live in the per-stream scratch block
-
 __device__ __forceinline__ float load_w(const void* weight, int wmode, long long m, int c, int C) {
   if (!weight) return 1.f;
   if (wmode == 0) return (float)reinterpret_cast<const uint8_t*>(weight)[m * C + c];
@@ -341,7 +339,7 @@ gfocal_fwd_kernel(const float* __restrict__ logits, long long M, int C, long lon
   const long long total = M * C;
   float acc = 0.f;
   // (row, column) advanced incrementally: the 64-bit division per element cost more than the loss itself
-  const long long step = (long long)GF_BLOCKS * 256;
+  const long long step = (long long)SCRATCH_BLOCKS * 256;      // launch_sum's grid
   const long long step_m = step / C;
   const int step_c = (int)(step - step_m * C);
   long long i = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -356,26 +354,7 @@ gfocal_fwd_kernel(const float* __restrict__ logits, long long M, int C, long lon
       acc += gfocal_elem(p, q, eps) * w;
     }
   }
-  __shared__ float red[8];
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  __shared__ bool last;
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += red[w];
-    scr->partials[blockIdx.x] = t;
-    __threadfence();
-    last = (atomicAdd(&scr->done, 1u) == GF_BLOCKS - 1);
-  }
-  __syncthreads();
-  if (last && threadIdx.x == 0) {
-    __threadfence();
-    float t = 0.f;
-    for (int b = 0; b < GF_BLOCKS; ++b) t += reinterpret_cast<volatile float*>(scr->partials)[b];
-    loss_sum[0] += t;
-    scr->done = 0;
-  }
+  block_partial_finish(acc, *scr, loss_sum);
 }
 
 __global__ void __launch_bounds__(256)
@@ -448,11 +427,8 @@ extern "C" int ptb_gfocal_sigmoid_fwd(const float* logits, int64_t M, int num_cl
   PTB_REQUIRE(wmode == 0 || wmode == 1, "wmode");
   if (M == 0) return 0;
   PTB_REQUIRE(logits && loss_sum, "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  gfocal_fwd_kernel<<<GF_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, M, num_classes, row_stride, target_label, weight, wmode,
-                                                               eps, loss_sum, &scr->gfocal);
-  return check_launch("ptb_gfocal_sigmoid_fwd");
+  return launch_sum(gfocal_fwd_kernel, stream, "ptb_gfocal_sigmoid_fwd", logits, M, num_classes, row_stride, target_label, weight,
+                    wmode, eps, loss_sum);
 }
 
 extern "C" int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,

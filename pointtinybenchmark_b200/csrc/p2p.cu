@@ -10,39 +10,11 @@
 namespace ptb {
 
 // ------------------------------------------------------------------------------------------------
-// deterministic sum helper: fixed grid, per-block partial, last block adds them in index order
-// ------------------------------------------------------------------------------------------------
-constexpr int SUM_BLOCKS = SCRATCH_BLOCKS;      // partials + counter: per-stream scratch block (ptb_common.cuh), not file-scope globals
-
-__device__ __forceinline__ void block_partial_finish(float acc, SumScratch& sc, float* out) {
-  __shared__ float red[32];
-  __shared__ bool last;
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-    sc.partials[blockIdx.x] = t;
-    __threadfence();
-    last = (atomicAdd(&sc.done, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (last && threadIdx.x == 0) {
-    __threadfence();
-    float t = 0.f;
-    for (int b = 0; b < (int)gridDim.x; ++b) t += reinterpret_cast<volatile float*>(sc.partials)[b];
-    out[0] += t;
-    sc.done = 0;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // decode + top-k
 // ------------------------------------------------------------------------------------------------
 // key[b][q] = max_c sigmoid(cls[b][cell][a*C + c]),  q = cell*k + a.   One warp per proposal.
 __global__ void __launch_bounds__(256)
-p2p_score_kernel(const float* __restrict__ cls_map, long long BQ, int k, int C, float* __restrict__ key) {
+p2p_score_kernel(const float* __restrict__ cls_map, long long BQ, int C, float* __restrict__ key) {
   const long long wq = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (wq >= BQ) return;
@@ -51,7 +23,6 @@ p2p_score_kernel(const float* __restrict__ cls_map, long long BQ, int k, int C, 
   for (int c = lane; c < C; c += 32) mx = fmaxf(mx, sigmoidf_acc(row[c]));
   mx = warp_max(mx);
   if (lane == 0) key[wq] = mx;
-  (void)k;
 }
 
 // Softmax over one row of C1 logits (background last), by one warp: m = max_c x_c, s = sum_c exp(x_c - m) (lane-strided partial
@@ -227,16 +198,25 @@ __global__ void pa_finish_kernel(const unsigned long long* __restrict__ best, in
 }
 
 // ------------------------------------------------------------------------------------------------
-// elementwise losses with sums
+// losses with fused forward / backward and a fixed-order sum
 // ------------------------------------------------------------------------------------------------
+// An elementwise loss is a functor over element e:  op(e, want_loss, grad, sc) returns e's term of the loss sum (read only when
+// want_loss) and, when grad is set, stores grad[e] = sc * d term / dx[e].  The kernel owns the loop and the sum.
+template <class Loss>
 __global__ void __launch_bounds__(256)
-focal_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight, long long M,
-             int C, float gamma, float alpha, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad,
-             SumScratch* __restrict__ scr) {
-  const long long total = M * C;
+loss_sum_kernel(Loss op, long long n, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad,
+                SumScratch* __restrict__ scr) {
   const float sc = (grad && scale) ? scale[0] : 1.f;
   float acc = 0.f;
-  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256) {
+  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < n; e += (long long)gridDim.x * 256)
+    acc += op(e, loss_sum != nullptr, grad, sc);
+  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
+}
+
+// FocalLoss (focal_loss.py:11-56) over M x C logits, the per-proposal weight broadcast over the classes
+struct FocalLoss {
+  const float* x; const int64_t* labels; const float* weight; int C; float gamma, alpha;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
     const long long m = e / C;
     const int c = (int)(e - m * C);
     const float w = weight ? weight[m] : 1.f;
@@ -247,31 +227,26 @@ focal_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, co
     const float a = alpha * t + (1.f - alpha) * (1.f - t);
     const float ptg = (gamma == 2.f) ? pt * pt : powf(pt, gamma);
     const float bce = fmaxf(v, 0.f) - v * t + log1pf(expf(-fabsf(v)));
-    acc += bce * (a * ptg) * w;
     if (grad) {
       const float dpt = (t > 0.5f ? -1.f : 1.f) * p * (1.f - p);
       const float ptg1 = (gamma == 2.f) ? 2.f * pt : gamma * powf(pt, gamma - 1.f);
       grad[e] = sc * w * a * (ptg1 * dpt * bce + ptg * (p - t));
     }
+    return bce * (a * ptg) * w;
   }
-  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
-}
+};
 
-__global__ void __launch_bounds__(256)
-smooth_l1_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ weight, long long n,
-                 float inv_norm, float beta, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad,
-                 SumScratch* __restrict__ scr) {
-  const float sc = (grad && scale) ? scale[0] : 1.f;
-  float acc = 0.f;
-  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < n; e += (long long)gridDim.x * 256) {
+// SmoothL1Loss (smooth_l1_loss.py:25-31) on the normalised points
+struct SmoothL1Loss {
+  const float* pred; const float* target; const float* weight; float inv_norm, beta;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
     const float w = weight ? weight[e] : 1.f;
     const float diff = (pred[e] - target[e]) * inv_norm;
     const float d = fabsf(diff);
-    acc += (d < beta ? 0.5f * d * d / beta : d - 0.5f * beta) * w;
     if (grad) grad[e] = sc * w * inv_norm * (d < beta ? diff / beta : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f)));
+    return (d < beta ? 0.5f * d * d / beta : d - 0.5f * beta) * w;
   }
-  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
-}
+};
 
 // CrossEntropyLoss(use_sigmoid=True) = binary_cross_entropy (cross_entropy_loss.py:42-89): labels expanded to one-hot rows
 // (_expand_onehot_labels; a label outside [0, C), e.g. the background label C, is an all-zero row), the per-proposal weight
@@ -280,42 +255,50 @@ smooth_l1_kernel(const float* __restrict__ pred, const float* __restrict__ targe
 // then the weighted sum of weight_reduce_loss (the caller divides by avg_factor).  d/dx = sigmoid(x) - t.
 // POS_WEIGHT: CrossEntropyLoss.class_weight, which binary_cross_entropy passes as pos_weight (cross_entropy_loss.py:85-86), in
 // ATen's CPU order: log_weight = (pw_c - 1) * t + 1, loss = (1 - t) * x - log_sigmoid(x) * log_weight; d/dx = (pw_c t + 1 - t)
-// sigmoid(x) - pw_c t (binary_cross_entropy_with_logits_backward).  Without it the kernel is the class_weight=None form above.
+// sigmoid(x) - pw_c t (binary_cross_entropy_with_logits_backward).  Without it this is the class_weight=None form above.
+// The log is computed only when the sum is wanted: the backward launch skips it.
 template <bool POS_WEIGHT>
-__global__ void __launch_bounds__(256)
-sigmoid_bce_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, const float* __restrict__ weight,
-                   const float* __restrict__ pos_weight, long long M, int C, float* loss_sum, const float* __restrict__ scale,
-                   float* __restrict__ grad, SumScratch* __restrict__ scr) {
-  const long long total = M * C;
-  const float sc = (grad && scale) ? scale[0] : 1.f;
-  float acc = 0.f;
-  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256) {
+struct SigmoidBCELoss {
+  const float* x; const int64_t* labels; const float* weight; const float* pos_weight; int C;
+  __device__ __forceinline__ float operator()(long long e, bool want_loss, float* grad, float sc) const {
     const long long m = e / C;
     const int c = (int)(e - m * C);
     const float w = weight ? weight[m] : 1.f;
     const float t = (labels[m] == c) ? 1.f : 0.f;
     const float v = x[e];
+    float term = 0.f;
     if constexpr (POS_WEIGHT) {
       const float pw = pos_weight[c];
-      if (loss_sum) {
+      if (want_loss) {
         const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
         const float log_w = __fadd_rn(__fmul_rn(__fsub_rn(pw, 1.f), t), 1.f);
-        acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), __fmul_rn(log_sig, log_w)), w);
+        term = __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), __fmul_rn(log_sig, log_w)), w);
       }
       if (grad) {
         const float pt = __fmul_rn(pw, t);
         grad[e] = sc * w * __fsub_rn(__fmul_rn(__fsub_rn(__fadd_rn(pt, 1.f), t), sigmoidf_acc(v)), pt);
       }
     } else {
-      if (loss_sum) {
+      if (want_loss) {
         const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
-        acc += __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
+        term = __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
       }
       if (grad) grad[e] = sc * w * (sigmoidf_acc(v) - t);
     }
+    return term;
   }
-  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
-}
+};
+
+// MSELoss (mse_loss.py:9-48): sum ((pred - target) * inv_norm)^2 * weight on the normalised points; d/dpred = 2 diff inv_norm w
+struct MSELoss {
+  const float* pred; const float* target; const float* weight; float inv_norm;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
+    const float w = weight ? weight[e] : 1.f;
+    const float diff = (pred[e] - target[e]) * inv_norm;
+    if (grad) grad[e] = sc * w * inv_norm * 2.f * diff;
+    return __fmul_rn(__fmul_rn(diff, diff), w);
+  }
+};
 
 // CrossEntropyLoss(use_sigmoid=False) = cross_entropy (cross_entropy_loss.py:9-39): F.cross_entropy(x, y, weight=class_weight,
 // reduction='none') over rows of C1 logits (background label C1-1 is an ordinary column), times the per-proposal weight, summed
@@ -352,21 +335,6 @@ softmax_ce_kernel(const float* __restrict__ x, const int64_t* __restrict__ label
   if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
 }
 
-// MSELoss (mse_loss.py:9-48): sum ((pred - target) * inv_norm)^2 * weight on the normalised points; d/dpred = 2 diff inv_norm w
-__global__ void __launch_bounds__(256)
-mse_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ weight, long long n,
-           float inv_norm, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad, SumScratch* __restrict__ scr) {
-  const float sc = (grad && scale) ? scale[0] : 1.f;
-  float acc = 0.f;
-  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < n; e += (long long)gridDim.x * 256) {
-    const float w = weight ? weight[e] : 1.f;
-    const float diff = (pred[e] - target[e]) * inv_norm;
-    acc += __fmul_rn(__fmul_rn(diff, diff), w);
-    if (grad) grad[e] = sc * w * inv_norm * 2.f * diff;
-  }
-  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
-}
-
 }  // namespace ptb
 
 using namespace ptb;
@@ -398,7 +366,7 @@ static int p2p_decode_topk(const float* cls_map, const float* reg_map, int B, in
     if (SOFTMAX)
       p2p_softmax_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, num_classes, key);
     else
-      p2p_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, k, num_classes, key);
+      p2p_score_kernel<<<(unsigned)((BQ * 32 + 255) / 256), 256, 0, st>>>(cls_map, BQ, num_classes, key);
     snprintf(what, sizeof(what), "%s/score", name);
     if ((rc = check_launch(what))) return rc;
     p2p_select_kernel<<<B, SEL_THREADS, 0, st>>>(key, Q, P, out_topk_idx, P);
@@ -480,11 +448,8 @@ extern "C" int ptb_sigmoid_focal_fwd_bwd(const float* logits, const int64_t* lab
   PTB_REQUIRE(M >= 0 && num_classes > 0, "shape");
   if (M == 0) return 0;
   PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  focal_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, M, num_classes, gamma, alpha, loss_sum, scale,
-                                                           grad, &scr->focal);
-  return check_launch("ptb_sigmoid_focal_fwd_bwd");
+  return launch_sum(loss_sum_kernel<FocalLoss>, stream, "ptb_sigmoid_focal_fwd_bwd",
+                    FocalLoss{logits, labels, weight, num_classes, gamma, alpha}, M * num_classes, loss_sum, scale, grad);
 }
 
 extern "C" int ptb_smooth_l1_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, float inv_norm,
@@ -492,23 +457,8 @@ extern "C" int ptb_smooth_l1_fwd_bwd(const float* pred, const float* target, con
   PTB_REQUIRE(M >= 0 && beta > 0.f, "shape");
   if (M == 0) return 0;
   PTB_REQUIRE(pred && target && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  smooth_l1_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(pred, target, weight, M * 2, inv_norm, beta, loss_sum, scale, grad,
-                                                               &scr->sl1);
-  return check_launch("ptb_smooth_l1_fwd_bwd");
-}
-
-extern "C" int ptb_sigmoid_bce_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, int64_t M, int num_classes,
-                                       float* loss_sum, const float* scale, float* grad, void* stream) {
-  PTB_REQUIRE(M >= 0 && num_classes > 0, "shape");
-  if (M == 0) return 0;
-  PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  sigmoid_bce_kernel<false><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, nullptr, M, num_classes, loss_sum,
-                                                                          scale, grad, &scr->bce);
-  return check_launch("ptb_sigmoid_bce_fwd_bwd");
+  return launch_sum(loss_sum_kernel<SmoothL1Loss>, stream, "ptb_smooth_l1_fwd_bwd", SmoothL1Loss{pred, target, weight, inv_norm, beta},
+                    M * 2, loss_sum, scale, grad);
 }
 
 extern "C" int ptb_sigmoid_bce_cw_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, const float* pos_weight,
@@ -516,15 +466,17 @@ extern "C" int ptb_sigmoid_bce_cw_fwd_bwd(const float* logits, const int64_t* la
   PTB_REQUIRE(M >= 0 && num_classes > 0, "shape");
   if (M == 0) return 0;
   PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
+  const char* name = "ptb_sigmoid_bce_cw_fwd_bwd";
   if (pos_weight)
-    sigmoid_bce_kernel<true><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, pos_weight, M, num_classes,
-                                                                           loss_sum, scale, grad, &scr->bce_pw);
-  else
-    sigmoid_bce_kernel<false><<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, nullptr, M, num_classes,
-                                                                            loss_sum, scale, grad, &scr->bce_pw);
-  return check_launch("ptb_sigmoid_bce_cw_fwd_bwd");
+    return launch_sum(loss_sum_kernel<SigmoidBCELoss<true>>, stream, name,
+                      SigmoidBCELoss<true>{logits, labels, weight, pos_weight, num_classes}, M * num_classes, loss_sum, scale, grad);
+  return launch_sum(loss_sum_kernel<SigmoidBCELoss<false>>, stream, name,
+                    SigmoidBCELoss<false>{logits, labels, weight, nullptr, num_classes}, M * num_classes, loss_sum, scale, grad);
+}
+
+extern "C" int ptb_sigmoid_bce_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, int64_t M, int num_classes,
+                                       float* loss_sum, const float* scale, float* grad, void* stream) {
+  return ptb_sigmoid_bce_cw_fwd_bwd(logits, labels, weight, nullptr, M, num_classes, loss_sum, scale, grad, stream);
 }
 
 extern "C" int ptb_softmax_ce_fwd_bwd(const float* logits, const int64_t* labels, const float* weight, const float* class_weight,
@@ -532,11 +484,8 @@ extern "C" int ptb_softmax_ce_fwd_bwd(const float* logits, const int64_t* labels
   PTB_REQUIRE(M >= 0 && num_cols >= 2, "shape (softmax needs at least two columns)");
   if (M == 0) return 0;
   PTB_REQUIRE(logits && labels && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  softmax_ce_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(logits, labels, weight, class_weight, M, num_cols, loss_sum, scale,
-                                                                  grad, &scr->ce);
-  return check_launch("ptb_softmax_ce_fwd_bwd");
+  return launch_sum(softmax_ce_kernel, stream, "ptb_softmax_ce_fwd_bwd", logits, labels, weight, class_weight, M, num_cols, loss_sum,
+                    scale, grad);
 }
 
 extern "C" int ptb_mse_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, float inv_norm,
@@ -544,8 +493,6 @@ extern "C" int ptb_mse_fwd_bwd(const float* pred, const float* target, const flo
   PTB_REQUIRE(M >= 0, "shape");
   if (M == 0) return 0;
   PTB_REQUIRE(pred && target && (loss_sum || grad), "NULL input");
-  StreamScratch* scr = stream_scratch(stream);
-  if (!scr) return 1;
-  mse_kernel<<<SUM_BLOCKS, 256, 0, (cudaStream_t)stream>>>(pred, target, weight, M * 2, inv_norm, loss_sum, scale, grad, &scr->mse);
-  return check_launch("ptb_mse_fwd_bwd");
+  return launch_sum(loss_sum_kernel<MSELoss>, stream, "ptb_mse_fwd_bwd", MSELoss{pred, target, weight, inv_norm}, M * 2, loss_sum,
+                    scale, grad);
 }

@@ -40,9 +40,10 @@ inline int check_launch(const char* what) {
 
 // ---------------------------------------------------------------------------------------------
 // per-(device, stream) scratch: self-resetting scheduler tickets / "last block" counters and block partials of the fixed-order
-// reductions.  Launches on ONE stream are serialised, so a scratch block per stream makes the counters race-free for
-// concurrent launches on different streams (round 1 kept them in file-scope __device__ globals).  Allocated lazily
-// (cudaMalloc + memset, once per stream) by capi.cu; ptb_reset_stream_state() zeroes it after an aborted launch.
+// reductions.  Launches on ONE stream are serialised, and the last block of every fixed-order sum resets `done` before its
+// kernel ends, so one SumScratch serves every sum kernel of the stream; a block per stream keeps concurrent launches on
+// different streams apart.  Allocated lazily (cudaMalloc + memset, once per stream) by capi.cu; ptb_reset_stream_state()
+// zeroes it after an aborted launch.
 // ---------------------------------------------------------------------------------------------
 constexpr int SCRATCH_BLOCKS = 528;      // 4 x 132 (H100 SMs): grid of the fixed-order sum kernels
 struct SumScratch {
@@ -51,8 +52,7 @@ struct SumScratch {
 };
 struct StreamScratch {
   unsigned int gather_ticket, gather_done;       // bag_gather chunk scheduler
-  unsigned int ticket2, done2;                   // second scheduler (fused training gather)
-  SumScratch gfocal, focal, sl1, bce, mse, ce, bce_pw;
+  SumScratch sum;
   unsigned int spare[60];
 };
 StreamScratch* stream_scratch(void* stream);     // NULL on failure (g_err set)
@@ -181,6 +181,41 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// deterministic sum over launch_sum's fixed grid of SCRATCH_BLOCKS x 256 threads: each block writes its partial, the last block
+// to finish adds them in block order into out[0] and resets the counter, so the next sum kernel on the stream finds `done` at 0.
+// The trip counts are the grid's constants: the final loop is latency-bound, and a known count lets the compiler batch its loads.
+__device__ __forceinline__ void block_partial_finish(float acc, SumScratch& sc, float* out) {
+  __shared__ float red[8];
+  __shared__ bool last;
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += red[w];
+    sc.partials[blockIdx.x] = t;
+    __threadfence();
+    last = (atomicAdd(&sc.done, 1u) == SCRATCH_BLOCKS - 1);
+  }
+  __syncthreads();
+  if (last && threadIdx.x == 0) {
+    __threadfence();
+    float t = 0.f;
+    for (int b = 0; b < SCRATCH_BLOCKS; ++b) t += reinterpret_cast<volatile float*>(sc.partials)[b];
+    out[0] += t;
+    sc.done = 0;
+  }
+}
+
+// launches a kernel that ends in block_partial_finish on SCRATCH_BLOCKS x 256 threads, with the stream's SumScratch appended to args
+template <class... Params, class... Args>
+inline int launch_sum(void (*kernel)(Params...), void* stream, const char* name, Args... args) {
+  StreamScratch* scr = stream_scratch(stream);
+  if (!scr) return 1;
+  kernel<<<SCRATCH_BLOCKS, 256, 0, (cudaStream_t)stream>>>(args..., &scr->sum);
+  return check_launch(name);
 }
 
 // streaming 128-bit store (output that is not re-read by this kernel: keep it out of the way of the map in L2)

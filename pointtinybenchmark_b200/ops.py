@@ -656,50 +656,42 @@ def point_assigner(points, gt_bboxes, scale=4, pos_num=3):
     return out
 
 
+def _loss_sum(fn, x, args, scale, want_grad):
+    """fn(x, *args, loss_sum, scale, grad, stream), the calling convention of the fused loss entry points.  Returns the (1,) loss
+    sum or, with want_grad, the gradient scale * d/dx instead (the sum is then not computed)."""
+    loss = torch.zeros(1, dtype=torch.float32, device=x.device)
+    grad = torch.empty_like(x) if want_grad else None
+    check(fn(_ptr(x), *args, _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()), fn.__name__)
+    return grad if want_grad else loss
+
+
 def sigmoid_focal(logits, labels, weight, gamma, alpha, scale=None, want_grad=False):
     """sum_m,c focal(logits, labels) * weight[m]; optional grad = scale * d/dlogits."""
     lib = _lib.load()
     _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels')
     M, C = logits.shape
-    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
-    grad = torch.empty_like(logits) if want_grad else None
-    check(lib.ptb_sigmoid_focal_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), M, C, float(gamma), float(alpha),
-                                        _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
-          'ptb_sigmoid_focal_fwd_bwd')
-    return grad if want_grad else loss
+    return _loss_sum(lib.ptb_sigmoid_focal_fwd_bwd, logits, (_ptr(labels), _ptr(weight), M, C, float(gamma), float(alpha)), scale,
+                     want_grad)
 
 
 def smooth_l1(pred, target, weight, inv_norm, beta, scale=None, want_grad=False):
     lib = _lib.load()
     _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target')
-    M = pred.shape[0]
-    loss = torch.zeros(1, dtype=torch.float32, device=pred.device)
-    grad = torch.empty_like(pred) if want_grad else None
-    check(lib.ptb_smooth_l1_fwd_bwd(_ptr(pred), _ptr(target), _ptr(weight), M, float(inv_norm), float(beta),
-                                    _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
-          'ptb_smooth_l1_fwd_bwd')
-    return grad if want_grad else loss
+    return _loss_sum(lib.ptb_smooth_l1_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], float(inv_norm), float(beta)),
+                     scale, want_grad)
 
 
-def sigmoid_bce(logits, labels, weight, scale=None, want_grad=False, pos_weight=None):
+def sigmoid_bce(logits, labels, weight, pos_weight=None, scale=None, want_grad=False):
     """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels), pos_weight) * weight[m] (labels == C: background row);
     optional grad = scale * d/dlogits.  pos_weight (C,) = CrossEntropyLoss.class_weight in sigmoid mode."""
     lib = _lib.load()
     _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels')
     M, C = logits.shape
-    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
-    grad = torch.empty_like(logits) if want_grad else None
-    if pos_weight is None:
-        check(lib.ptb_sigmoid_bce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), M, C, _ptr(loss) if not want_grad else None,
-                                          _ptr(scale), _ptr(grad), _stream()), 'ptb_sigmoid_bce_fwd_bwd')
-        return grad if want_grad else loss
-    _chk(pos_weight, torch.float32, 'pos_weight')
-    if pos_weight.shape != (C,):
-        raise ValueError(f'pos_weight must have shape ({C},), got {tuple(pos_weight.shape)}')
-    check(lib.ptb_sigmoid_bce_cw_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), _ptr(pos_weight), M, C,
-                                         _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
-          'ptb_sigmoid_bce_cw_fwd_bwd')
-    return grad if want_grad else loss
+    if pos_weight is not None:
+        _chk(pos_weight, torch.float32, 'pos_weight')
+        if pos_weight.shape != (C,):
+            raise ValueError(f'pos_weight must have shape ({C},), got {tuple(pos_weight.shape)}')
+    return _loss_sum(lib.ptb_sigmoid_bce_cw_fwd_bwd, logits, (_ptr(labels), _ptr(weight), _ptr(pos_weight), M, C), scale, want_grad)
 
 
 def softmax_ce(logits, labels, weight, class_weight=None, scale=None, want_grad=False):
@@ -712,24 +704,14 @@ def softmax_ce(logits, labels, weight, class_weight=None, scale=None, want_grad=
         _chk(class_weight, torch.float32, 'class_weight')
         if class_weight.shape != (C1,):
             raise ValueError(f'class_weight must have shape ({C1},), got {tuple(class_weight.shape)}')
-    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
-    grad = torch.empty_like(logits) if want_grad else None
-    check(lib.ptb_softmax_ce_fwd_bwd(_ptr(logits), _ptr(labels), _ptr(weight), _ptr(class_weight), M, C1,
-                                     _ptr(loss) if not want_grad else None, _ptr(scale), _ptr(grad), _stream()),
-          'ptb_softmax_ce_fwd_bwd')
-    return grad if want_grad else loss
+    return _loss_sum(lib.ptb_softmax_ce_fwd_bwd, logits, (_ptr(labels), _ptr(weight), _ptr(class_weight), M, C1), scale, want_grad)
 
 
 def mse(pred, target, weight, inv_norm, scale=None, want_grad=False):
     """sum ((pred - target) * inv_norm)^2 * weight over (M, 2) points; optional grad = scale * d/dpred."""
     lib = _lib.load()
     _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target')
-    M = pred.shape[0]
-    loss = torch.zeros(1, dtype=torch.float32, device=pred.device)
-    grad = torch.empty_like(pred) if want_grad else None
-    check(lib.ptb_mse_fwd_bwd(_ptr(pred), _ptr(target), _ptr(weight), M, float(inv_norm), _ptr(loss) if not want_grad else None,
-                              _ptr(scale), _ptr(grad), _stream()), 'ptb_mse_fwd_bwd')
-    return grad if want_grad else loss
+    return _loss_sum(lib.ptb_mse_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], float(inv_norm)), scale, want_grad)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -32,84 +32,23 @@ def _iou_of(nms_cfg):
     return float(v)
 
 
-class _FocalSumFn(torch.autograd.Function):
-    """sum_m,c sigmoid_focal(logits, labels) * weight[m]   (losses/focal_loss.py:11-56)"""
+class _LossSumFn(torch.autograd.Function):
+    """op(x, *args)[0] for a fused loss of ops (sigmoid_focal, sigmoid_bce, softmax_ce, smooth_l1, mse), differentiable in x: the
+    backward is op's gradient launch, op(x, *args, scale=g, want_grad=True)."""
 
     @staticmethod
-    def forward(ctx, logits, labels, weight, gamma, alpha):
-        ctx.save_for_backward(logits, labels, weight)
-        ctx.ga = (gamma, alpha)
-        return ops.sigmoid_focal(logits, labels, weight, gamma, alpha)[0]
-
-    @staticmethod
-    def backward(ctx, g):
-        logits, labels, weight = ctx.saved_tensors
-        scale = g.reshape(1).float().contiguous()
-        return ops.sigmoid_focal(logits, labels, weight, ctx.ga[0], ctx.ga[1], scale=scale, want_grad=True), None, None, None, None
-
-
-class _SigmoidBCESumFn(torch.autograd.Function):
-    """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels), pos_weight=class_weight) * weight[m]
-    (losses/cross_entropy_loss.py:42-89)"""
-
-    @staticmethod
-    def forward(ctx, logits, labels, weight, pos_weight=None):
-        ctx.save_for_backward(logits, labels, weight, pos_weight)
-        return ops.sigmoid_bce(logits, labels, weight, pos_weight=pos_weight)[0]
+    def forward(ctx, op, x, *args):
+        is_tensor = [isinstance(a, torch.Tensor) for a in args]
+        ctx.save_for_backward(x, *(a if t else None for a, t in zip(args, is_tensor)))
+        ctx.op, ctx.args = op, [None if t else a for a, t in zip(args, is_tensor)]
+        return op(x, *args)[0]
 
     @staticmethod
     def backward(ctx, g):
-        logits, labels, weight, pos_weight = ctx.saved_tensors
+        x, *tensors = ctx.saved_tensors
+        args = [a if t is None else t for a, t in zip(ctx.args, tensors)]
         scale = g.reshape(1).float().contiguous()
-        return ops.sigmoid_bce(logits, labels, weight, scale=scale, want_grad=True, pos_weight=pos_weight), None, None, None
-
-
-class _SoftmaxCESumFn(torch.autograd.Function):
-    """sum_m cross_entropy(logits[m], labels[m], weight=class_weight) * weight[m] over C+1 columns
-    (losses/cross_entropy_loss.py:9-39, use_sigmoid=False)"""
-
-    @staticmethod
-    def forward(ctx, logits, labels, weight, class_weight=None):
-        ctx.save_for_backward(logits, labels, weight, class_weight)
-        return ops.softmax_ce(logits, labels, weight, class_weight)[0]
-
-    @staticmethod
-    def backward(ctx, g):
-        logits, labels, weight, class_weight = ctx.saved_tensors
-        scale = g.reshape(1).float().contiguous()
-        return ops.softmax_ce(logits, labels, weight, class_weight, scale=scale, want_grad=True), None, None, None
-
-
-class _MSESumFn(torch.autograd.Function):
-    """sum ((pred - target) * inv_norm)^2 * weight   (losses/mse_loss.py:9-48)"""
-
-    @staticmethod
-    def forward(ctx, pred, target, weight, inv_norm):
-        ctx.save_for_backward(pred, target, weight)
-        ctx.inv_norm = inv_norm
-        return ops.mse(pred, target, weight, inv_norm)[0]
-
-    @staticmethod
-    def backward(ctx, g):
-        pred, target, weight = ctx.saved_tensors
-        scale = g.reshape(1).float().contiguous()
-        return ops.mse(pred, target, weight, ctx.inv_norm, scale=scale, want_grad=True), None, None, None
-
-
-class _SmoothL1SumFn(torch.autograd.Function):
-    """sum smooth_l1((pred - target) * inv_norm, beta) * weight   (losses/smooth_l1_loss.py:25-31)"""
-
-    @staticmethod
-    def forward(ctx, pred, target, weight, inv_norm, beta):
-        ctx.save_for_backward(pred, target, weight)
-        ctx.nb = (inv_norm, beta)
-        return ops.smooth_l1(pred, target, weight, inv_norm, beta)[0]
-
-    @staticmethod
-    def backward(ctx, g):
-        pred, target, weight = ctx.saved_tensors
-        scale = g.reshape(1).float().contiguous()
-        return ops.smooth_l1(pred, target, weight, ctx.nb[0], ctx.nb[1], scale=scale, want_grad=True), None, None, None, None
+        return (None, ctx.op(x, *args, scale=scale, want_grad=True)) + (None,) * len(args)
 
 
 MAX_OUT_CHANNELS = 512     # widest output of the wgmma conv (ptb_conv_tc_f16x2): bounds num_points * num_classes
@@ -321,24 +260,23 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         cls_type, reg_type = self.loss_cls_cfg['type'], self.loss_reg_cfg['type']
         if cls_type not in LOSS_CLS_TYPES or reg_type not in LOSS_REG_TYPES:
             raise NotImplementedError(f'P2PHead: loss_cls must be one of {LOSS_CLS_TYPES} and loss_reg one of {LOSS_REG_TYPES}')
-        gamma, alpha = self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25)
         # loss_single (p2p_head.py:220-231): CrossEntropyLoss averages over every proposal of the batch, FocalLoss over the positives
         cls_avg = float(B * Q) if cls_type == 'CrossEntropyLoss' else num_total_pos
         inv_norm = 1.0 / (s * self.reg_norm)
         cw = self.class_weight.to(dev) if self.class_weight is not None else None
+        if cls_type == 'FocalLoss':
+            cls_op, cls_args = ops.sigmoid_focal, (self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25))
+        else:
+            cls_op, cls_args = (ops.sigmoid_bce if self.use_sigmoid_cls else ops.softmax_ce), (cw,)
+        if reg_type == 'MSELoss':
+            reg_op, reg_args = ops.mse, (inv_norm,)
+        else:
+            reg_op, reg_args = ops.smooth_l1, (inv_norm, self.loss_reg_cfg.get('beta', 1.0))
         loss_cls, loss_pts = [], []
         for b in range(B):
-            if cls_type == 'CrossEntropyLoss' and not self.use_sigmoid_cls:
-                lc = _SoftmaxCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], cw)
-            elif cls_type == 'CrossEntropyLoss':
-                lc = _SigmoidBCESumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], cw)
-            else:
-                lc = _FocalSumFn.apply(cls[b].contiguous(), labels_l[b], lw_l[b], gamma, alpha)
+            lc = _LossSumFn.apply(cls_op, cls[b].contiguous(), labels_l[b], lw_l[b], *cls_args)
             loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / cls_avg)
-            if reg_type == 'MSELoss':
-                lp = _MSESumFn.apply(pred[b].contiguous(), gp_l[b], pw_l[b], inv_norm)
-            else:
-                lp = _SmoothL1SumFn.apply(pred[b].contiguous(), gp_l[b], pw_l[b], inv_norm, self.loss_reg_cfg.get('beta', 1.0))
+            lp = _LossSumFn.apply(reg_op, pred[b].contiguous(), gp_l[b], pw_l[b], *reg_args)
             loss_pts.append(self.loss_reg_cfg.get('loss_weight', 1.0) * lp / num_total_pos)
         self._last_targets = dict(labels=labels_l, label_weights=lw_l, gt_pts=gp_l, pts_weights=pw_l)
         return dict(loss_cls=loss_cls, loss_pts=loss_pts)

@@ -118,11 +118,15 @@ def test_sigmoid_bce_pos_weight_matches_float64(ops, C):
     from pointtinybenchmark_b200.ops import _ptr, _stream
     lib = _lib.load()
     for want_grad in (False, True):
-        out = torch.zeros(1, device=dev) if not want_grad else torch.empty_like(xd)
-        lsum, grad = (None, out) if want_grad else (out, None)
-        rc = lib.ptb_sigmoid_bce_cw_fwd_bwd(_ptr(xd), _ptr(ld), _ptr(wd), None, M, C, _ptr(lsum), _ptr(sc), _ptr(grad), _stream())
-        assert rc == 0, lib.ptb_last_error()
-        assert torch.equal(out, ops.sigmoid_bce(xd, ld, wd, scale=sc, want_grad=want_grad)), 'NULL pos_weight = class_weight None'
+        outs = []
+        for call in (lambda *out: lib.ptb_sigmoid_bce_cw_fwd_bwd(_ptr(xd), _ptr(ld), _ptr(wd), None, M, C, *out),
+                     lambda *out: lib.ptb_sigmoid_bce_fwd_bwd(_ptr(xd), _ptr(ld), _ptr(wd), M, C, *out)):
+            out = torch.zeros(1, device=dev) if not want_grad else torch.empty_like(xd)
+            lsum, grad = (None, out) if want_grad else (out, None)
+            rc = call(_ptr(lsum), _ptr(sc), _ptr(grad), _stream())
+            assert rc == 0, lib.ptb_last_error()
+            outs.append(out)
+        assert torch.equal(*outs), 'NULL pos_weight = class_weight None'
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
