@@ -229,7 +229,9 @@ struct FocalLoss {
     const float bce = fmaxf(v, 0.f) - v * t + log1pf(expf(-fabsf(v)));
     if (grad) {
       const float dpt = (t > 0.5f ? -1.f : 1.f) * p * (1.f - p);
-      const float ptg1 = (gamma == 2.f) ? 2.f * pt : gamma * powf(pt, gamma - 1.f);
+      // d pt^gamma / d pt.  At gamma 0 it is 0, as torch's pow_backward makes it: gamma * powf(pt, -1) would be 0 * inf = NaN
+      // for a saturated, correctly classified element (pt == 0)
+      const float ptg1 = (gamma == 2.f) ? 2.f * pt : (gamma == 0.f ? 0.f : gamma * powf(pt, gamma - 1.f));
       grad[e] = sc * w * a * (ptg1 * dpt * bce + ptg * (p - t));
     }
     return bce * (a * ptg) * w;
@@ -243,7 +245,8 @@ struct SmoothL1Loss {
     const float w = weight ? weight[e] : 1.f;
     const float diff = (pred[e] - target[e]) * inv_norm;
     const float d = fabsf(diff);
-    if (grad) grad[e] = sc * w * inv_norm * (d < beta ? diff / beta : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f)));
+    // a NaN diff keeps its NaN gradient (0 * |diff|), as torch's does through the unselected branch of torch.where
+    if (grad) grad[e] = sc * w * inv_norm * (d < beta ? diff / beta : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f * d)));
     return (d < beta ? 0.5f * d * d / beta : d - 0.5f * beta) * w;
   }
 };
