@@ -591,6 +591,9 @@ extern "C" int ptb_cpr_refine(const float* bag_prob, const float* bag_pts, const
   PTB_REQUIRE(out_pts && out_score && out_not_refine, "NULL output");
   const size_t smem = (size_t)3 * Kt * sizeof(float);
   PTB_REQUIRE(smem <= 48 * 1024, "bag too large for shared memory");
+  if (smem > 40 * 1024 &&     // static (384 B) + dynamic beyond the 48 KB default needs the opt-in; per-device attribute -> per call
+      cudaFuncSetAttribute(refine_stage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return fail("%s", "ptb_cpr_refine: shared memory opt-in failed");
   refine_stage_kernel<<<G, RF_THREADS, smem, (cudaStream_t)stream>>>(bag_prob, bag_pts, bag_valid, Kt, K, num_classes, labels,
                                                                    bag_img, img_hw, grp_of, grp_ptr, grp_idx, not_refine_in,
                                                                    cfg, out_pts, out_score, out_not_refine, out_chosen,
