@@ -11,9 +11,13 @@
 //                 K = taps x Cin.  One K-block = (tap, 64 B of input channels) = one SWIZZLE_64B row.
 //   Outputs wider than 128 channels run as ceil(n_mma / 128) slices of 128 in ONE launch (2 at 256, 3 at 320, 4 at 512); the
 //   persistent CTAs walk the (tile, slice) items, the weight TMA box of slice s starts at row 128 s (rows >= n_mma zero-filled).
-//   * A operand: 4-D TMA box {64 B ch, tile w, tile h, 1 img} of the channels-last activation at the tap-shifted origin;
-//     out-of-bounds (the zero padding of the conv and partial edge tiles) is zero-filled by the TMA unit.
+//   * A operand: 4-D TMA box {64 B ch, tile w, tile h + 2, 1 img} of the channels-last activation at (h0 - 1, w0 + kw - 1): one
+//     box serves the three vertical taps kh = 0, 1, 2 of column offset kw, as the same shared memory at + kh x tile w x 64 B (whole
+//     512 B swizzle atoms for every tile shape, so the wgmma descriptors only move their start address).  A 1-tap conv loads the
+//     tile itself.  Out-of-bounds (the zero padding of the conv and partial edge tiles) is zero-filled by the TMA unit.
 //   * B operand: 2-D TMA box {64 B k, NT co} of the packed weights W2[co][tap*Cin + ci]; rows beyond n_mma are zero-filled.
+//   * K order (9 taps): (kw, channel block, kh); one activation box (hi + lo) serves 3 K-blocks, each with its own weight box
+//     (hi + lo) of tap (kh, kw).  That is 22.7 KB of TMA traffic per K-block instead of 32 KB with one box per tap.
 //   * fp32 accuracy (the head's logits must match the fp32 reference to 1e-4).  Every operand is split x = hi + lo and three
 //     MMAs per k-step accumulate hi*hi + lo*hi + hi*lo (the lo*lo term is below 2^-22 |a||b|):
 //       F16 = true  (default): hi = fp16(x*s), lo = fp16(x*s - hi) with one power-of-two scale s per tensor (undone exactly in
@@ -25,8 +29,10 @@
 //     absolute terms); the epilogue adds the two in fp32 (round-to-nearest).
 //   * warp roles (384 threads, 1 CTA / SM, persistent over (tile, channel slice) items): warpgroup 0 = TMA producer (one thread),
 //     warpgroups 1 and 2 = MMA + epilogue for pixel rows 0-63 / 64-127 of the tile, each holding two 64 x NT fp32 accumulators in
-//     registers (128 per thread at NT = 128).  Six 32 KB shared-memory stages (mbarrier full / empty ring): the producer runs ahead
-//     into the next item while the MMA warpgroups store the previous one.
+//     registers (128 per thread at NT = 128).  Two mbarrier full / empty rings in shared memory: 4 x 24 KB activation boxes,
+//     released after their last K-block, and 8 x 16 KB weight boxes, released after every K-block, so the weight loads of the
+//     next K-blocks never wait for a whole activation box to retire.  The producer runs ahead into the next item while the MMA
+//     warpgroups store the previous one.
 //   * epilogue: straight from the accumulator registers (add, scale, bias) to global memory (8-byte stores, 32 contiguous bytes per
 //     row and quad); GroupNorm sum / sum of squares per (image, group of 8 channels) by a halving butterfly over the 32 lanes of a
 //     warp + one fp64 atomic per lane.
@@ -42,11 +48,17 @@ constexpr int CV_BM = 128;                      // output pixels per tile
 constexpr int CV_NT = 128;                      // widest output-channel slice of one item
 constexpr int CV_KB = 16;                       // fp32/TF32 input channels per K-block (64 B = one SWIZZLE_64B row)
 constexpr int CV_KB_F16 = 32;                   // fp16 input channels per K-block (also 64 B)
-constexpr int CV_STAGES = 6;                    // 6 x 32 KB ring
-constexpr uint32_t CV_A_BYTES = CV_BM * 64;                 // 8 KB
+constexpr int CV_KH = 3;                        // K-blocks per activation box: the vertical taps kh = 0, 1, 2 share one box
+constexpr int CV_A_STAGES = 4;                  // activation ring: 4 x 24 KB (hi + lo box)
+constexpr int CV_B_STAGES = 8;                  // weight ring: 8 x 16 KB (hi + lo box of one K-block)
+constexpr uint32_t CV_A_BYTES = (CV_BM + 2 * 32) * 64;      // 12 KB: the tallest box, (4 + 2) x 32 pixels (tile shape 1)
 constexpr uint32_t CV_B_BYTES = CV_NT * 64;                 // 8 KB (a narrower slice uses the front of it)
-constexpr uint32_t CV_STAGE_BYTES = 2 * CV_A_BYTES + 2 * CV_B_BYTES;   // 32 KB
-constexpr uint32_t CV_SMEM_BYTES = CV_STAGES * CV_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr uint32_t CV_A_STAGE_BYTES = 2 * CV_A_BYTES;       // 24 KB
+constexpr uint32_t CV_B_STAGE_BYTES = 2 * CV_B_BYTES;       // 16 KB
+constexpr uint32_t CV_RING_BYTES = CV_A_STAGES * CV_A_STAGE_BYTES + CV_B_STAGES * CV_B_STAGE_BYTES;   // 224 KB
+constexpr uint32_t CV_SMEM_BYTES = CV_RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(CV_SMEM_BYTES <= 227 * 1024, "the conv rings must fit the 227 KB of opt-in shared memory");
+static_assert(2 * 8 * (CV_A_STAGES + CV_B_STAGES) <= 256, "the conv barriers must fit their 256 B");
 constexpr int CV_THREADS = 384;
 
 // Output tiling.  A tile is always 128 pixels; the main region uses 8 x 16 tiles and the two edge strips that 8 x 16 tiles would
@@ -98,19 +110,27 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
   constexpr int KBC = F16 ? CV_KB_F16 : CV_KB;      // channels per K-block
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // swizzle atoms need (at least) 512 B alignment
-  const uint32_t bar_base = smem_base + CV_STAGES * CV_STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
+  const uint32_t sA_base = smem_base, sB_base = smem_base + CV_A_STAGES * CV_A_STAGE_BYTES;
+  const uint32_t bar_base = smem_base + CV_RING_BYTES;
+  auto full_a = [&](int s) { return bar_base + 8u * s; };
+  auto empty_a = [&](int s) { return bar_base + 8u * (CV_A_STAGES + s); };
+  auto full_b = [&](int s) { return bar_base + 8u * (2 * CV_A_STAGES + s); };
+  auto empty_b = [&](int s) { return bar_base + 8u * (2 * CV_A_STAGES + CV_B_STAGES + s); };
 
   const int wg = threadIdx.x >> 7;
   const int kblocks_per_tap = cs.Cin / KBC;
-  const int n_kb = cs.taps * kblocks_per_tap;
+  const int n_kh = cs.taps == 9 ? CV_KH : 1;             // K-blocks per activation box
+  const int n_boxes_item = (cs.taps / n_kh) * kblocks_per_tap;   // activation boxes per item: (kw, channel block), kh innermost
   const int n_items = cs.n_tiles * cs.n_slices;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < CV_STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);                    // one arrive per MMA warp
+    for (int s = 0; s < CV_A_STAGES; ++s) {
+      mbar_init(full_a(s), 1);
+      mbar_init(empty_a(s), 8);                      // one arrive per MMA warp
+    }
+    for (int s = 0; s < CV_B_STAGES; ++s) {
+      mbar_init(full_b(s), 1);
+      mbar_init(empty_b(s), 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -120,26 +140,33 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
     // =============================== TMA producer ===============================
     regs_dealloc<40>();
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      int a_st = 0, b_st = 0;
+      uint32_t a_ph = 0, b_ph = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         const int tile = item / cs.n_slices, n0 = (item - tile * cs.n_slices) * NT;
         const TileAt ta = tile_at(cs, tile);
-        for (int kb = 0; kb < n_kb; ++kb) {
-          const int tap = kb / kblocks_per_tap, cblk = kb - tap * kblocks_per_tap;
-          const int kh = cs.taps == 9 ? tap / 3 : 1, kw = cs.taps == 9 ? tap - (tap / 3) * 3 : 1;
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sA_hi = smem_base + stage * CV_STAGE_BYTES;
-          const uint32_t sA_lo = sA_hi + CV_A_BYTES;
-          const uint32_t sB_hi = sA_lo + CV_A_BYTES;
-          const uint32_t sB_lo = sB_hi + CV_B_BYTES;
-          const int kcol = tap * cs.Cin + cblk * KBC;
-          mbar_expect_tx(full_bar(stage), 2 * CV_A_BYTES + 2 * NT * 64);
-          tma_load_4d(&mp.x[ta.shape][0], full_bar(stage), sA_hi, cblk * KBC, ta.w0 + kw - 1, ta.h0 + kh - 1, ta.b);
-          tma_load_4d(&mp.x[ta.shape][1], full_bar(stage), sA_lo, cblk * KBC, ta.w0 + kw - 1, ta.h0 + kh - 1, ta.b);
-          tma_load_2d(&mp.w[0], full_bar(stage), sB_hi, kcol, n0);
-          tma_load_2d(&mp.w[1], full_bar(stage), sB_lo, kcol, n0);
-          if (++stage == CV_STAGES) { stage = 0; phase ^= 1u; }
+        // 9 taps: the box is the tile shifted by kw - 1 columns and grown by one row above and below (the maps' box height is
+        // tile h + 2); 1 tap: the tile itself
+        const uint32_t a_bytes = (uint32_t)(CV_BM + ((n_kh - 1) << ta.twl)) * 64u;
+        for (int ks = 0; ks < n_boxes_item; ++ks) {
+          const int kw = cs.taps == 9 ? ks / kblocks_per_tap : 1, cblk = ks - (ks / kblocks_per_tap) * kblocks_per_tap;
+          mbar_wait(empty_a(a_st), a_ph ^ 1u);
+          const uint32_t sA_hi = sA_base + a_st * CV_A_STAGE_BYTES;
+          mbar_expect_tx(full_a(a_st), 2 * a_bytes);
+          const int aw = ta.w0 + kw - 1, ah = ta.h0 - (n_kh > 1 ? 1 : 0);
+          tma_load_4d(&mp.x[ta.shape][0], full_a(a_st), sA_hi, cblk * KBC, aw, ah, ta.b);
+          tma_load_4d(&mp.x[ta.shape][1], full_a(a_st), sA_hi + CV_A_BYTES, cblk * KBC, aw, ah, ta.b);
+          if (++a_st == CV_A_STAGES) { a_st = 0; a_ph ^= 1u; }
+          for (int kh = 0; kh < n_kh; ++kh) {                // the weight rows of taps (kh, kw), kh = 0 .. n_kh - 1
+            const int tap = cs.taps == 9 ? 3 * kh + kw : 0;
+            const int kcol = tap * cs.Cin + cblk * KBC;
+            mbar_wait(empty_b(b_st), b_ph ^ 1u);
+            const uint32_t sB_hi = sB_base + b_st * CV_B_STAGE_BYTES;
+            mbar_expect_tx(full_b(b_st), 2 * NT * 64);
+            tma_load_2d(&mp.w[0], full_b(b_st), sB_hi, kcol, n0);
+            tma_load_2d(&mp.w[1], full_b(b_st), sB_hi + CV_B_BYTES, kcol, n0);
+            if (++b_st == CV_B_STAGES) { b_st = 0; b_ph ^= 1u; }
+          }
         }
       }
     }
@@ -150,46 +177,65 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     const float sc = F16 ? (dev_out_scale ? __fmul_rn(out_scale, *dev_out_scale) : out_scale) : 1.f;   // powers of two: exact
     float acc[NT / 2], cor[NT / 2];
-    int stage = 0;
-    uint32_t phase = 0;
+    int a_st = 0, b_st = 0;
+    uint32_t a_ph = 0, b_ph = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       const int tile = item / cs.n_slices, n0 = (item - tile * cs.n_slices) * NT;
-      int prev = 0;
-      for (int kb = 0; kb < n_kb; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        const uint32_t sA_hi = smem_base + stage * CV_STAGE_BYTES + (uint32_t)cw * (CV_A_BYTES / 2);
-        const uint32_t sA_lo = sA_hi + CV_A_BYTES;
-        const uint32_t sB_hi = smem_base + stage * CV_STAGE_BYTES + 2 * CV_A_BYTES;
-        const uint32_t sB_lo = sB_hi + CV_B_BYTES;
-        wgmma_fence();
+      const TileAt ta = tile_at(cs, tile);
+      // pixel p of the tile sits at box row p + kh * tile w for vertical tap kh: kh * (512 / 1024 / 2048 B), whole swizzle atoms
+      const uint32_t kh_step = 64u << ta.twl;
+      // the K loop of one item with a compile-time count of K-blocks per box (a run-time count inside the MMA sequence makes
+      // ptxas fence the accumulators between the K-blocks).  Each K-block is one commit group; once the next one is issued and
+      // the previous one has completed, its weight slot goes back, and its activation slot too after the box's last K-block.
+      auto k_loop = [&](auto kh_n_) {
+        constexpr int KH_N = decltype(kh_n_)::value;
+        int prev_a = 0, prev_b = 0;
+        for (int ks = 0; ks < n_boxes_item; ++ks) {
+          mbar_wait(full_a(a_st), a_ph);
+          const uint32_t sA_hi = sA_base + a_st * CV_A_STAGE_BYTES + (uint32_t)cw * (CV_BM * 64 / 2);
+          const uint32_t sA_lo = sA_hi + CV_A_BYTES;
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {                        // 32 B (16 fp16 / 8 tf32) of K per MMA inside the 64 B swizzle row
-          const uint64_t a_hi = gmma_desc(sA_hi + 32u * k, 16u, 512u, GMMA_SW64), a_lo = gmma_desc(sA_lo + 32u * k, 16u, 512u, GMMA_SW64);
-          const uint64_t b_hi = gmma_desc(sB_hi + 32u * k, 16u, 512u, GMMA_SW64), b_lo = gmma_desc(sB_lo + 32u * k, 16u, 512u, GMMA_SW64);
-          const uint32_t first = (kb | k) != 0;
-          if constexpr (F16) {
-            wgmma_f16<0, 0>(acc, a_hi, b_hi, first);
-            wgmma_f16<0, 0>(cor, a_lo, b_hi, first);
-            wgmma_f16<0, 0>(cor, a_hi, b_lo, 1u);
-          } else {
-            wgmma_tf32(acc, a_hi, b_hi, first);
-            wgmma_tf32(cor, a_lo, b_hi, first);
-            wgmma_tf32(cor, a_hi, b_lo, 1u);
+          for (int kh = 0; kh < KH_N; ++kh) {
+            mbar_wait(full_b(b_st), b_ph);
+            const uint32_t a_off = kh_step * kh, sB_hi = sB_base + b_st * CV_B_STAGE_BYTES, sB_lo = sB_hi + CV_B_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {                    // 32 B (16 fp16 / 8 tf32) of K per MMA inside the 64 B swizzle row
+              const uint64_t a_hi = gmma_desc(sA_hi + a_off + 32u * k, 16u, 512u, GMMA_SW64);
+              const uint64_t a_lo = gmma_desc(sA_lo + a_off + 32u * k, 16u, 512u, GMMA_SW64);
+              const uint64_t b_hi = gmma_desc(sB_hi + 32u * k, 16u, 512u, GMMA_SW64), b_lo = gmma_desc(sB_lo + 32u * k, 16u, 512u, GMMA_SW64);
+              const uint32_t first = (ks | kh | k) != 0;
+              if constexpr (F16) {
+                wgmma_f16<0, 0>(acc, a_hi, b_hi, first);
+                wgmma_f16<0, 0>(cor, a_lo, b_hi, first);
+                wgmma_f16<0, 0>(cor, a_hi, b_lo, 1u);
+              } else {
+                wgmma_tf32(acc, a_hi, b_hi, first);
+                wgmma_tf32(cor, a_lo, b_hi, first);
+                wgmma_tf32(cor, a_hi, b_lo, 1u);
+              }
+            }
+            wgmma_commit();
+            if ((ks | kh) != 0) {                            // the previous K-block's MMAs have read their slots: hand them back
+              wgmma_wait<1>();
+              if (lane == 0) {
+                mbar_arrive(empty_b(prev_b));
+                if (kh == 0) mbar_arrive(empty_a(prev_a));   // the previous K-block was the last one of its box
+              }
+            }
+            prev_b = b_st;
+            if (++b_st == CV_B_STAGES) { b_st = 0; b_ph ^= 1u; }
           }
+          prev_a = a_st;
+          if (++a_st == CV_A_STAGES) { a_st = 0; a_ph ^= 1u; }
         }
-        wgmma_commit();
-        if (kb > 0) {                                        // the previous K-block's MMAs have read their stage: hand it back
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(empty_bar(prev));
-        }
-        prev = stage;
-        if (++stage == CV_STAGES) { stage = 0; phase ^= 1u; }
-      }
-      wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(empty_bar(prev));
+        wgmma_wait<0>();
+        if (lane == 0) { mbar_arrive(empty_b(prev_b)); mbar_arrive(empty_a(prev_a)); }
+      };
+      if (n_kh == CV_KH) k_loop(std::integral_constant<int, CV_KH>{});
+      else k_loop(std::integral_constant<int, 1>{});
 
       // ---- epilogue: rows r0 and r0 + 8, columns n0 + 8 i + 2 (lane % 4) (+1) ----
-      const TileAt ta = tile_at(cs, tile);
       const int h_end = ta.shape == 2 ? cs.right_h : cs.H;   // the right strip stops where the bottom strip begins
       float* row_ptr[2];
       bool valid[2];
@@ -512,14 +558,17 @@ EncodeTiledFn tc_get_encode() {
 }
 
 constexpr int CV_SHAPE_TW[3] = {16, 32, 8}, CV_SHAPE_TH[3] = {8, 4, 16};
+static_assert((CV_SHAPE_TH[0] + 2) * CV_SHAPE_TW[0] * 64 <= CV_A_BYTES && (CV_SHAPE_TH[1] + 2) * CV_SHAPE_TW[1] * 64 <= CV_A_BYTES &&
+              (CV_SHAPE_TH[2] + 2) * CV_SHAPE_TW[2] * 64 <= CV_A_BYTES, "a conv3x3 activation box overflows its stage slot");
 
-static int make_act_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, int C, bool f16, int shape) {
+// halo: extra image rows of the box (2 for a conv3x3: the three vertical taps of one column offset read one box)
+static int make_act_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, int C, bool f16, int shape, int halo) {
   EncodeTiledFn enc = tc_get_encode();
   if (!enc) return fail("%s", "cuTensorMapEncodeTiled is unavailable (driver too old?)");
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   const cuuint64_t es = f16 ? 2 : 4;
   cuuint64_t strides[3] = {(cuuint64_t)C * es, (cuuint64_t)W * C * es, (cuuint64_t)H * W * C * es};
-  cuuint32_t box[4] = {(cuuint32_t)(f16 ? CV_KB_F16 : CV_KB), (cuuint32_t)CV_SHAPE_TW[shape], (cuuint32_t)CV_SHAPE_TH[shape], 1};
+  cuuint32_t box[4] = {(cuuint32_t)(f16 ? CV_KB_F16 : CV_KB), (cuuint32_t)CV_SHAPE_TW[shape], (cuuint32_t)(CV_SHAPE_TH[shape] + halo), 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(tm, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -607,8 +656,8 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
   ConvMaps mp;
   int rc;
   for (int sh = 0; sh < 3; ++sh) {
-    if ((rc = make_act_map(&mp.x[sh][0], x_hi, B, H, W, Cin, F16, sh))) return rc;
-    if ((rc = make_act_map(&mp.x[sh][1], x_lo, B, H, W, Cin, F16, sh))) return rc;
+    if ((rc = make_act_map(&mp.x[sh][0], x_hi, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
+    if ((rc = make_act_map(&mp.x[sh][1], x_lo, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
   }
   if ((rc = make_w_map(&mp.w[0], w_hi, n_mma, taps * Cin, F16, nt))) return rc;
   if ((rc = make_w_map(&mp.w[1], w_lo, n_mma, taps * Cin, F16, nt))) return rc;
