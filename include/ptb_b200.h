@@ -177,6 +177,29 @@ int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld
                      const float* scale /*[1] device scalar*/, float* grad_logits /*[G][Kt][ld], cls+ins columns written*/,
                      void* stream);
 
+/* Loss term of the positive bags (MILLoss / AllPosLoss `loss_type`, multi_instance_learning_loss.py:187-202, 229-240):
+ *   PTB_LOSS_GFOCAL  gfocal_loss(p, onehot) x label weight (the bag's any-weight flag for MIL, w_k for AllPos)
+ *   PTB_LOSS_BCE     F.binary_cross_entropy(p, onehot) UNWEIGHTED: (t-1) max(log1p(-p), -100) - t max(log p, -100), as ATen on the CPU;
+ *                    a MIL bag whose weights are all zero (prob = 0) still adds 100 at its label column, with zero gradient.
+ *                    A probability above 1 (rounding of saturated sigmoids; ATen raises) gives NaN.
+ * The _kind entry points below are the entry points above with a loss_kind argument; loss_kind = PTB_LOSS_GFOCAL gives their results
+ * bit for bit. */
+#define PTB_LOSS_GFOCAL 0
+#define PTB_LOSS_BCE 1
+int ptb_mil_loss_fwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                          const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum, float* out_stats,
+                          float* out_mt, void* stream);
+int ptb_mil_loss_bwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                          const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale, float* grad_logits,
+                          void* stream);
+/* AllPosLoss forward (multi_instance_learning_loss.py:206-243): every bag sample is a row p = sigmoid(logits[g][k][0..num_classes)) with
+ * the label of its bag.  aux [3*G] scratch; fixed-order sums (deterministic):
+ *   out_loss_sum[0] += sum_{g,k,c} term(p, onehot) (x weight[g][k] for PTB_LOSS_GFOCAL; unweighted over ALL samples for PTB_LOSS_BCE)
+ *   out_stats[0] += #samples with weight > 0 ;  out_stats[1] += #samples whose top-1 class (first maximum) == label */
+int ptb_cpr_allpos_fwd(const float* logits /*[G][K][ld]*/, int G, int K, int num_classes, int ld, const float* weight /*[G][K]*/,
+                       const int32_t* labels, float eps, int loss_kind, float* aux, float* out_loss_sum /*[1]*/, float* out_stats /*[2]*/,
+                       void* stream);
+
 /* Fused bag gather + MIL forward (ring bags, num_classes <= 128): samples the [cls | ins] logit map (columns 0.. and ins_off..) at every
  * bag point like ptb_cpr_bag_gather, writes the sampled rows (out_bag_logits [G][K][ld], needed by the backward), the sample validity
  * as weights (out_weight [G][K] = 0/1), and evaluates ptb_mil_loss_fwd on the fly with online softmax accumulators: the (G,K,ld) tensor
@@ -186,6 +209,10 @@ int ptb_cpr_bag_mil_fwd(const float* logit_map /*[B][H][W][ld]*/, int B, int H, 
                         const int32_t* pad_hw, const int32_t* labels, float eps, float* out_bag_logits, float* out_weight,
                         float* out_bag_prob, float* out_loss_sum /*[1]*/, float* out_stats /*[2]*/, float* out_mt /*[G][N][2] or NULL*/,
                         void* stream);
+int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off, const float* centers,
+                             const int32_t* bag_img, int G, const float* offsets, int K, float stride, const int32_t* pad_hw,
+                             const int32_t* labels, float eps, int loss_kind, float* out_bag_logits, float* out_weight, float* out_bag_prob,
+                             float* out_loss_sum, float* out_stats, float* out_mt, void* stream);
 
 /* Backward of the whole CPR training loss w.r.t. the LOGIT MAP in one deterministic kernel (gather formulation, no atomics on global
  * memory): replaces autograd of MILLoss (multi_instance_learning_loss.py:153-203), of the gt / neg gfocal terms (cpr_head.py:1159-1184,
@@ -216,6 +243,21 @@ int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const
                              const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
                              float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
                              void* workspace, float* grad_map /*[B][H][W][ld], accumulated into*/, void* stream);
+/* The two map backwards with the loss kind of the bag term and a per-sample positive term (AllPosLoss):
+ *   mil_mt == NULL      no MIL term (bag_prob, label_weight, scale_mil unused; the ins columns get no gradient);
+ *   scale_pos != NULL   every sample k of every bag adds scale_pos * w * term'(sigmoid(cls)) * sigmoid'(cls) to its cls columns, with
+ *                       w = weight[g][k] for PTB_LOSS_GFOCAL and w = 1 for PTB_LOSS_BCE (samples outside pad_shape included). */
+int ptb_cpr_loss_bwd_map_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                              const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
+                              const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                              float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
+                              const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
+                              int loss_kind, const float* scale_pos /*[1] or NULL*/, void* workspace, float* grad_map, void* stream);
+int ptb_cpr_loss_bwd_scatter_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                  const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
+                                  const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                  float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
+                                  int loss_kind, const float* scale_pos /*[1] or NULL*/, void* workspace, float* grad_map, void* stream);
 
 /* gfocal on sigmoid(logits) vs a one-hot / all-zero target with per-element weights — replaces
  * MILLoss.gfocal_loss (multi_instance_learning_loss.py:148-151) as used for gt_loss and neg_loss
@@ -228,6 +270,10 @@ int ptb_gfocal_sigmoid_fwd(const float* logits, int64_t M, int num_classes, int6
 int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
                            const int32_t* target_label, const void* weight, int wmode, float eps,
                            const float* scale, float* grad, int64_t grad_row_stride, int accumulate, void* stream);
+/* ptb_gfocal_sigmoid_bwd with the loss kind: PTB_LOSS_BCE gives scale * weight * d BCE(sigmoid(logit), target) / d logit. */
+int ptb_sigmoid_loss_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride, const int32_t* target_label,
+                         const void* weight, int wmode, float eps, int loss_kind, const float* scale, float* grad,
+                         int64_t grad_row_stride, int accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * P2P decode + top-k — replaces P2PHead.get_pred_points (p2p_head.py:125-170) and the per-level

@@ -194,10 +194,13 @@ class _CPRLossFn(torch.autograd.Function):
             lmap = ops.conv_tc_f16(fh, fl, ops.conv_tc_pack_weight_f16(wcat, 1), 1, LD, bias=bcat, dev_out_scale=finv, ldy=LD).view(M, LD)
         else:
             lmap = ops.linear_rows(x2d, wcat, bcat)                              # (M, LD) fp32 FFMA GEMM
-        fused_fwd = isinstance(bags, _CircleBags) and hp['with_mil_loss'] and N <= 128 and os.environ.get('PTB_LOSS_FWD', 'fused') == 'fused'
+        allpos, kind = hp['allpos'], hp['loss_kind']
+        fused_fwd = isinstance(bags, _CircleBags) and hp['with_mil_loss'] and not allpos and N <= 128 and \
+            os.environ.get('PTB_LOSS_FWD', 'fused') == 'fused'
         if fused_fwd:   # ring-bag gather + MIL forward in ONE kernel (online softmax): the (G,K,LD) tensor is written once, never re-read
             bl, weight, bag_prob, mil_sum, mil_stats, mil_mt, mil_lw = ops.bag_mil_fwd(
-                lmap.view(B, H, W, LD), N, NP, gt.centers, gt.bag_img, bags.offsets, bags.stride, gt.pad_hw, gt.labels, hp['eps'])
+                lmap.view(B, H, W, LD), N, NP, gt.centers, gt.bag_img, bags.offsets, bags.stride, gt.pad_hw, gt.labels, hp['eps'],
+                loss_kind=kind)
             aux = None
         else:
             bl, _, valid, aux = bags.gather(lmap.view(B, H, W, LD), gt)          # (G,K,LD), (G,K)
@@ -214,11 +217,23 @@ class _CPRLossFn(torch.autograd.Function):
             num_pos = torch.clamp((wc > 0).sum().float(), min=1.0)               # cpr_head.py:1180
             gt_loss = hp['gt_loss_weight'] * (s[0] / num_pos)
             saved['valid_center'], saved['num_pos_gt'] = wc, num_pos
-        if hp['with_mil_loss']:
+        if hp['with_mil_loss'] and allpos:
+            # AllPosLoss (multi_instance_learning_loss.py:206-243): every bag sample is a positive row; num_sample counts the samples
+            # with weight > 0, bag_acc is over all G*K samples.  The reference returns loss + bag_ins_outs * 0 (the scalar broadcast to
+            # the instance logits' shape, reduced by .mean() when the losses are parsed): this returns the scalar, and the instance
+            # classifier gets its exactly-zero gradient from the backward
+            s, stats = ops.allpos_fwd(bl, N, weight, gt.labels, hp['eps'], kind)
+            saved['mil_mt'] = saved['mil_lw'] = None
+            num_sample = torch.clamp(stats[0], min=1.0)
+            pos_loss = hp['mil_loss_weight'] * (s[0] / num_sample)
+            bag_acc = stats[1] * (100.0 / max(G * K, 1))
+            num_pos = num_sample                                                 # cpr_head.py:1216 rebinds num_pos
+            saved['num_sample'] = num_sample
+        elif hp['with_mil_loss']:
             if fused_fwd:
                 s, stats = mil_sum, mil_stats
             else:
-                bag_prob, s, stats, mil_mt, mil_lw = ops.mil_loss_fwd(bl, N, NP, weight, gt.labels, hp['eps'], want_aux=True)
+                bag_prob, s, stats, mil_mt, mil_lw = ops.mil_loss_fwd(bl, N, NP, weight, gt.labels, hp['eps'], want_aux=True, loss_kind=kind)
             saved['mil_mt'], saved['mil_lw'] = mil_mt, mil_lw
             num_sample = torch.clamp(stats[0], min=1.0)                          # multi_instance_learning_loss.py:176
             pos_loss = hp['mil_loss_weight'] * (s[0] / num_sample)
@@ -241,11 +256,16 @@ class _CPRLossFn(torch.autograd.Function):
     def _bwd_map_staged(ctx, g_gt, g_pos, g_neg, bl, weight, lmap, B, H, W, N, NP, LD, M, G, K):
         """round-1 chain (kept for grid-cell bags and as PTB_LOSS_BWD=staged): (G,K,LD) gradient tensor -> scatter-add with fp32 atomics."""
         hp, gt, sv = ctx.hp, ctx.gt, ctx.saved
-        full = hp['with_mil_loss'] and NP == N       # MIL backward then writes every column of every row
+        allpos, kind = hp['allpos'], hp['loss_kind']
+        full = hp['with_mil_loss'] and not allpos and NP == N       # MIL backward then writes every column of every row
         dbl = torch.empty_like(bl) if full else torch.zeros_like(bl)
         if hp['with_mil_loss']:
             scale = (g_pos * hp['mil_loss_weight'] / sv['num_sample']).reshape(1).float().contiguous()
-            ops.mil_loss_bwd(bl, N, NP, weight, gt.labels, hp['eps'], sv['bag_prob'], scale, grad_out=dbl)
+            if allpos:      # per-sample term on every row: x w_k (gfocal) or unweighted (BCE); the ins columns stay zero
+                ops.gfocal_bwd(bl, G * K, N, LD, gt.labels.repeat_interleave(K), weight.reshape(-1) if kind == 0 else None, hp['eps'], scale,
+                               dbl, LD, accumulate=True, loss_kind=kind)
+            else:
+                ops.mil_loss_bwd(bl, N, NP, weight, gt.labels, hp['eps'], sv['bag_prob'], scale, grad_out=dbl, loss_kind=kind)
         if hp['with_gt_loss']:
             scale = (g_gt * hp['gt_loss_weight'] / sv['num_pos_gt']).reshape(1).float().contiguous()
             ops.gfocal_bwd(bl[:, K - 1], G, N, K * LD, gt.labels, sv['valid_center'], hp['eps'], scale, dbl[:, K - 1],
@@ -274,14 +294,17 @@ class _CPRLossFn(torch.autograd.Function):
                 raise RuntimeError(msg)
             warnings.warn(msg)
         f1 = lambda t: t.reshape(1).float().contiguous()
+        # the positive-bag term: MIL (per-(bag, class) statistics of the forward) or AllPos (a per-sample term on every bag sample)
+        allpos, kind = hp['allpos'], hp['loss_kind']
+        s_bag = f1(g_pos * hp['mil_loss_weight'] / sv['num_sample'])
+        bag_kw = dict(loss_kind=kind, scale_mil=None if allpos else s_bag, scale_pos=s_bag if allpos else None)
         if path == 'tiles':
             # DETERMINISTIC mode (torch.use_deterministic_algorithms(True) or PTB_LOSS_BWD=tiles): MIL + gt + neg gfocal backward and the
             # grid_sample backward in one gather-formulated kernel, one CTA per 8x8 map tile, every sum formed by one thread in a fixed
             # order: bit-identical gradients run to run (2.2 ms at the headline batch)
             dlmap = ops.cpr_loss_bwd_map(
                 bl, weight, sv['mil_mt'], sv['bag_prob'], sv['mil_lw'], gt.labels, gt.centers, gt.img_ptr, ctx.bags.offsets, (B, H, W, LD), N, NP,
-                ctx.bags.stride, ctx.bags.reach, hp['eps'],
-                scale_mil=f1(g_pos * hp['mil_loss_weight'] / sv['num_sample']),
+                ctx.bags.stride, ctx.bags.reach, hp['eps'], **bag_kw,
                 scale_gt=f1(g_gt * hp['gt_loss_weight'] / sv['num_pos_gt']) if hp['with_gt_loss'] else None,
                 valid_center=sv['valid_center'] if hp['with_gt_loss'] else None,
                 logit_map=lmap if hp['with_neg'] else None, neg_mask=sv['neg_mask'] if hp['with_neg'] else None,
@@ -301,8 +324,7 @@ class _CPRLossFn(torch.autograd.Function):
                     ops.gfocal_bwd(lmap, M, N, LD, None, sv['neg_mask'], hp['eps'], f1(g_neg * hp['neg_loss_weight'] / ctx.num_pos), dlmap, LD,
                                    accumulate=True)
             ops.cpr_loss_bwd_scatter(bl, weight, sv['mil_mt'], sv['bag_prob'], sv['mil_lw'], gt.labels, gt.centers, gt.bag_img, ctx.bags.offsets,
-                                     dlmap, N, NP, ctx.bags.stride, hp['eps'],
-                                     scale_mil=f1(g_pos * hp['mil_loss_weight'] / sv['num_sample']),
+                                     dlmap, N, NP, ctx.bags.stride, hp['eps'], **bag_kw,
                                      scale_gt=f1(g_gt * hp['gt_loss_weight'] / sv['num_pos_gt']) if hp['with_gt_loss'] else None,
                                      valid_center=sv['valid_center'] if hp['with_gt_loss'] else None)
         else:
@@ -392,8 +414,11 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 raise NotImplementedError(f'CPRHead: {what} is not supported by the CUDA path')
         need(len(self.strides) == 1, 'more than one FPN level (the reference asserts a single level too, cpr_head.py:799,1152)')
         need(self.ins_share_head_feat, 'ins_share_head_feat=False')
-        need(self.loss_mil_cfg.get('type', 'MILLoss') == 'MILLoss', 'loss_mil.type != MILLoss')
-        need(self.loss_mil_cfg.get('loss_type', 'gfocal_loss') == 'gfocal_loss', 'MILLoss.loss_type != gfocal_loss')
+        mil_type = self.loss_mil_cfg.get('type', 'MILLoss')
+        need(mil_type in ('MILLoss', 'AllPosLoss'), f'loss_mil.type {mil_type}')
+        need(self.loss_mil_cfg.get('loss_type', 'gfocal_loss') in ops.LOSS_KINDS, f"{mil_type}.loss_type {self.loss_mil_cfg.get('loss_type')}")
+        need(mil_type != 'AllPosLoss' or self.train_pts_extractor['pos_generator']['type'] == 'CirclePtFeatGenerator',
+             'AllPosLoss with grid-cell bags (its zero-padded bag slots would be scored as samples)')
         need(self.normal_cfg['prob_cls_type'] in ('sigmoid', 'softmax', 'normed_sigmoid'), f"prob_cls_type {self.normal_cfg['prob_cls_type']}")
         need(not self.normal_cfg['out_bg_cls'], 'out_bg_cls=True')
         need(self.loss_type == 0, 'loss_type != 0')
@@ -484,7 +509,21 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 wrep = (vf[:, K - 1] * gw).reshape(-1, 1)
                 num_pos = torch.clamp((wrep > 0).sum(), min=1)
                 losses['gt_loss'] = hp['gt_loss_weight'] * (_gfocal(gt_prob, onehot, wrep, eps).sum() / num_pos)
-            if hp['with_mil_loss']:
+            if hp['with_mil_loss'] and hp['allpos']:
+                # AllPosLoss (multi_instance_learning_loss.py:206-243): rows = bag samples, label = the bag's; the reference's
+                # `loss + bag_ins_outs * 0` is reduced here as the losses are parsed (.mean()): scalar + zero gradient to the instance head
+                pw = (vf * gw.reshape(-1, 1)).reshape(G * K, 1)
+                prob = self.get_cls_prob(pos_cls).reshape(G * K, N)
+                lab_rep = labels.repeat_interleave(K)
+                oh = onehot.repeat_interleave(K, dim=0)
+                acc = (prob.argmax(dim=1) == lab_rep).float().sum().reshape(1) * (100.0 / max(G * K, 1))
+                num_sample = torch.clamp((pw > 0).float().sum(), min=1.0)
+                l_all = _gfocal(prob, oh, pw, eps) if hp['loss_kind'] == 0 else \
+                    torch.nn.functional.binary_cross_entropy(prob, oh, reduction='none')
+                losses['pos_loss'] = hp['mil_loss_weight'] * (l_all.sum() / num_sample) + (pos_ins * 0).mean()
+                losses['bag_acc'] = acc.detach()
+                num_pos = num_sample
+            elif hp['with_mil_loss']:
                 pw = vf * gw.reshape(-1, 1)                                       # (G,K) = valid * gt_weight (cpr_head.py:1211)
                 prob_cls = self.get_cls_prob(pos_cls)
                 nb = 2 if self.binary_ins else 1
@@ -496,9 +535,13 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 num_sample = torch.clamp((lw.sum(dim=-1) > 0).float().sum(), min=1.0)
                 if self.binary_ins:                                               # negative bag probability trained towards 0 (:179-186)
                     p_all = torch.cat([prob[..., 0], prob[..., 1]])
-                    l_all = _gfocal(p_all, torch.cat([onehot, torch.zeros_like(onehot)]), torch.cat([lw, lw]), eps)
+                    t_all, lw_all = torch.cat([onehot, torch.zeros_like(onehot)]), torch.cat([lw, lw])
                 else:
-                    l_all = _gfocal(prob[..., 0], onehot, lw, eps)
+                    p_all, t_all, lw_all = prob[..., 0], onehot, lw
+                if hp['loss_kind'] == 0:
+                    l_all = _gfocal(p_all, t_all, lw_all, eps)
+                else:       # binary_cross_entropy: NOT label-weighted (multi_instance_learning_loss.py:202 passes weight=None)
+                    l_all = torch.nn.functional.binary_cross_entropy(p_all, t_all, reduction='none')
                 losses['pos_loss'] = hp['mil_loss_weight'] * (l_all.sum() / num_sample)
                 losses['bag_acc'] = acc.detach()
                 num_pos = num_sample
@@ -584,6 +627,8 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                   with_gt_loss=bool(self.loss_cfg.get('with_gt_loss', False)),
                   gt_loss_weight=float(self.loss_cfg.get('gt_loss_weight', 1.0)),
                   with_mil_loss=bool(self.loss_cfg.get('with_mil_loss', True)),
+                  allpos=self.loss_mil_cfg.get('type', 'MILLoss') == 'AllPosLoss',
+                  loss_kind=ops.LOSS_KINDS[self.loss_mil_cfg.get('loss_type', 'gfocal_loss')],
                   with_neg=bool(self.loss_cfg.get('with_neg', True)),
                   neg_loss_weight=float(self.loss_cfg.get('neg_loss_weight', 1.0)),
                   neg_radius=float(neg['radius']), neg_class_wise=bool(neg.get('class_wise', False)))

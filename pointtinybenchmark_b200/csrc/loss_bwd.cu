@@ -4,8 +4,10 @@
 //   d loss / d lmap[cell][ch] =   sum over (bag g, sample k, tap t on this cell)  w_t * d loss / d bag_logit[g][k][ch]      (grid_sample backward)
 //                               + [ch < N] neg-loss term of the cell itself                                                (cpr_head.py:1219-1228)
 //   d/d cls logit = gp * pi * sg (1 - sg)   [+ centre sample: gt-loss term, cpr_head.py:1159-1184]      gp = dLoss/dprob[g][c] (gfocal')
+//                   [+ every sample: per-sample positive term s_pos * w_k * term'(sg) sg (1 - sg)  (AllPosLoss; w_k = 1 for BCE)]
 //   d/d ins logit = gp * pi * (sg - p)                                                                 pi = e w / T, e = exp(ins - m)
-//   (MILLoss.forward, multi_instance_learning_loss.py:153-203; m, 1/T, p, gfocal'(p) per (bag, class) come from the forward kernel)
+//   (MILLoss.forward, multi_instance_learning_loss.py:153-203; m, 1/T, p, gfocal'(p) per (bag, class) come from the forward kernel;
+//    term' is the loss-term functor's d/dp, cpr_loss_term.cuh.  AllPosLoss has no MIL term: coef == NULL, ins gradient 0)
 //
 // One CTA owns a tile of 8 x 8 map cells and ALL channels of it; thread (cell, 32-channel group) keeps its 32 sums in registers.
 //   A  the bags of the image whose sample window reaches the tile, in GT order (ordered ballot compaction);
@@ -22,6 +24,7 @@
 // issues about 2.5x fewer instructions.
 // Samples whose taps straddle a tile border are evaluated by each tile they touch (~1.25x).
 #include "ptb_common.cuh"
+#include "cpr_loss_term.cuh"
 #include <math_constants.h>
 
 namespace ptb {
@@ -35,23 +38,23 @@ constexpr int LB_NIT = 8;                     // class iterations per lane: up t
 constexpr int LB_MAXK = 320;                  // samples per bag handled by the 10 warps of the evaluation step
 
 __device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-__device__ __forceinline__ float gfocal_dp_f(float p, float q, float eps) {      // d/dp of -( (p-q)^2 (q log(p+eps) + (1-q) log(1-p+eps)) )
-  const float d = p - q;
-  const float L = q * __logf(p + eps) + (1.f - q) * __logf(1.f - p + eps);
-  const float dL = __fdividef(q, p + eps) - __fdividef(1.f - q, 1.f - p + eps);
-  return -(2.f * d * L + d * d * dL);
+// d/dp of the per-sample positive term (AllPosLoss): gfocal x w_k or BCE unweighted
+__device__ __forceinline__ float pos_term_dp(int kind, float p, float q, float wk, float eps) {
+  return kind == LOSS_BCE ? BceTerm{eps}.dp_fast(p, q) : wk * GfocalTerm{eps}.dp_fast(p, q);
 }
 
 struct LossBwdArgs {
   const float* bl;          // [G][K][LD] sampled logits (cls at 0, ins at NP)
   const float* weight;      // [G][K]
-  const float4* coef;       // [G][N]  (max ins, 1/T or 0, bag prob, label_weight * gfocal'(prob, onehot))
+  const float4* coef;       // [G][N]  (max ins, 1/T or 0, bag prob, dLoss/dprob of the bag term) or NULL (no MIL term)
   const int32_t* labels;    // [G]
   const float* centers;     // [G][2]
   const int32_t* img_ptr;   // [B+1]
   const float* offsets;     // [K][2]
   const float* scale_mil;   // [1] or NULL (no MIL term)
   const float* scale_gt;    // [1] or NULL
+  const float* scale_pos;   // [1] or NULL: per-sample positive term on every sample (AllPosLoss)
+  int pos_kind;             // LOSS_GFOCAL | LOSS_BCE of that term
   const float* wc;          // [G] validity of the centre sample (gt loss) or NULL
   const float* lmap;        // [B][H][W][LD] logit map (neg term) or NULL
   const uint8_t* neg_mask;  // [B][H][W][N]
@@ -87,6 +90,7 @@ cpr_loss_bwd_tile_kernel(const LossBwdArgs a) {
   const float hw = 0.5f * (float)W, hh = 0.5f * (float)H;
   const float s_mil = a.scale_mil ? a.scale_mil[0] : 0.f;
   const float s_gt = (a.scale_gt && a.wc) ? a.scale_gt[0] : 0.f;
+  const float s_pos = a.scale_pos ? a.scale_pos[0] : 0.f;
   const int g_lo = a.img_ptr[b], g_hi = a.img_ptr[b + 1];
   const int nit = (N + 31) / 32;
   float acc[32];
@@ -105,7 +109,7 @@ cpr_loss_bwd_tile_kernel(const LossBwdArgs a) {
       for (int r = warp; r < nr; r += nwarps) {
         const LbRec rec = s_rec[r0 + r];
         const float* row = a.bl + ((size_t)rec.g * K + rec.k) * LD;
-        const float4* cf = a.coef + (size_t)rec.g * N;
+        const float4* cf = a.coef ? a.coef + (size_t)rec.g * N : nullptr;
         const int lab = a.labels[rec.g];
         const float sgt = (s_gt != 0.f && rec.k == K - 1) ? s_gt * a.wc[rec.g] : 0.f;
         float* out = st + (size_t)r * LDS;
@@ -113,14 +117,20 @@ cpr_loss_bwd_tile_kernel(const LossBwdArgs a) {
         for (int i = 0; i < LB_NIT; ++i) {
           const int c = lane + 32 * i;
           if (i < nit && c < N) {
-            const float xc = __ldg(row + c), xi = __ldg(row + NP + c);
-            const float4 q = __ldg(cf + c);                                // (m, 1/T, p, lw * gfocal'(p))
+            const float xc = __ldg(row + c);
             const float sg = fast_sigmoid(xc);
-            const float gpi = s_mil * q.w * (__expf(xi - q.x) * rec.wk * q.y);
-            float dc = gpi * sg * (1.f - sg);
+            float dc = 0.f, di = 0.f;
+            if (cf) {
+              const float xi = __ldg(row + NP + c);
+              const float4 q = __ldg(cf + c);                              // (m, 1/T, p, dLoss/dprob)
+              const float gpi = s_mil * q.w * (__expf(xi - q.x) * rec.wk * q.y);
+              dc = gpi * sg * (1.f - sg);
+              di = gpi * (sg - q.z);
+            }
             if (sgt != 0.f) dc += sgt * gfocal_dp_f(sg, c == lab ? 1.f : 0.f, a.eps) * sg * (1.f - sg);
+            if (s_pos != 0.f) dc += s_pos * pos_term_dp(a.pos_kind, sg, c == lab ? 1.f : 0.f, rec.wk, a.eps) * sg * (1.f - sg);
             out[c] = dc;
-            out[NP + c] = gpi * (sg - q.z);
+            out[NP + c] = di;
           }
         }
       }
@@ -299,20 +309,22 @@ cpr_loss_bwd_scatter_kernel(const LossBwdArgs a, const int32_t* __restrict__ bag
   if (slice >= slices) return;
   const float s_mil = a.scale_mil ? a.scale_mil[0] : 0.f;
   const float sgt = (a.scale_gt && a.wc) ? a.scale_gt[0] * a.wc[g] : 0.f;
+  const float s_pos = a.scale_pos ? a.scale_pos[0] : 0.f;
+  const bool mil = a.coef != nullptr;
   const int lab = a.labels[g];
   float cm[4], cit[4], cpb[4], cgd[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int c = 4 * q + j;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (c < N) v = __ldg(a.coef + (size_t)g * N + c);
+    if (mil && c < N) v = __ldg(a.coef + (size_t)g * N + c);
     cm[j] = v.x; cit[j] = v.y; cpb[j] = v.z; cgd[j] = s_mil * v.w;
   }
   float* map = a.dlmap + (size_t)b * H * W * LD;
   for (int k = slice; k < K; k += slices) {
     const float* row = a.bl + ((size_t)g * K + k) * LD;
     const float4 xc4 = __ldcs(reinterpret_cast<const float4*>(row + 4 * q));
-    const float4 xi4 = __ldcs(reinterpret_cast<const float4*>(row + NP + 4 * q));
+    const float4 xi4 = mil ? __ldcs(reinterpret_cast<const float4*>(row + NP + 4 * q)) : make_float4(0.f, 0.f, 0.f, 0.f);
     const float wk = a.weight[(size_t)g * K + k];
     const float xc[4] = {xc4.x, xc4.y, xc4.z, xc4.w}, xi[4] = {xi4.x, xi4.y, xi4.z, xi4.w};
     float dc[4], di[4];
@@ -321,10 +333,11 @@ cpr_loss_bwd_scatter_kernel(const LossBwdArgs a, const int32_t* __restrict__ bag
     for (int j = 0; j < 4; ++j) {
       const int c = 4 * q + j;
       const float sg = fast_sigmoid(xc[j]);
-      const float gpi = cgd[j] * (__expf(xi[j] - cm[j]) * wk * cit[j]);
+      const float gpi = mil ? cgd[j] * (__expf(xi[j] - cm[j]) * wk * cit[j]) : 0.f;
       dc[j] = gpi * sg * (1.f - sg);
       di[j] = gpi * (sg - cpb[j]);
       if (centre) dc[j] += sgt * gfocal_dp_f(sg, c == lab ? 1.f : 0.f, a.eps) * sg * (1.f - sg);
+      if (s_pos != 0.f) dc[j] += s_pos * pos_term_dp(a.pos_kind, sg, c == lab ? 1.f : 0.f, wk, a.eps) * sg * (1.f - sg);
       if (c >= N) { dc[j] = 0.f; di[j] = 0.f; }
     }
     const LsTap t = s_tap[k];
@@ -334,21 +347,32 @@ cpr_loss_bwd_scatter_kernel(const LossBwdArgs a, const int32_t* __restrict__ bag
       if (w != 0.f) {
         float* base = map + (size_t)t.o[tt] * LD;
         atomicAdd(reinterpret_cast<float4*>(base + 4 * q), make_float4(w * dc[0], w * dc[1], w * dc[2], w * dc[3]));
-        atomicAdd(reinterpret_cast<float4*>(base + NP + 4 * q), make_float4(w * di[0], w * di[1], w * di[2], w * di[3]));
+        if (mil) atomicAdd(reinterpret_cast<float4*>(base + NP + 4 * q), make_float4(w * di[0], w * di[1], w * di[2], w * di[3]));
       }
     }
   }
 }
 
-// coef[g][c] = (max_k ins, 1/T or 0, bag prob, label_weight * gfocal'(prob, onehot(label)))  from the forward's outputs
+// coef[g][c] = (max_k ins, 1/T or 0, bag prob, dLoss/dprob)  from the forward's outputs;  dLoss/dprob = label_weight * gfocal'(prob,
+// onehot(label)), or BCE'(prob, onehot(label)) unweighted
+template <class Loss>
 __global__ void __launch_bounds__(256)
 mil_coef_kernel(const float* __restrict__ mt, const float* __restrict__ bag_prob, const float* __restrict__ lw,
-                const int32_t* __restrict__ labels, int G, int N, float eps, float4* __restrict__ coef) {
+                const int32_t* __restrict__ labels, int G, int N, Loss term, float4* __restrict__ coef) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= G * N) return;
   const int g = i / N, c = i - g * N;
   const float p = bag_prob[i];
-  coef[i] = make_float4(mt[2 * i], mt[2 * i + 1], p, lw[g] * gfocal_dp_f(p, c == labels[g] ? 1.f : 0.f, eps));
+  const float q = c == labels[g] ? 1.f : 0.f;
+  coef[i] = make_float4(mt[2 * i], mt[2 * i + 1], p, Loss::label_weighted ? lw[g] * term.dp_fast(p, q) : term.dp_fast(p, q));
+}
+
+static int launch_coef(int kind, const float* mt, const float* bag_prob, const float* lw, const int32_t* labels, int G, int N, float eps,
+                       float4* coef, cudaStream_t st) {
+  const unsigned blocks = (unsigned)((G * N + 255) / 256);
+  if (kind == LOSS_BCE) mil_coef_kernel<<<blocks, 256, 0, st>>>(mt, bag_prob, lw, labels, G, N, BceTerm{eps}, coef);
+  else mil_coef_kernel<<<blocks, 256, 0, st>>>(mt, bag_prob, lw, labels, G, N, GfocalTerm{eps}, coef);
+  return 0;
 }
 
 }  // namespace ptb
@@ -359,30 +383,32 @@ extern "C" uint64_t ptb_cpr_loss_bwd_map_workspace(int G, int num_classes) {
   return (uint64_t)(G > 0 ? G : 1) * (uint64_t)(num_classes > 0 ? num_classes : 1) * sizeof(float4);
 }
 
-extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                    const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
-                                    const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                    float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
-                                    const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
-                                    void* workspace, float* grad_map, void* stream) {
+extern "C" int ptb_cpr_loss_bwd_map_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                         const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
+                                         const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                         float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
+                                         const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
+                                         int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 32 * LB_NIT, "shape (num_classes <= 256)");
   PTB_REQUIRE(ld >= ins_off + num_classes && ins_off >= num_classes && stride > 0.f && reach_px >= 0.f, "ld / ins_off / stride");
   PTB_REQUIRE(ld % 32 == 0 && ld <= 512, "ld must be a multiple of 32 (32-channel register groups), at most 512");
   PTB_REQUIRE(K <= LB_MAXK, "at most 320 samples per bag");
-  PTB_REQUIRE(img_ptr && grad_map && workspace &&
-                  (G == 0 || (bag_logits && weight && mil_mt && bag_prob && label_weight && labels && centers && offsets)), "NULL input");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
+  PTB_REQUIRE(img_ptr && grad_map && workspace && (G == 0 || (bag_logits && weight && labels && centers && offsets)), "NULL input");
+  PTB_REQUIRE(!mil_mt || (bag_prob && label_weight), "the MIL term needs mil_mt, bag_prob and label_weight");
   PTB_REQUIRE(!logit_map || (neg_mask && scale_neg), "the neg term needs logit_map, neg_mask and scale_neg");
   PTB_REQUIRE(((uintptr_t)workspace % 16 == 0) && ((uintptr_t)grad_map % 16 == 0), "16-byte alignment");
   cudaStream_t st = (cudaStream_t)stream;
-  float4* coef = reinterpret_cast<float4*>(workspace);
-  if (G > 0) {
-    mil_coef_kernel<<<(G * num_classes + 255) / 256, 256, 0, st>>>(mil_mt, bag_prob, label_weight, labels, G, num_classes, eps, coef);
+  float4* coef = mil_mt ? reinterpret_cast<float4*>(workspace) : nullptr;
+  if (G > 0 && coef) {
+    launch_coef(loss_kind, mil_mt, bag_prob, label_weight, labels, G, num_classes, eps, coef, st);
     int rc = check_launch("ptb_cpr_loss_bwd_map/coef");
     if (rc) return rc;
   }
   LossBwdArgs a;
   a.bl = bag_logits; a.weight = weight; a.coef = coef; a.labels = labels;
   a.centers = centers; a.img_ptr = img_ptr; a.offsets = offsets; a.scale_mil = scale_mil; a.scale_gt = scale_gt; a.wc = valid_center;
+  a.scale_pos = scale_pos; a.pos_kind = loss_kind;
   a.lmap = logit_map; a.neg_mask = neg_mask; a.scale_neg = scale_neg; a.dlmap = grad_map;
   a.H = H; a.W = W; a.N = num_classes; a.NP = ins_off; a.LD = ld; a.K = K; a.stride = stride; a.reach_px = reach_px; a.eps = eps;
   const size_t smem = (size_t)LB_ROUND * (ld + 4) * sizeof(float);
@@ -401,25 +427,41 @@ extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight
   return check_launch("ptb_cpr_loss_bwd_map");
 }
 
-extern "C" int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                        const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
-                                        const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                        float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
-                                        void* workspace, float* grad_map, void* stream) {
+extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                    const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
+                                    const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                    float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
+                                    const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
+                                    void* workspace, float* grad_map, void* stream) {
+  PTB_REQUIRE(G == 0 || mil_mt, "NULL input");
+  return ptb_cpr_loss_bwd_map_kind(bag_logits, weight, mil_mt, bag_prob, label_weight, labels, centers, img_ptr, offsets, B, H, W, G, K,
+                                   num_classes, ins_off, ld, stride, reach_px, eps, scale_mil, scale_gt, valid_center, logit_map, neg_mask,
+                                   scale_neg, LOSS_GFOCAL, nullptr, workspace, grad_map, stream);
+}
+
+extern "C" int ptb_cpr_loss_bwd_scatter_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                             const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
+                                             const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                             float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
+                                             int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 4 * LS_THREADS, "shape");
   PTB_REQUIRE(ld >= ins_off + num_classes && ins_off >= num_classes && ins_off % 4 == 0 && ld % 4 == 0 && stride > 0.f, "ld / ins_off / stride");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
-  PTB_REQUIRE(bag_logits && weight && mil_mt && bag_prob && label_weight && labels && centers && bag_img && offsets && workspace && grad_map,
-              "NULL input");
+  PTB_REQUIRE(bag_logits && weight && labels && centers && bag_img && offsets && workspace && grad_map, "NULL input");
+  PTB_REQUIRE(!mil_mt || (bag_prob && label_weight), "the MIL term needs mil_mt, bag_prob and label_weight");
   PTB_REQUIRE(((uintptr_t)workspace % 16 == 0) && ((uintptr_t)grad_map % 16 == 0) && ((uintptr_t)bag_logits % 16 == 0), "16-byte alignment");
   cudaStream_t st = (cudaStream_t)stream;
-  float4* coef = reinterpret_cast<float4*>(workspace);
-  mil_coef_kernel<<<(G * num_classes + 255) / 256, 256, 0, st>>>(mil_mt, bag_prob, label_weight, labels, G, num_classes, eps, coef);
-  int rc = check_launch("ptb_cpr_loss_bwd_scatter/coef");
-  if (rc) return rc;
+  float4* coef = mil_mt ? reinterpret_cast<float4*>(workspace) : nullptr;
+  if (coef) {
+    launch_coef(loss_kind, mil_mt, bag_prob, label_weight, labels, G, num_classes, eps, coef, st);
+    int rc = check_launch("ptb_cpr_loss_bwd_scatter/coef");
+    if (rc) return rc;
+  }
   LossBwdArgs a;
   a.bl = bag_logits; a.weight = weight; a.coef = coef; a.labels = labels;
   a.centers = centers; a.img_ptr = nullptr; a.offsets = offsets; a.scale_mil = scale_mil; a.scale_gt = scale_gt; a.wc = valid_center;
+  a.scale_pos = scale_pos; a.pos_kind = loss_kind;
   a.lmap = nullptr; a.neg_mask = nullptr; a.scale_neg = nullptr; a.dlmap = grad_map;
   a.H = H; a.W = W; a.N = num_classes; a.NP = ins_off; a.LD = ld; a.K = K; a.stride = stride; a.reach_px = 0.f; a.eps = eps;
   const size_t smem = (size_t)K * sizeof(LsTap);
@@ -429,4 +471,15 @@ extern "C" int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* we
     return fail("%s", "ptb_cpr_loss_bwd_scatter: shared memory opt-in failed");
   cpr_loss_bwd_scatter_kernel<<<G, LS_THREADS, smem, st>>>(a, bag_img);
   return check_launch("ptb_cpr_loss_bwd_scatter");
+}
+
+extern "C" int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                        const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
+                                        const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                        float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
+                                        void* workspace, float* grad_map, void* stream) {
+  PTB_REQUIRE(G == 0 || mil_mt, "NULL input");
+  return ptb_cpr_loss_bwd_scatter_kind(bag_logits, weight, mil_mt, bag_prob, label_weight, labels, centers, bag_img, offsets, B, H, W, G, K,
+                                       num_classes, ins_off, ld, stride, eps, scale_mil, scale_gt, valid_center, LOSS_GFOCAL, nullptr,
+                                       workspace, grad_map, stream);
 }

@@ -7,6 +7,7 @@
 //   prob = (N/Z) / max(T/Z, 1e-12)                       (softmax over the bag, x valid, F.normalize(p=1), weighted sum)
 // Reductions use fixed-order trees: results are deterministic run to run.
 #include "ptb_common.cuh"
+#include "cpr_loss_term.cuh"
 #include <math_constants.h>
 
 namespace ptb {
@@ -14,17 +15,10 @@ namespace ptb {
 constexpr int MIL_KS = 4;         // sample slices per bag
 constexpr int MIL_MAXCP = 256;    // padded class lanes supported per pass
 
-__device__ __forceinline__ float gfocal_elem(float p, float q, float eps) {
-  // -( (p-q)^2 * ( q*log(p+eps) + (1-q)*log(1-p+eps) ) )
-  const float l1 = (p - q) * (p - q);
-  const float l2 = q * logf(p + eps) + (1.f - q) * logf(1.f - p + eps);
-  return -(l1 * l2);
-}
-__device__ __forceinline__ float gfocal_dp(float p, float q, float eps) {
-  const float d = p - q;
-  const float L = q * logf(p + eps) + (1.f - q) * logf(1.f - p + eps);
-  const float dL = q / (p + eps) - (1.f - q) / (1.f - p + eps);
-  return -(2.f * d * L + d * d * dL);
+// the bag loss term of the positive bags: GfocalTerm x label weight, or BceTerm unweighted (cpr_loss_term.cuh)
+template <class Loss>
+__device__ __forceinline__ float bag_term(const Loss& L, float p, float q, float lw) {
+  return Loss::label_weighted ? L.value(p, q) * lw : L.value(p, q);
 }
 
 // shared: per (slice, class) partials
@@ -67,9 +61,10 @@ __device__ __forceinline__ void mil_stats(const float* __restrict__ row0, int Kt
   m = mx; Z = z; T = t; N = n;
 }
 
+template <class Loss>
 __global__ void __launch_bounds__(MIL_KS * MIL_MAXCP)
 mil_fwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, int ins_off, const float* __restrict__ weight,
-               const int32_t* __restrict__ labels, float eps, float* __restrict__ bag_prob, float* __restrict__ aux, int G,
+               const int32_t* __restrict__ labels, Loss term, float* __restrict__ bag_prob, float* __restrict__ aux, int G,
                float* __restrict__ out_mt /*[G][C][2] = (max ins, 1/T or 0 when the normalisation clamp is active) or NULL*/) {
   __shared__ MilShared sh;
   __shared__ float s_red[MIL_MAXCP / 32];
@@ -104,7 +99,7 @@ mil_fwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
       out_mt[((size_t)g * C + cl) * 2] = m;
       out_mt[((size_t)g * C + cl) * 2 + 1] = (tn >= 1e-12f) ? 1.f / T : 0.f;       // mil_bwd's `degenerate` test
     }
-    lossc = gfocal_elem(prob, cl == l ? 1.f : 0.f, eps) * lw;
+    lossc = bag_term(term, prob, cl == l ? 1.f : 0.f, lw);
   }
   // reduce over class lanes of slice 0 (threads 0..CP-1; CP is a multiple of 32)
   float ls = warp_sum(lossc);
@@ -127,15 +122,16 @@ mil_fwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
       tot += s_red[i];
       if (s_argv[i] > best || (s_argv[i] == best && s_arg[i] < besti)) { best = s_argv[i]; besti = s_arg[i]; }
     }
-    aux[g] = tot;                       // bag loss (already x label weight)
+    aux[g] = tot;                       // bag loss (gfocal: already x label weight)
     aux[(size_t)G + g] = lw;            // bag counted in num_sample
     aux[(size_t)2 * G + g] = (besti == l) ? 1.f : 0.f;   // top-1 hit (accuracy(), losses/accuracy.py)
   }
 }
 
+template <class Loss>
 __global__ void __launch_bounds__(MIL_KS * MIL_MAXCP)
 mil_bwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, int ins_off, const float* __restrict__ weight,
-               const int32_t* __restrict__ labels, float eps, const float* __restrict__ bag_prob,
+               const int32_t* __restrict__ labels, Loss term, const float* __restrict__ bag_prob,
                const float* __restrict__ scale, float* __restrict__ grad) {
   __shared__ MilShared sh;
   const int g = blockIdx.x;
@@ -157,7 +153,7 @@ mil_bwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
   if (!act) return;
   const float p = bag_prob[(size_t)g * C + cl];
   const float q = (cl == labels[g]) ? 1.f : 0.f;
-  const float gp = scale[0] * lw * gfocal_dp(p, q, eps);     // dLoss/dprob
+  const float gp = Loss::label_weighted ? scale[0] * lw * term.dp(p, q) : scale[0] * term.dp(p, q);     // dLoss/dprob
   const bool degenerate = !(T / Z >= 1e-12f);                 // normalisation clamp active (all weights ~0): prob const
   for (int k = ks; k < Kt; k += MIL_KS) {
     const float e = expf(row0[(size_t)k * ld + ins_off + cl] - m);
@@ -182,10 +178,11 @@ mil_bwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
 constexpr int BM_THREADS = 320;
 struct BmTap { int o[4]; float w[4]; };
 
+template <class Loss>
 __global__ void __launch_bounds__(BM_THREADS)
 bag_mil_fwd_kernel(const float* __restrict__ lmap, int H, int W, int LD, int N, int NP, const float* __restrict__ centers,
                    const int32_t* __restrict__ bag_img, const float* __restrict__ offsets, int K, float stride,
-                   const int32_t* __restrict__ pad_hw, const int32_t* __restrict__ labels, float eps, float* __restrict__ bl,
+                   const int32_t* __restrict__ pad_hw, const int32_t* __restrict__ labels, Loss term, float* __restrict__ bl,
                    float* __restrict__ weight /*[G][K]*/, float* __restrict__ bag_prob, float* __restrict__ aux, int G,
                    float* __restrict__ out_mt) {
   extern __shared__ uint8_t bm_raw[];
@@ -282,7 +279,7 @@ bag_mil_fwd_kernel(const float* __restrict__ lmap, int H, int W, int LD, int N, 
         out_mt[((size_t)g * N + c) * 2] = M;
         out_mt[((size_t)g * N + c) * 2 + 1] = (tn >= 1e-12f) ? 1.f / T : 0.f;
       }
-      lossc += gfocal_elem(prob, c == l ? 1.f : 0.f, eps) * lw;
+      lossc += bag_term(term, prob, c == l ? 1.f : 0.f, lw);
       if (prob > bv) { bv = prob; bi = c; }             // ascending c inside the lane: first maximum
     }
   }
@@ -324,6 +321,61 @@ __global__ void __launch_bounds__(1024) mil_finish_kernel(const float* __restric
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------------
+// AllPosLoss forward (multi_instance_learning_loss.py:206-243): every bag sample is one row of probabilities sigmoid(cls logits) with
+// the label of its bag.  One CTA per bag, warp w takes samples w, w + 8, ..., lanes = classes.  Per bag (fixed order: warps in order,
+// lanes by warp_sum):
+//   aux[g]       = sum_k sum_c term(p[k][c], onehot) (x w_k for gfocal, unweighted for BCE: samples outside pad_shape count too)
+//   aux[G + g]   = #samples with w_k > 0            (num_sample)
+//   aux[2G + g]  = #samples whose top-1 class (first maximum) is the label  (accuracy() over all G*K samples)
+// mil_finish_kernel then adds the three over the bags in bag order.
+// ---------------------------------------------------------------------------------------------------------------------------------
+constexpr int AP_THREADS = 256;
+
+template <class Loss>
+__global__ void __launch_bounds__(AP_THREADS)
+allpos_fwd_kernel(const float* __restrict__ logits, int K, int C, int ld, const float* __restrict__ weight,
+                  const int32_t* __restrict__ labels, Loss term, float* __restrict__ aux, int G) {
+  __shared__ float s_red[3][AP_THREADS / 32];
+  const int g = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int l = labels[g];
+  float acc = 0.f, cnt = 0.f, hit = 0.f;
+  for (int k = warp; k < K; k += AP_THREADS / 32) {
+    const float* row = logits + ((size_t)g * K + k) * ld;
+    const float wk = weight[(size_t)g * K + k];
+    float bv = -CUDART_INF_F;
+    int bi = 0x7fffffff;
+    for (int c = lane; c < C; c += 32) {
+      const float p = sigmoidf_acc(row[c]);
+      const float q = c == l ? 1.f : 0.f;
+      acc += Loss::label_weighted ? term.value(p, q) * wk : term.value(p, q);
+      if (p > bv) { bv = p; bi = c; }                                        // ascending c inside the lane: first maximum
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    if (lane == 0) {
+      cnt += wk > 0.f ? 1.f : 0.f;
+      hit += bi == l ? 1.f : 0.f;
+    }
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) { s_red[0][warp] = acc; s_red[1][warp] = cnt; s_red[2][warp] = hit; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t[3] = {0.f, 0.f, 0.f};
+    for (int w = 0; w < AP_THREADS / 32; ++w)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) t[j] += s_red[j][w];
+    aux[g] = t[0];
+    aux[(size_t)G + g] = t[1];
+    aux[(size_t)2 * G + g] = t[2];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // gfocal on sigmoid(logits) with weights; fixed grid + last-block reduction (deterministic sum)
 // ------------------------------------------------------------------------------------------------
@@ -357,9 +409,10 @@ gfocal_fwd_kernel(const float* __restrict__ logits, long long M, int C, long lon
   block_partial_finish(acc, *scr, loss_sum);
 }
 
+template <class Loss>
 __global__ void __launch_bounds__(256)
 gfocal_bwd_kernel(const float* __restrict__ logits, long long M, int C, long long row_stride, const int32_t* __restrict__ tl,
-                  const void* __restrict__ weight, int wmode, float eps, const float* __restrict__ scale,
+                  const void* __restrict__ weight, int wmode, Loss term, const float* __restrict__ scale,
                   float* __restrict__ grad, long long grad_row_stride, int accumulate) {
   const long long total = M * C;
   const float sc = scale[0];
@@ -376,7 +429,7 @@ gfocal_bwd_kernel(const float* __restrict__ logits, long long M, int C, long lon
     if (w != 0.f) {
       const float p = sigmoidf_acc(logits[m * row_stride + c]);
       const float q = (tl && tl[m] == c) ? 1.f : 0.f;
-      gv = sc * w * gfocal_dp(p, q, eps) * p * (1.f - p);
+      gv = sc * w * term.dp(p, q) * p * (1.f - p);
     }
     float* dst = grad + m * grad_row_stride + c;
     *dst = accumulate ? (*dst + gv) : gv;
@@ -389,35 +442,81 @@ using namespace ptb;
 
 static int mil_cp(int C) { return ((C + 31) / 32) * 32; }
 
-extern "C" int ptb_mil_loss_fwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                const int32_t* labels, float eps, float* out_bag_prob, float* out_loss_sum, float* out_stats,
-                                float* out_mt, void* stream) {
+// runs f(term) with the loss-term functor of `kind` (LOSS_GFOCAL | LOSS_BCE); the caller has validated kind
+template <class F>
+static int with_term(int kind, float eps, F&& f) {
+  if (kind == LOSS_BCE) return f(BceTerm{eps});
+  return f(GfocalTerm{eps});
+}
+
+extern "C" int ptb_mil_loss_fwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                     const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum,
+                                     float* out_stats, float* out_mt, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
   PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
   PTB_REQUIRE(logits && weight && labels && out_bag_prob && out_loss_sum && out_stats, "NULL input");
   // aux lives behind bag_prob: caller allocates out_bag_prob with G*num_classes + 3*G floats
   float* aux = out_bag_prob + (size_t)G * num_classes;
   const int CP = mil_cp(num_classes);
   cudaStream_t st = (cudaStream_t)stream;
-  mil_fwd_kernel<<<G, MIL_KS * CP, 0, st>>>(logits, Kt, num_classes, CP, ld, ins_off, weight, labels, eps, out_bag_prob, aux, G, out_mt);
+  with_term(loss_kind, eps, [&](auto term) {
+    mil_fwd_kernel<<<G, MIL_KS * CP, 0, st>>>(logits, Kt, num_classes, CP, ld, ins_off, weight, labels, term, out_bag_prob, aux, G, out_mt);
+    return 0;
+  });
   int rc = check_launch("ptb_mil_loss_fwd");
   if (rc) return rc;
   mil_finish_kernel<<<1, 1024, 0, st>>>(aux, G, out_loss_sum, out_stats);
   return check_launch("ptb_mil_loss_fwd/finish");
 }
 
-extern "C" int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                const int32_t* labels, float eps, const float* bag_prob, const float* scale, float* grad_logits,
-                                void* stream) {
+extern "C" int ptb_mil_loss_fwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                const int32_t* labels, float eps, float* out_bag_prob, float* out_loss_sum, float* out_stats,
+                                float* out_mt, void* stream) {
+  return ptb_mil_loss_fwd_kind(logits, G, Kt, num_classes, ld, ins_off, weight, labels, eps, LOSS_GFOCAL, out_bag_prob, out_loss_sum,
+                               out_stats, out_mt, stream);
+}
+
+extern "C" int ptb_mil_loss_bwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                     const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale,
+                                     float* grad_logits, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
   PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
   PTB_REQUIRE(logits && weight && labels && bag_prob && scale && grad_logits, "NULL input");
   const int CP = mil_cp(num_classes);
-  mil_bwd_kernel<<<G, MIL_KS * CP, 0, (cudaStream_t)stream>>>(logits, Kt, num_classes, CP, ld, ins_off, weight, labels, eps,
-                                                            bag_prob, scale, grad_logits);
+  with_term(loss_kind, eps, [&](auto term) {
+    mil_bwd_kernel<<<G, MIL_KS * CP, 0, (cudaStream_t)stream>>>(logits, Kt, num_classes, CP, ld, ins_off, weight, labels, term,
+                                                              bag_prob, scale, grad_logits);
+    return 0;
+  });
   return check_launch("ptb_mil_loss_bwd");
+}
+
+extern "C" int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                const int32_t* labels, float eps, const float* bag_prob, const float* scale, float* grad_logits,
+                                void* stream) {
+  return ptb_mil_loss_bwd_kind(logits, G, Kt, num_classes, ld, ins_off, weight, labels, eps, LOSS_GFOCAL, bag_prob, scale, grad_logits,
+                               stream);
+}
+
+extern "C" int ptb_cpr_allpos_fwd(const float* logits, int G, int K, int num_classes, int ld, const float* weight, const int32_t* labels,
+                                  float eps, int loss_kind, float* aux, float* out_loss_sum, float* out_stats, void* stream) {
+  PTB_REQUIRE(G >= 0 && K > 0 && num_classes > 0 && ld >= num_classes, "shape");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
+  if (G == 0) return 0;
+  PTB_REQUIRE(logits && weight && labels && aux && out_loss_sum && out_stats, "NULL input");
+  cudaStream_t st = (cudaStream_t)stream;
+  with_term(loss_kind, eps, [&](auto term) {
+    allpos_fwd_kernel<<<G, AP_THREADS, 0, st>>>(logits, K, num_classes, ld, weight, labels, term, aux, G);
+    return 0;
+  });
+  int rc = check_launch("ptb_cpr_allpos_fwd");
+  if (rc) return rc;
+  mil_finish_kernel<<<1, 1024, 0, st>>>(aux, G, out_loss_sum, out_stats);
+  return check_launch("ptb_cpr_allpos_fwd/finish");
 }
 
 extern "C" int ptb_gfocal_sigmoid_fwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
@@ -431,27 +530,40 @@ extern "C" int ptb_gfocal_sigmoid_fwd(const float* logits, int64_t M, int num_cl
                     wmode, eps, loss_sum);
 }
 
-extern "C" int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
-                                      const int32_t* target_label, const void* weight, int wmode, float eps, const float* scale,
-                                      float* grad, int64_t grad_row_stride, int accumulate, void* stream) {
+extern "C" int ptb_sigmoid_loss_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride, const int32_t* target_label,
+                                    const void* weight, int wmode, float eps, int loss_kind, const float* scale, float* grad,
+                                    int64_t grad_row_stride, int accumulate, void* stream) {
   PTB_REQUIRE(M >= 0 && num_classes > 0 && row_stride >= num_classes && grad_row_stride >= num_classes, "shape");
   PTB_REQUIRE(wmode == 0 || wmode == 1, "wmode");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (M == 0) return 0;
   PTB_REQUIRE(logits && scale && grad, "NULL input");
   long long blocks = (M * num_classes + 255) / 256;
   const long long cap = (long long)sm_count() * 8;
   if (blocks > cap) blocks = cap;
-  gfocal_bwd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(logits, M, num_classes, row_stride, target_label, weight,
-                                                                      wmode, eps, scale, grad, grad_row_stride, accumulate);
+  with_term(loss_kind, eps, [&](auto term) {
+    gfocal_bwd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(logits, M, num_classes, row_stride, target_label, weight,
+                                                                        wmode, term, scale, grad, grad_row_stride, accumulate);
+    return 0;
+  });
   return check_launch("ptb_gfocal_sigmoid_bwd");
 }
 
-extern "C" int ptb_cpr_bag_mil_fwd(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off, const float* centers,
-                                   const int32_t* bag_img, int G, const float* offsets, int K, float stride, const int32_t* pad_hw,
-                                   const int32_t* labels, float eps, float* out_bag_logits, float* out_weight, float* out_bag_prob,
-                                   float* out_loss_sum, float* out_stats, float* out_mt, void* stream) {
+extern "C" int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
+                                      const int32_t* target_label, const void* weight, int wmode, float eps, const float* scale,
+                                      float* grad, int64_t grad_row_stride, int accumulate, void* stream) {
+  return ptb_sigmoid_loss_bwd(logits, M, num_classes, row_stride, target_label, weight, wmode, eps, LOSS_GFOCAL, scale, grad,
+                              grad_row_stride, accumulate, stream);
+}
+
+extern "C" int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off,
+                                        const float* centers, const int32_t* bag_img, int G, const float* offsets, int K, float stride,
+                                        const int32_t* pad_hw, const int32_t* labels, float eps, int loss_kind, float* out_bag_logits,
+                                        float* out_weight, float* out_bag_prob, float* out_loss_sum, float* out_stats, float* out_mt,
+                                        void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 128 && stride > 0.f, "shape (num_classes <= 128)");
   PTB_REQUIRE(ld % 4 == 0 && ins_off % 4 == 0 && ins_off >= num_classes && ld >= ins_off + ((num_classes + 3) / 4) * 4, "ld / ins_off");
+  PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
   PTB_REQUIRE(logit_map && centers && bag_img && offsets && pad_hw && labels && out_bag_logits && out_weight && out_bag_prob && out_loss_sum &&
                   out_stats, "NULL input");
@@ -459,14 +571,27 @@ extern "C" int ptb_cpr_bag_mil_fwd(const float* logit_map, int B, int H, int W, 
   const int ng = (num_classes + 3) / 4, slices = BM_THREADS / ng;
   const size_t smem = (size_t)K * sizeof(BmTap) + (size_t)((K + 3) & ~3) * sizeof(float) + (size_t)slices * 4 * ng * sizeof(float4);
   PTB_REQUIRE(smem <= 200 * 1024, "bag too large for shared memory");
-  if (smem > 40 * 1024 && cudaFuncSetAttribute(bag_mil_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-    return fail("%s", "ptb_cpr_bag_mil_fwd: shared memory opt-in failed");
   float* aux = out_bag_prob + (size_t)G * num_classes;          // caller allocates G*num_classes + 3*G floats (like ptb_mil_loss_fwd)
   cudaStream_t st = (cudaStream_t)stream;
-  bag_mil_fwd_kernel<<<G, BM_THREADS, smem, st>>>(logit_map, H, W, ld, num_classes, ins_off, centers, bag_img, offsets, K, stride, pad_hw,
-                                                  labels, eps, out_bag_logits, out_weight, out_bag_prob, aux, G, out_mt);
-  int rc = check_launch("ptb_cpr_bag_mil_fwd");
+  int rc = with_term(loss_kind, eps, [&](auto term) {
+    if (smem > 40 * 1024 &&
+        cudaFuncSetAttribute(bag_mil_fwd_kernel<decltype(term)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      return fail("%s", "ptb_cpr_bag_mil_fwd: shared memory opt-in failed");
+    bag_mil_fwd_kernel<<<G, BM_THREADS, smem, st>>>(logit_map, H, W, ld, num_classes, ins_off, centers, bag_img, offsets, K, stride, pad_hw,
+                                                    labels, term, out_bag_logits, out_weight, out_bag_prob, aux, G, out_mt);
+    return 0;
+  });
+  if (rc) return rc;
+  rc = check_launch("ptb_cpr_bag_mil_fwd");
   if (rc) return rc;
   mil_finish_kernel<<<1, 1024, 0, st>>>(aux, G, out_loss_sum, out_stats);
   return check_launch("ptb_cpr_bag_mil_fwd/finish");
+}
+
+extern "C" int ptb_cpr_bag_mil_fwd(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off, const float* centers,
+                                   const int32_t* bag_img, int G, const float* offsets, int K, float stride, const int32_t* pad_hw,
+                                   const int32_t* labels, float eps, float* out_bag_logits, float* out_weight, float* out_bag_prob,
+                                   float* out_loss_sum, float* out_stats, float* out_mt, void* stream) {
+  return ptb_cpr_bag_mil_fwd_kind(logit_map, B, H, W, ld, num_classes, ins_off, centers, bag_img, G, offsets, K, stride, pad_hw, labels, eps,
+                                  LOSS_GFOCAL, out_bag_logits, out_weight, out_bag_prob, out_loss_sum, out_stats, out_mt, stream);
 }
