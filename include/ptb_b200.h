@@ -331,7 +331,8 @@ int ptb_multiclass_nms_boxes(const float* boxes /*[B][P][4]*/, const float* scor
  * ptb_multiclass_nms, but out_det[..][4] is the DECAYED score and the order is the soft-NMS selection order (non-increasing decayed
  * score).  Give either pts (pseudo boxes) or boxes.  method: 0 naive, 1 linear, 2 gaussian.
  * Images whose classes are not separated by the class offset (negative coordinates on near-square images) take an exact global
- * path, like ptb_multiclass_nms. */
+ * path, like ptb_multiclass_nms.  Naive needs iou_thr > 0.  Gaussian refuses an image with two candidate boxes of zero area (after
+ * the class offset) or one of negative / NaN area, where mmcv's weight exp(-(0/0)^2 / sigma) is NaN: out_count[b] = -1 there. */
 int ptb_multiclass_soft_nms(const float* pts /*[B][P][2] or NULL*/, const float* boxes /*[B][P][4] or NULL*/,
                             const float* scores /*[B][P][C]*/, int B, int P, int num_classes, float pseudo_w, float pseudo_h,
                             float score_thr, float iou_thr, float sigma, float min_score, int method, int max_per_img,

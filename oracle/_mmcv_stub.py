@@ -120,9 +120,20 @@ def batched_nms(boxes, scores, idxs, nms_cfg, class_agnostic=False):
         b = boxes + (idxs.to(boxes) * (boxes.max() + 1))[:, None]
     t = cfg.pop('type', 'nms')
     assert t == 'nms'
-    cfg.pop('split_thr', None)
-    dets, keep = nms(b, scores, **cfg)
-    return torch.cat([boxes[keep], dets[:, -1:]], -1), keep
+    split_thr = cfg.pop('split_thr', 10000)
+    if len(b) < split_thr:
+        dets, keep = nms(b, scores, **cfg)
+        return torch.cat([boxes[keep], dets[:, -1:]], -1), keep
+    # mmcv 1.3.x at split_thr boxes or more: NMS class by class (by idxs, also when class_agnostic), kept entries sorted by
+    # score (restated, unpinned)
+    total = torch.zeros(scores.shape, dtype=torch.bool)
+    for c in torch.unique(idxs):
+        m = (idxs == c).nonzero(as_tuple=False).view(-1)
+        total[m[nms(b[m], scores[m], **cfg)[1]]] = True
+    keep = total.nonzero(as_tuple=False).view(-1)
+    sc, inds = scores[keep].sort(descending=True, stable=True)
+    keep = keep[inds]
+    return torch.cat([boxes[keep], sc[:, None]], -1), keep
 
 
 def sigmoid_focal_loss(pred, target, gamma=2.0, alpha=0.25, weight=None, reduction='none'):

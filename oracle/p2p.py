@@ -290,24 +290,57 @@ def soft_nms(boxes, scores, iou_threshold=0.3, sigma=0.5, min_score=1e-3, method
     return torch.from_numpy(dets[:n].copy()), torch.from_numpy(inds[:n].copy())
 
 
+SPLIT_THR = 10000
+
+
+def _split_branch(boxes_for_nms, scores, idxs, nms_op):
+    """batched_nms at split_thr candidates or more: nms_op(boxes, scores) -> (dets, keep) class by class (by `idxs`, also when
+    class_agnostic dropped the offset) on the boxes given, then the kept entries sorted by their score after NMS, descending - for
+    soft-NMS the DECAYED score (dets[:, -1]); versions early in mmcv's 1.3.2..1.4.0 window may sort by the original scores.  mmcv's
+    sort has no tie contract; here ties keep the candidate order (ascending flat id), as the kernels' merge does.  Restated from
+    SURVEY.md's description of mmcv 1.3.x: unpinned."""
+    total = torch.zeros(scores.shape, dtype=torch.bool)
+    after = scores.new_zeros(scores.shape)
+    for c in torch.unique(idxs):
+        m = (idxs == c).nonzero(as_tuple=False).view(-1)
+        dets, keep = nms_op(boxes_for_nms[m], scores[m])
+        total[m[keep]] = True
+        after[m[keep]] = dets[:, -1]
+    keep = total.nonzero(as_tuple=False).view(-1)
+    sc, inds = after[keep].sort(descending=True, stable=True)
+    return sc, keep[inds]
+
+
 def batched_soft_nms(boxes, scores, idxs, nms_cfg):
-    """batched_nms with nms_cfg['type'] == 'soft_nms' (mmcv/ops/nms.py): class offset, soft_nms on everything, boxes[keep] with the
-    DECAYED scores of dets[:, -1]."""
+    """batched_nms with nms_cfg['type'] == 'soft_nms' (mmcv/ops/nms.py): class offset, then soft_nms on everything (fewer than
+    nms_cfg.get('split_thr', 10000) candidates) or class by class (the split branch); boxes[keep] with the DECAYED scores."""
     cfg = {k: v for k, v in nms_cfg.items() if k not in ('type', 'split_thr', 'class_agnostic')}
-    b = boxes if nms_cfg.get('class_agnostic', False) else boxes + (idxs.to(boxes) * (boxes.max() + 1))[:, None]
-    dets, keep = soft_nms(b, scores, **cfg)
-    return torch.cat([boxes[keep], dets[:, -1:]], -1), keep
+    agnostic = nms_cfg.get('class_agnostic', False)
+    b = boxes if agnostic else boxes + (idxs.to(boxes) * (boxes.max() + 1))[:, None]
+    if len(boxes) < nms_cfg.get('split_thr', SPLIT_THR):
+        dets, keep = soft_nms(b, scores, **cfg)
+        return torch.cat([boxes[keep], dets[:, -1:]], -1), keep
+    sc, keep = _split_branch(b, scores, idxs, lambda bb, ss: soft_nms(bb, ss, **cfg))
+    return torch.cat([boxes[keep], sc[:, None]], -1), keep
 
 
-def batched_nms(boxes, scores, idxs, iou_threshold, class_agnostic=False):
-    """mmcv.ops.nms.batched_nms: offset every box by label*(boxes.max()+1) then plain NMS.
+def batched_nms(boxes, scores, idxs, iou_threshold, class_agnostic=False, split_thr=SPLIT_THR):
+    """mmcv.ops.nms.batched_nms: offset every box by label*(boxes.max()+1), then plain NMS over everything (fewer than split_thr
+    boxes) or class by class with the kept entries sorted by score (the split branch, which loops over `idxs` even when class_agnostic).
     returns dets (k,5) [original boxes, score] and keep."""
     if class_agnostic:
         b = boxes
     else:
         b = boxes + (idxs.to(boxes) * (boxes.max() + 1))[:, None]
-    keep = nms(b, scores, iou_threshold)
-    return torch.cat([boxes[keep], scores[keep, None]], -1), keep
+    if len(boxes) < split_thr:
+        keep = nms(b, scores, iou_threshold)
+        return torch.cat([boxes[keep], scores[keep, None]], -1), keep
+
+    def op(bb, ss):
+        k = nms(bb, ss, iou_threshold)
+        return ss[k, None], k
+    sc, keep = _split_branch(b, scores, idxs, op)
+    return torch.cat([boxes[keep], sc[:, None]], -1), keep
 
 
 def multiclass_nms(multi_bboxes, multi_scores, score_thr, iou_threshold, max_num=-1, nms_cfg=None, score_factors=None):
@@ -333,7 +366,8 @@ def multiclass_nms(multi_bboxes, multi_scores, score_thr, iou_threshold, max_num
     if nms_cfg is not None and nms_cfg.get('type', 'nms') == 'soft_nms':
         dets, keep = batched_soft_nms(bboxes, scores, labels, nms_cfg)
     else:
-        dets, keep = batched_nms(bboxes, scores, labels, iou_threshold, class_agnostic=bool(nms_cfg and nms_cfg.get('class_agnostic', False)))
+        dets, keep = batched_nms(bboxes, scores, labels, iou_threshold, class_agnostic=bool(nms_cfg and nms_cfg.get('class_agnostic', False)),
+                                 split_thr=(nms_cfg or {}).get('split_thr', SPLIT_THR))
     if max_num > 0:
         dets, keep = dets[:max_num], keep[:max_num]
     return dets, labels[keep], keep, inds

@@ -17,13 +17,24 @@ namespace ptb {
 
 constexpr int NMS_MAXP = 4096;      // points per image supported (nms_pre)
 constexpr int NMS_T0 = 1024;
+// mmcv batched_nms's default split_thr: from this many candidates on it runs NMS class by class and sorts the kept entries by
+// score, so the classes never interact whatever the offset does - the per-class kernels and the merge are that branch exactly
+constexpr int NMS_SPLIT_THR = 10000;
 
 struct NmsImg {       // per-image header in the workspace
   float max_coord;
   int cand_count;
-  int slow;           // 1: boxes of adjacent classes may overlap despite the class offset -> exact global path
-  int pad;
+  int slow;           // 1: boxes of adjacent classes may overlap despite the class offset (and cand_count < NMS_SPLIT_THR)
+                      //    -> exact global path
+  int degenerate;     // gaussian soft-NMS: candidates whose offset box has zero area (1 each) or a negative / NaN area (2 each)
 };
+
+// Gaussian soft-NMS weighs by exp(-IoU^2 / sigma) even where IoU = 0/0 = NaN: two zero-area boxes (of any classes, disjoint or
+// not) turn a score into NaN in mmcv's loop, and what happens next depends on mmcv's swap arrangement (the NaN never compares
+// above anything, never drops below min_score), which neither the per-class decomposition nor the global kernel reproduce.  A
+// box of negative area can meet any box with a union of 0.  The gaussian method therefore refuses an image whose candidates
+// weigh >= 2 here: its out_count is -1.  Hard NMS, naive and linear only compare the IoU, and NaN compares false everywhere.
+__device__ __forceinline__ int degenerate_weight(float area) { return area > 0.f ? 0 : (area == 0.f ? 1 : 2); }
 
 struct Box {
   float x1, y1, x2, y2, area;
@@ -135,7 +146,8 @@ nms_prepare_kernel(const float* __restrict__ pts, const float* __restrict__ boxe
     for (int w = 1; w < NMS_T0 / 32; ++w) m = fmaxf(m, s_max[w]);
     hdr[b].max_coord = m;
     hdr[b].cand_count = running;
-    hdr[b].slow = s_slow;
+    hdr[b].slow = s_slow && running < NMS_SPLIT_THR;   // the exact global path replays the offset branch only
+    hdr[b].degenerate = 0;
     out_cand_count[b] = running;
   }
 }
@@ -247,6 +259,10 @@ nms_merge_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
   extern __shared__ int head[];   // [C]
   const int b = blockIdx.x, lane = threadIdx.x;
   if (hdr[b].slow) return;
+  if (hdr[b].degenerate >= 2) {   // gaussian soft-NMS only (the class kernel counts nothing otherwise)
+    if (lane == 0) out_count[b] = -1;
+    return;
+  }
   for (int c = lane; c < C; c += 32) head[c] = 0;
   __syncwarp();
   const float* sc = scores + (size_t)b * P * C;
@@ -295,6 +311,7 @@ nms_merge_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
 // classes are disjoint after the class offset and every soft-NMS weight is exactly 1 at IoU 0, so the sequential algorithm
 // decomposes per class exactly like hard NMS; scores only decay, so a class's selections come out in non-increasing score
 // order and the image's first max_per_img detections are a C-way merge of the first <= max_per_img selections of every class.
+// (The gaussian weight is exactly 1 at IoU 0 but NaN at 0/0: images with degenerate boxes are refused, see degenerate_weight.)
 // One CTA per (image, class): candidates (ascending point index = the reference's array order) live in shared memory; per
 // selection one block-wide arg-max (highest score, lowest position) and one parallel decay pass.
 // method: 0 naive (weight 0 when IoU >= thr), 1 linear (1 - IoU when IoU >= thr), 2 gaussian (exp(-IoU^2 / sigma)).
@@ -314,7 +331,7 @@ __device__ __forceinline__ float soft_weight(float ovr, float iou_thr, float sig
 __global__ void __launch_bounds__(SNMS_T)
 soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C,
                       float hw, float hh, float score_thr, float iou_thr, float sigma, float min_score, int method, int max_keep,
-                      const NmsImg* __restrict__ hdr, int32_t* __restrict__ cls_cnt, int32_t* __restrict__ cls_list,
+                      NmsImg* __restrict__ hdr, int32_t* __restrict__ cls_cnt, int32_t* __restrict__ cls_list,
                       float* __restrict__ cls_score) {
   extern __shared__ float sm[];                 // x1 | y1 | x2 | y2 | area | score : [P] each, then idx [P] (int), alive [P] (u8)
   float* bx1 = sm; float* by1 = sm + P; float* bx2 = sm + 2 * P; float* by2 = sm + 3 * P; float* bar = sm + 4 * P; float* bsc = sm + 5 * P;
@@ -349,6 +366,11 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
     }
     n += total;
     __syncthreads();
+  }
+  if (method == 2) {          // degenerate boxes of the whole image, summed over its classes; the merge refuses the image
+    int d = 0;
+    for (int j = threadIdx.x; j < n; j += SNMS_T) d += degenerate_weight(bar[j]);
+    if (d) atomicAdd(&hdr[b].degenerate, d);
   }
   int nk = 0;
   while (nk < max_keep) {
@@ -418,8 +440,23 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
   float* st = state + (size_t)b * P * C;
   const float m1 = __fadd_rn(hdr[b].max_coord, 1.f);
   const int N = P * C;
-  for (int e = threadIdx.x; e < N; e += NMS_T0) st[e] = sc[e] > score_thr ? sc[e] : -1.f;
+  __shared__ int s_deg;
+  if (threadIdx.x == 0) s_deg = 0;
   __syncthreads();
+  int deg = 0;
+  for (int e = threadIdx.x; e < N; e += NMS_T0) {
+    st[e] = sc[e] > score_thr ? sc[e] : -1.f;
+    if (method == 2 && sc[e] > score_thr) {
+      const int p = e / C, c = e - p * C;
+      deg += degenerate_weight(offset_box(raw_box(pp, bx, p, hw, hh), __fmul_rn((float)c, m1)).area);
+    }
+  }
+  if (deg) atomicAdd(&s_deg, deg);
+  __syncthreads();
+  if (s_deg >= 2) {           // see degenerate_weight
+    if (threadIdx.x == 0) out_count[b] = -1;
+    return;
+  }
   int nk = 0;
   while (nk < max_keep) {
     unsigned long long mine = 0xFFFFFFFFFFFFFFFFull;
@@ -478,7 +515,8 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
   if (threadIdx.x == 0) out_count[b] = nk;
 }
 
-// Exact global path (rare: near-square images with candidates in both extreme corners).  One CTA per flagged image
+// Exact global path (rare: near-square images with candidates in both extreme corners and fewer than NMS_SPLIT_THR
+// candidates; from NMS_SPLIT_THR on, batched_nms itself goes class by class).  One CTA per flagged image
 // walks the candidates in descending (score, flat id) order - one block-wide arg-min per examined candidate - and
 // tests each against the <= max_keep kept boxes of ALL classes on the offset coordinates, i.e. the reference's
 // batched_nms literally, stopping at max_keep.
@@ -638,6 +676,8 @@ extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, con
   PTB_REQUIRE(max_per_img > 0 && max_per_img <= 1024, "max_per_img must be in [1,1024]");
   PTB_REQUIRE(method >= 0 && method <= 2, "method: 0 naive, 1 linear, 2 gaussian");
   PTB_REQUIRE(method != 2 || sigma > 0.f, "sigma must be > 0 for the gaussian method");
+  // naive weight at IoU 0 is 0 when iou_thr <= 0: a selection would zero every other class too (no per-class decomposition)
+  PTB_REQUIRE(method != 0 || iou_thr > 0.f, "the naive method needs iou_thr > 0 (per-class decomposition)");
   PTB_REQUIRE((pts != nullptr) != (boxes != nullptr), "give either pts (pseudo boxes) or boxes");
   PTB_REQUIRE(scores && out_count && out_det && out_label && out_keep && out_cand_count, "NULL input");
   PTB_REQUIRE(workspace && workspace_bytes >= ptb_multiclass_soft_nms_workspace(B, P, num_classes), "workspace too small");
@@ -653,8 +693,9 @@ extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, con
   nms_prepare_kernel<<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
   if ((rc = check_launch("ptb_multiclass_soft_nms/prepare"))) return rc;
   const size_t smem = (size_t)P * (7 * sizeof(float) + 1) + 16;
-  if (smem > 48 * 1024 &&      // per-device attribute: set whenever it is needed (a process may drive several devices)
-      cudaFuncSetAttribute(soft_nms_class_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+  // the kernel's own 104 B of static shared memory count against the 48 KB default too (P = 1691..1694 have smem <= 48 KB but fail
+  // to launch without the opt-in): set the per-device attribute on every call (a process may drive several devices)
+  if (cudaFuncSetAttribute(soft_nms_class_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return fail("%s", "ptb_multiclass_soft_nms: shared memory opt-in failed");
   dim3 g1(num_classes, B);
   soft_nms_class_kernel<<<g1, SNMS_T, smem, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,

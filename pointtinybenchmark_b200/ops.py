@@ -563,6 +563,11 @@ def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max
                                       B, P, C, float(wh[0]), float(wh[1]), float(score_thr), float(iou_thr), float(sigma),
                                       float(min_score), SOFT_NMS_METHODS[method], int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab),
                                       _ptr(keep), _ptr(cc), _ptr(ws), nbytes, _stream()), 'ptb_multiclass_soft_nms')
+    if method == 'gaussian':              # refused images (count -1): one device read, gaussian only
+        bad = torch.nonzero(cnt < 0).flatten().tolist()
+        if bad:
+            raise RuntimeError(f'ptb_multiclass_soft_nms: gaussian soft-NMS refused image(s) {bad}: two candidate boxes of zero area '
+                               '(or one of negative area) give IoU 0/0 = NaN weights')
     return cnt, det, lab, keep, cc
 
 

@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .post_processing import check_split_thr
 from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
 from .registry import CfgNode, register_head
 
@@ -304,6 +305,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
                                   self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
         wh = cfg.get('pseudo_wh', (16, 16))
         nms = cfg.get('nms')
+        check_split_thr(nms)
         if nms.get('type', 'nms') == 'soft_nms':       # batched_nms dispatches on nms_cfg['type'] (mmcv/ops/nms.py)
             cnt, det, lab, keep, cc = ops.multiclass_soft_nms(pts, scores, wh, cfg.get('score_thr'), nms.get('iou_threshold', 0.3),
                                                               cfg.get('max_per_img'), nms.get('sigma', 0.5),
@@ -370,6 +372,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         if boxes.shape[0] == 0 or scores.shape[1] == 0:
             return [(boxes.new_zeros((0, 5)), boxes.new_zeros((0,), dtype=torch.long))]
         nms = cfg.get('nms')
+        check_split_thr(nms)
         if nms.get('type', 'nms') == 'soft_nms':
             cnt, det, lab, _, _ = ops.multiclass_soft_nms(boxes[None], scores[None], None, cfg.get('score_thr'),
                                                           nms.get('iou_threshold', 0.3), cfg.get('max_per_img'), nms.get('sigma', 0.5),

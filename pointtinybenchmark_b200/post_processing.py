@@ -7,6 +7,13 @@ import torch
 from . import ops
 
 
+def check_split_thr(nms_cfg):
+    """mmcv's batched_nms switches to class-by-class NMS at `split_thr` candidates (default 10000); the NMS kernels hard-code that
+    default, so any other value would silently give the other branch's answer."""
+    if nms_cfg.get('split_thr', 10000) != 10000:
+        raise NotImplementedError(f"nms split_thr={nms_cfg.get('split_thr')}: only mmcv's default 10000 is implemented")
+
+
 def multiclass_nms(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num=-1, score_factors=None, return_inds=False):
     """bbox_nms.py:7-94.  Options beyond what the point heads use (round 2, pinned by tests/golden/multiclass_nms_options.npz):
     `score_factors` (>= 0; the threshold sees the raw scores, the NMS ranks by the products, bbox_nms.py:52-62), class-specific boxes
@@ -22,6 +29,7 @@ def multiclass_nms(multi_bboxes, multi_scores, score_thr, nms_cfg, max_num=-1, s
     if max_num > 1024:
         raise NotImplementedError('max_num must be <= 1024')
     kmax = 1024 if unlimited else int(max_num)
+    check_split_thr(nms_cfg)
     cfg = dict(nms_cfg)
     kind = cfg.pop('type', 'nms')
     agnostic = bool(cfg.pop('class_agnostic', False))
