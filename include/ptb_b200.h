@@ -352,6 +352,37 @@ int ptb_p2p_cost_matrix(const float* cls_logits /*[Q][C]*/, const float* pts /*[
                         float w_cls, float alpha, float gamma, float eps, float w_dis, float fx, float fy,
                         float* cost, void* stream);
 
+/* Hungarian cost matrix over a list of match costs — HungarianAssignerV2.assign's `sum(cls_costs) + sum(reg_costs)`
+ * (hungarian_assigner.py:223-227) for the point costs of match_cost.py:
+ *   PTB_MATCH_COST_FOCAL        FocalLossCost(weight, alpha, gamma, eps)                    (classification)
+ *   PTB_MATCH_COST_CLS_SIGMOID  ClassificationCostV2(use_sigmoid=True):  -sigmoid(x)[:, l] * w
+ *   PTB_MATCH_COST_CLS_SOFTMAX  ClassificationCostV2(use_sigmoid=False): -softmax(x, -1)[:, l] * w over all num_cols columns
+ *   PTB_MATCH_COST_ZERO         ZeroCost (contributes 0)
+ *   PTB_MATCH_COST_DIS          DisCostV2(weight, norm_with_img_wh, p = 1 or 2) on (x, y)     (regression)
+ * The classification terms are summed in list order from 0, the DisCostV2 terms likewise, then the two sums are added.  At most
+ * PTB_MAX_MATCH_COST_TERMS of each.  DisCostV2 divides by (img_w, img_h) when norm_with_img_wh is set.  p = 2 follows torch.cdist's
+ * CPU dispatch: the matmul formulation when n_rows > 25 or n_gt > 25, the direct one otherwise.
+ * workspace: ptb_p2p_cost_matrix_terms_workspace(n_rows) bytes when a CLS_SOFTMAX term is listed (per-row softmax statistics),
+ * else may be NULL. */
+#define PTB_MATCH_COST_FOCAL 0
+#define PTB_MATCH_COST_CLS_SIGMOID 1
+#define PTB_MATCH_COST_CLS_SOFTMAX 2
+#define PTB_MATCH_COST_ZERO 3
+#define PTB_MATCH_COST_DIS 4
+#define PTB_MAX_MATCH_COST_TERMS 8
+typedef struct {
+  int32_t kind;                             /* PTB_MATCH_COST_* */
+  float weight, alpha, gamma, eps;          /* alpha, gamma, eps: FocalLossCost only */
+  int32_t p;                                /* DisCostV2 only: 1 or 2 */
+  int32_t norm_with_img_wh;                 /* DisCostV2 only */
+} ptb_match_cost;
+int ptb_p2p_cost_matrix_terms(const float* cls_logits /*[Q][num_cols]*/, const float* pts /*[Q][ldp]*/, int ldp,
+                              const int32_t* row_idx /*[n_rows] or NULL*/, int n_rows, int num_cols,
+                              const float* gts /*[n_gt][2]*/, const int32_t* gt_labels, int n_gt,
+                              const ptb_match_cost* terms, int n_terms, float img_w, float img_h,
+                              float* cost, void* workspace, uint64_t workspace_bytes, void* stream);
+uint64_t ptb_p2p_cost_matrix_terms_workspace(int n_rows);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * RPN proposals for dense anchors — replaces RPNHead._get_bboxes (mmdet/models/dense_heads/rpn_head.py:78-186) with the grid
  * anchors of AnchorGenerator (mmdet/core/anchor/anchor_generator.py:207-270), DeltaXYWHBBoxCoder.decode

@@ -18,6 +18,12 @@ class RefineCfg(ctypes.Structure):
     _fields_ = [('merge_th', c_float), ('gt_alpha', c_float), ('refine_th', c_float), ('flags', ctypes.c_int32)]
 
 
+class MatchCost(ctypes.Structure):
+    """ptb_match_cost: one term of ptb_p2p_cost_matrix_terms."""
+    _fields_ = [('kind', ctypes.c_int32), ('weight', c_float), ('alpha', c_float), ('gamma', c_float), ('eps', c_float),
+                ('p', ctypes.c_int32), ('norm_with_img_wh', ctypes.c_int32)]
+
+
 P = c_void_p
 # name -> (restype, argtypes); must list every symbol of include/ptb_b200.h (tests/test_capi_symbols.py checks)
 SIGNATURES = {
@@ -72,6 +78,8 @@ SIGNATURES = {
     'ptb_multiclass_nms_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_int, P, P, P, P, P, P, c_u64, P]),
     'ptb_p2p_cost_matrix': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, c_float, c_float, c_float, c_float, c_float,
                                     c_float, c_float, P, P]),
+    'ptb_p2p_cost_matrix_terms': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, P, c_int, c_float, c_float, P, P, c_u64, P]),
+    'ptb_p2p_cost_matrix_terms_workspace': (c_u64, [c_int]),
     'ptb_rpn_proposals_workspace': (c_u64, [P, c_int, c_int, c_int, c_int, c_int]),
     'ptb_rpn_proposals': (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, P, P, c_float, c_int, c_float, c_float, c_int, P, P, P, P, P, P, P, P, c_u64, P]),
     'ptb_hungarian_v2_workspace': (c_u64, [c_int, c_int]),

@@ -66,25 +66,96 @@ class PointAssigner:
         return AssignResult(g.shape[0], gt_inds, None, labels)
 
 
+MAX_MATCH_COST_TERMS = 8        # per list (PTB_MAX_MATCH_COST_TERMS)
+_BOX_COSTS = ('BBoxL1Cost', 'IoUCost', 'IoUCostV2')
+
+
+def match_cost_terms(cls_costs, reg_costs):
+    """HungarianAssignerV2's cls_costs / reg_costs (a dict or a list of dicts each, hungarian_assigner.py:160-163) -> the ordered term
+    list of ops.p2p_cost_matrix_terms: the classification terms, then the DisCostV2 terms, each in config order.  Raises
+    NotImplementedError, naming the type, for every cost this matching does not compute."""
+    def as_list(c):
+        return list(c) if isinstance(c, (list, tuple)) else [c]
+
+    def common(c, t):
+        if t == 'ClassificationCost':
+            raise NotImplementedError('ClassificationCost is not implemented: it computes -softmax(x)[:, label] * weight, which '
+                                      "ClassificationCostV2(use_sigmoid=False) computes; use that")
+        if t in _BOX_COSTS:
+            raise NotImplementedError(f'{t} is a box cost; the point matching takes FocalLossCost, ClassificationCostV2, ZeroCost '
+                                      'and DisCostV2')
+        raise NotImplementedError(f'match cost {t}')
+
+    terms = []
+    cls_l, reg_l = as_list(cls_costs), as_list(reg_costs)
+    for name, lst in (('cls_costs', cls_l), ('reg_costs', reg_l)):
+        if len(lst) > MAX_MATCH_COST_TERMS:
+            raise NotImplementedError(f'{name}: {len(lst)} costs; at most {MAX_MATCH_COST_TERMS} per list are implemented')
+    for c in cls_l:
+        c = dict(c)
+        t = c.get('type')
+        w = c.get('weight', 1.0)
+        if t == 'FocalLossCost':
+            terms.append(dict(kind=t, weight=w, alpha=c.get('alpha', 0.25), gamma=c.get('gamma', 2), eps=c.get('eps', 1e-12)))
+        elif t == 'ClassificationCostV2':
+            terms.append(dict(kind='ClassificationCostV2_sigmoid' if c.get('use_sigmoid', False) else 'ClassificationCostV2_softmax',
+                              weight=w))
+        elif t == 'ZeroCost':
+            terms.append(dict(kind=t, weight=0.0))
+        elif t == 'DisCostV2':
+            raise NotImplementedError('DisCostV2 as a classification cost: the reference calls cls_costs with (cls_pred, gt_labels)')
+        else:
+            common(c, t)
+    for c in reg_l:
+        c = dict(c)
+        t = c.get('type')
+        if t == 'DisCostV2':
+            p = c.get('p', 1)
+            if p not in (1, 2):
+                raise NotImplementedError(f'DisCostV2 p={p}: p = 1 and p = 2 are implemented')
+            terms.append(dict(kind=t, weight=c.get('weight', 1.0), p=int(p), norm_with_img_wh=bool(c.get('norm_with_img_wh', True))))
+        elif t == 'ZeroCost':
+            raise NotImplementedError('ZeroCost as a regression cost: the reference calls reg_costs with three arguments and '
+                                      'ZeroCost takes two (TypeError)')
+        elif t in ('FocalLossCost', 'ClassificationCostV2'):
+            raise NotImplementedError(f'{t} as a regression cost: the reference calls reg_costs with (bbox_pred, gt_bboxes, img_meta)')
+        else:
+            common(c, t)
+    if not terms:
+        raise NotImplementedError('HungarianAssignerV2: no match costs')
+    return terms
+
+
+def is_focal_l1_pair(terms):
+    """the shipped pair, one FocalLossCost + one DisCostV2(p=1), which ops.p2p_cost_matrix computes"""
+    return len(terms) == 2 and terms[0]['kind'] == 'FocalLossCost' and terms[1]['kind'] == 'DisCostV2' and terms[1]['p'] == 1
+
+
+def cost_matrix(cls, pts, row_idx, gts, gt_labels, terms, img_shape, out=None):
+    """the matching's cost matrix for one image on the device: the shipped pair through ops.p2p_cost_matrix, every other term list
+    through ops.p2p_cost_matrix_terms.  img_shape: (h, w, ...) of img_meta, read only when a DisCostV2 has norm_with_img_wh."""
+    norm = any(t.get('norm_with_img_wh', False) for t in terms)
+    fx, fy = (float(img_shape[1]), float(img_shape[0])) if norm else (1.0, 1.0)
+    if is_focal_l1_pair(terms):
+        fc, dc = terms
+        return ops.p2p_cost_matrix(cls, pts, row_idx, gts, gt_labels, fc['weight'], fc['alpha'], fc['gamma'], fc['eps'], dc['weight'],
+                                   fx, fy, out=out)
+    return ops.p2p_cost_matrix_terms(cls, pts, row_idx, gts, gt_labels, terms, fx, fy, out=out)
+
+
 class HungarianAssignerV2:
-    """mmdet/core/bbox/assigners/hungarian_assigner.py:149-270 for the point setting the reference uses it in (P2PHead: FocalLossCost +
-    DisCostV2 on (x, y) points): cost matrix and the <= topk_k matching rounds both on the device (ptb_p2p_cost_matrix,
-    ptb_hungarian_v2_batch); `assign` keeps the reference's argument order.  P2PHead.loss uses the batched form directly."""
+    """mmdet/core/bbox/assigners/hungarian_assigner.py:149-270 for the point setting the reference uses it in (P2PHead: cost lists of
+    FocalLossCost, ClassificationCostV2, ZeroCost and DisCostV2(p=1 or 2) on (x, y) points): cost matrix and the <= topk_k matching
+    rounds both on the device (ptb_p2p_cost_matrix or ptb_p2p_cost_matrix_terms, ptb_hungarian_v2_batch); `assign` keeps the
+    reference's argument order.  P2PHead.loss uses the batched form directly."""
 
     def __init__(self, cls_costs=None, reg_costs=None, topk_k=1):
         # the reference's defaults are the DETR costs (ClassificationCost; BBoxL1Cost + IoUCost, hungarian_assigner.py:153-158), which no
-        # CPR / P2P config uses: they are rejected below like every other unsupported cost, never silently replaced
+        # CPR / P2P config uses: they are rejected like every other unsupported cost, never silently replaced
         cc = cls_costs if cls_costs is not None else [dict(type='ClassificationCost', weight=1.)]
         rc = reg_costs if reg_costs is not None else [dict(type='BBoxL1Cost', weight=1.0, norm_with_img_size=True),
                                                       dict(type='IoUCost', iou_mode='giou', weight=1.0)]
-        cc = cc[0] if isinstance(cc, (list, tuple)) and len(cc) == 1 else cc
-        rc = rc[0] if isinstance(rc, (list, tuple)) and len(rc) == 1 else rc
-        if not isinstance(cc, dict) or not isinstance(rc, dict) or cc.get('type') != 'FocalLossCost' or rc.get('type') != 'DisCostV2':
-            raise NotImplementedError('HungarianAssignerV2: one FocalLossCost + one DisCostV2 (the P2P configs) are implemented')
-        if rc.get('p', 1) != 1:
-            raise NotImplementedError('DisCostV2 p != 1')
-        self.w_cls, self.alpha, self.gamma, self.eps = cc.get('weight', 1.0), cc.get('alpha', 0.25), cc.get('gamma', 2), cc.get('eps', 1e-12)
-        self.w_dis, self.norm_wh = rc.get('weight', 1.0), rc.get('norm_with_img_wh', True)
+        self.terms = match_cost_terms(cc, rc)
         self.topk_k = topk_k
 
     def assign(self, bbox_pred, cls_pred, gt_bboxes, gt_labels, img_meta, gt_bboxes_ignore=None, eps=1e-7):
@@ -92,17 +163,15 @@ class HungarianAssignerV2:
         if not bbox_pred.is_cuda:
             raise RuntimeError('HungarianAssignerV2 runs on CUDA tensors only; there is no CPU fallback')
         if bbox_pred.shape[-1] != 2 or (gt_bboxes.numel() > 0 and gt_bboxes.shape[-1] != 2):
-            raise NotImplementedError('HungarianAssignerV2: (x, y) points only (DisCostV2 with k*2 = 2 coordinates, as P2PHead uses it)')
+            raise NotImplementedError('HungarianAssignerV2: DisCostV2 on (x, y) points only (k*2 = 2 coordinates, as P2PHead uses it)')
         N, n = bbox_pred.shape[0], gt_bboxes.shape[0]
         dev = bbox_pred.device
         gt_inds = torch.zeros((N,), dtype=torch.long, device=dev)
         labels = torch.full((N,), -1, dtype=torch.long, device=dev)
         if N == 0 or n == 0:                        # hungarian_assigner.py:211-219: no GT -> everything background
             return AssignResult(n, gt_inds, None, labels)
-        fx, fy = (img_meta['img_shape'][1], img_meta['img_shape'][0]) if self.norm_wh else (1.0, 1.0)
-        cost = ops.p2p_cost_matrix(cls_pred.detach().float().contiguous(), bbox_pred.detach()[:, :2].float().contiguous(), None,
-                                   gt_bboxes[:, :2].float().contiguous(), gt_labels.int().contiguous(), self.w_cls, self.alpha, self.gamma,
-                                   self.eps, self.w_dis, fx, fy)
+        cost = cost_matrix(cls_pred.detach().float().contiguous(), bbox_pred.detach()[:, :2].float().contiguous(), None,
+                           gt_bboxes[:, :2].float().contiguous(), gt_labels.int().contiguous(), self.terms, img_meta.get('img_shape'))
         status = ops.hungarian_v2_batch(cost.view(-1), [(N, n)], self.topk_k, gt_inds, [0])
         st = int(status[0])
         if st:

@@ -103,28 +103,109 @@ p2p_gather_kernel(const float* __restrict__ cls_map, const float* __restrict__ r
 // ------------------------------------------------------------------------------------------------
 // cost matrix
 // ------------------------------------------------------------------------------------------------
+// FocalLossCost (match_cost.py:94-100) of one logit
+__device__ __forceinline__ float focal_cost(float x, float alpha, float gamma, float eps, float w) {
+  const float p = sigmoidf_acc(x);
+  const float pg = (gamma == 2.f) ? __fmul_rn(p, p) : powf(p, gamma);
+  const float omp = __fsub_rn(1.f, p);
+  const float og = (gamma == 2.f) ? __fmul_rn(omp, omp) : powf(omp, gamma);
+  const float neg = __fmul_rn(__fmul_rn(-logf(__fadd_rn(omp, eps)), __fsub_rn(1.f, alpha)), pg);
+  const float pos = __fmul_rn(__fmul_rn(-logf(__fadd_rn(p, eps)), alpha), og);
+  return __fmul_rn(__fsub_rn(pos, neg), w);
+}
+
+// torch.cdist(p=1) of two points already divided by the image size: |dx| + |dy|
+__device__ __forceinline__ float l1_dist(float px, float py, float gx, float gy) {
+  return __fadd_rn(fabsf(__fsub_rn(px, gx)), fabsf(__fsub_rn(py, gy)));
+}
+
+// torch.cdist(p=2) with both sides <= 25 rows (ATen's direct path, Distance.cpp cdist_impl), as the CPU build computes it:
+// sqrt(fma(dy, dy, dx * dx)).  The plain formula without the FMA (ptb_common.cuh's cdist_direct) mismatched 5 646 of 69 271
+// random pairs against torch 2.11's CPU cdist on an AVX-512 host; this order mismatched none.
+__device__ __forceinline__ float l2_dist_direct(float px, float py, float gx, float gy) {
+  const float dx = __fsub_rn(px, gx), dy = __fsub_rn(py, gy);
+  return __fsqrt_rn(__fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+}
+
+// The cost of one (row, GT) element.  row r of the matrix is proposal q = row_idx[r] of cls / pts.
+// FocalL1Cost: the shipped pair FocalLossCost + DisCostV2(p=1), cost = focal + w_dis * |d|_1 (one add, as before the term lists).
+struct FocalL1Cost {
+  const float* cls; const float* pts; int ldp, C; const float* gts; const int32_t* gt_labels;
+  float w_cls, alpha, gamma, eps, w_dis, fx, fy;
+  __device__ __forceinline__ float operator()(long long, long long q, int g) const {
+    const float cc = focal_cost(cls[q * C + gt_labels[g]], alpha, gamma, eps, w_cls);
+    const float d = l1_dist(__fdiv_rn(pts[q * ldp], fx), __fdiv_rn(pts[q * ldp + 1], fy), __fdiv_rn(gts[2 * g], fx),
+                            __fdiv_rn(gts[2 * g + 1], fy));
+    return __fadd_rn(cc, __fmul_rn(d, w_dis));
+  }
+};
+
+// TermListCost: HungarianAssignerV2's `sum(cls_costs) + sum(reg_costs)` (hungarian_assigner.py:223-227) over an ordered term list.
+// Python's sum starts from 0, so each partial sum is 0 + t_1 + t_2 + ... in fp32 (0 + -0 is +0, as torch's tensor + 0), then one add
+// of the two partials.  Classification kinds go to the first partial, DisCostV2 to the second, each in list order.
+constexpr int MAX_COST_TERMS = 2 * PTB_MAX_MATCH_COST_TERMS;
+struct CostTerms {
+  ptb_match_cost t[MAX_COST_TERMS];
+  int n;
+};
+struct TermListCost {
+  const float* cls; const float* pts; int ldp, C; const float* gts; const int32_t* gt_labels;
+  const float2* sm_stats;            // [n_rows] (max, sum of exp) of each row's softmax, when a ClassificationCostV2 softmax term is listed
+  float img_w, img_h;
+  bool use_mm;                       // torch.cdist(p=2)'s matmul formulation: either side has more than 25 rows
+  CostTerms terms;
+  __device__ __forceinline__ float operator()(long long r, long long q, int g) const {
+    float cs = 0.f, rs = 0.f;
+    const float x = cls[q * C + gt_labels[g]];
+    for (int i = 0; i < terms.n; ++i) {
+      const ptb_match_cost& t = terms.t[i];
+      switch (t.kind) {
+        case PTB_MATCH_COST_FOCAL: cs = __fadd_rn(cs, focal_cost(x, t.alpha, t.gamma, t.eps, t.weight)); break;
+        case PTB_MATCH_COST_CLS_SIGMOID: cs = __fadd_rn(cs, __fmul_rn(-sigmoidf_acc(x), t.weight)); break;
+        case PTB_MATCH_COST_CLS_SOFTMAX: {    // -(exp(x - m) / s) * w, the numerics of the softmax decode (softmax_row_stats)
+          const float2 st = sm_stats[r];
+          cs = __fadd_rn(cs, __fmul_rn(-__fdiv_rn(sleef_expf_u10(__fsub_rn(x, st.x)), st.y), t.weight));
+          break;
+        }
+        case PTB_MATCH_COST_ZERO: cs = __fadd_rn(cs, 0.f); break;
+        default: {                            // PTB_MATCH_COST_DIS: match_cost.py:208-214, the division by (w, h) first
+          const float fx = t.norm_with_img_wh ? img_w : 1.f, fy = t.norm_with_img_wh ? img_h : 1.f;
+          const float px = __fdiv_rn(pts[q * ldp], fx), py = __fdiv_rn(pts[q * ldp + 1], fy);
+          const float gx = __fdiv_rn(gts[2 * g], fx), gy = __fdiv_rn(gts[2 * g + 1], fy);
+          float d;
+          if (t.p == 1) d = l1_dist(px, py, gx, gy);
+          else if (use_mm) d = cdist_mm(px, py, sq_norm2(px, py), gx, gy, sq_norm2(gx, gy));
+          else d = l2_dist_direct(px, py, gx, gy);
+          rs = __fadd_rn(rs, __fmul_rn(d, t.weight));
+        }
+      }
+    }
+    return __fadd_rn(cs, rs);
+  }
+};
+
+template <class Cost>
 __global__ void __launch_bounds__(256)
-cost_matrix_kernel(const float* __restrict__ cls, const float* __restrict__ pts, int ldp, const int32_t* __restrict__ row_idx,
-                   long long n_rows, int C, const float* __restrict__ gts, const int32_t* __restrict__ gt_labels, int n_gt,
-                   float w_cls, float alpha, float gamma, float eps, float w_dis, float fx, float fy, float* __restrict__ cost) {
+cost_matrix_kernel(Cost cost_of, const int32_t* __restrict__ row_idx, long long n_rows, int n_gt, float* __restrict__ cost) {
   const long long total = n_rows * n_gt;
   for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256) {
     const long long r = e / n_gt;
     const int g = (int)(e - r * n_gt);
-    const long long q = row_idx ? row_idx[r] : r;
-    const float p = sigmoidf_acc(cls[q * C + gt_labels[g]]);
-    const float pg = (gamma == 2.f) ? __fmul_rn(p, p) : powf(p, gamma);
-    const float omp = __fsub_rn(1.f, p);
-    const float og = (gamma == 2.f) ? __fmul_rn(omp, omp) : powf(omp, gamma);
-    // match_cost.py:95-99
-    const float neg = __fmul_rn(__fmul_rn(-logf(__fadd_rn(omp, eps)), __fsub_rn(1.f, alpha)), pg);
-    const float pos = __fmul_rn(__fmul_rn(-logf(__fadd_rn(p, eps)), alpha), og);
-    const float cc = __fmul_rn(__fsub_rn(pos, neg), w_cls);
-    const float dx = fabsf(__fsub_rn(__fdiv_rn(pts[q * ldp], fx), __fdiv_rn(gts[2 * g], fx)));
-    const float dy = fabsf(__fsub_rn(__fdiv_rn(pts[q * ldp + 1], fy), __fdiv_rn(gts[2 * g + 1], fy)));
-    const float dc = __fmul_rn(__fadd_rn(dx, dy), w_dis);    // cdist p=1, match_cost.py:213-214
-    cost[e] = __fadd_rn(cc, dc);
+    cost[e] = cost_of(r, row_idx ? row_idx[r] : r, g);
   }
+}
+
+// per-row softmax statistics (m, s) of the rows the matching uses, for ClassificationCostV2(use_sigmoid=False).  One warp per row.
+__global__ void __launch_bounds__(256)
+cost_softmax_stats_kernel(const float* __restrict__ cls, int C, const int32_t* __restrict__ row_idx, long long n_rows,
+                          float2* __restrict__ stats) {
+  const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  const long long q = row_idx ? row_idx[r] : r;
+  float m, s, e_fg;
+  softmax_row_stats(cls + q * C, C, lane, m, s, e_fg);
+  if (lane == 0) stats[r] = make_float2(m, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -401,6 +482,11 @@ extern "C" int ptb_p2p_decode_topk_softmax(const float* cls_map, const float* re
                                nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
 }
 
+static unsigned cost_matrix_blocks(int n_rows, int n_gt) {
+  const long long blocks = ((long long)n_rows * n_gt + 255) / 256, cap = (long long)sm_count() * 8;
+  return (unsigned)(blocks > cap ? cap : blocks);
+}
+
 extern "C" int ptb_p2p_cost_matrix(const float* cls_logits, const float* pts, int ldp, const int32_t* row_idx, int n_rows,
                                    int num_classes, const float* gts, const int32_t* gt_labels, int n_gt, float w_cls,
                                    float alpha, float gamma, float eps, float w_dis, float fx, float fy, float* cost,
@@ -408,13 +494,48 @@ extern "C" int ptb_p2p_cost_matrix(const float* cls_logits, const float* pts, in
   PTB_REQUIRE(n_rows >= 0 && n_gt >= 0 && num_classes > 0 && ldp >= 2, "shape");
   if (n_rows == 0 || n_gt == 0) return 0;
   PTB_REQUIRE(cls_logits && pts && gts && gt_labels && cost, "NULL input");
-  long long blocks = ((long long)n_rows * n_gt + 255) / 256;
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  cost_matrix_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(cls_logits, pts, ldp, row_idx, n_rows, num_classes, gts,
-                                                                       gt_labels, n_gt, w_cls, alpha, gamma, eps, w_dis, fx, fy,
-                                                                       cost);
+  cost_matrix_kernel<<<cost_matrix_blocks(n_rows, n_gt), 256, 0, (cudaStream_t)stream>>>(
+      FocalL1Cost{cls_logits, pts, ldp, num_classes, gts, gt_labels, w_cls, alpha, gamma, eps, w_dis, fx, fy}, row_idx, n_rows, n_gt,
+      cost);
   return check_launch("ptb_p2p_cost_matrix");
+}
+
+extern "C" uint64_t ptb_p2p_cost_matrix_terms_workspace(int n_rows) { return (uint64_t)(n_rows > 0 ? n_rows : 0) * sizeof(float2); }
+
+extern "C" int ptb_p2p_cost_matrix_terms(const float* cls_logits, const float* pts, int ldp, const int32_t* row_idx, int n_rows,
+                                         int num_cols, const float* gts, const int32_t* gt_labels, int n_gt, const ptb_match_cost* terms,
+                                         int n_terms, float img_w, float img_h, float* cost, void* workspace, uint64_t workspace_bytes,
+                                         void* stream) {
+  PTB_REQUIRE(n_rows >= 0 && n_gt >= 0 && num_cols > 0 && ldp >= 2, "shape");
+  PTB_REQUIRE(terms && n_terms > 0, "no cost terms");
+  int n_cls = 0, n_reg = 0;
+  bool softmax = false;
+  for (int i = 0; i < n_terms && i <= MAX_COST_TERMS; ++i) {
+    const ptb_match_cost& t = terms[i];
+    PTB_REQUIRE(t.kind >= PTB_MATCH_COST_FOCAL && t.kind <= PTB_MATCH_COST_DIS, "unknown cost kind");
+    PTB_REQUIRE(t.kind != PTB_MATCH_COST_DIS || t.p == 1 || t.p == 2, "DisCostV2 p must be 1 or 2");
+    (t.kind == PTB_MATCH_COST_DIS ? n_reg : n_cls) += 1;
+    softmax = softmax || t.kind == PTB_MATCH_COST_CLS_SOFTMAX;
+  }
+  PTB_REQUIRE(n_cls <= PTB_MAX_MATCH_COST_TERMS && n_reg <= PTB_MAX_MATCH_COST_TERMS,
+              "at most 8 classification and 8 DisCostV2 terms");
+  if (n_rows == 0 || n_gt == 0) return 0;
+  PTB_REQUIRE(cls_logits && pts && gts && gt_labels && cost, "NULL input");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  float2* stats = nullptr;
+  if (softmax) {
+    PTB_REQUIRE(workspace && workspace_bytes >= ptb_p2p_cost_matrix_terms_workspace(n_rows), "workspace too small");
+    stats = reinterpret_cast<float2*>(workspace);
+    cost_softmax_stats_kernel<<<(unsigned)(((long long)n_rows * 32 + 255) / 256), 256, 0, st>>>(cls_logits, num_cols, row_idx, n_rows,
+                                                                                              stats);
+    if ((rc = check_launch("ptb_p2p_cost_matrix_terms/softmax_stats"))) return rc;
+  }
+  TermListCost c{cls_logits, pts, ldp, num_cols, gts, gt_labels, stats, img_w, img_h, n_rows > 25 || n_gt > 25, {}};
+  for (int i = 0; i < n_terms; ++i) c.terms.t[i] = terms[i];
+  c.terms.n = n_terms;
+  cost_matrix_kernel<<<cost_matrix_blocks(n_rows, n_gt), 256, 0, st>>>(c, row_idx, n_rows, n_gt, cost);
+  return check_launch("ptb_p2p_cost_matrix_terms");
 }
 
 extern "C" uint64_t ptb_point_assigner_workspace(int N, int n) {

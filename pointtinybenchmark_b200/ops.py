@@ -592,6 +592,42 @@ def p2p_cost_matrix(cls_logits, pts, row_idx, gts, gt_labels, w_cls, alpha, gamm
     return cost
 
 
+MATCH_COST_KINDS = {'FocalLossCost': 0, 'ClassificationCostV2_sigmoid': 1, 'ClassificationCostV2_softmax': 2, 'ZeroCost': 3,
+                    'DisCostV2': 4}            # ptb_match_cost.kind (PTB_MATCH_COST_*)
+
+
+def p2p_cost_matrix_terms(cls_logits, pts, row_idx, gts, gt_labels, terms, fx=1.0, fy=1.0, out=None):
+    """ptb_p2p_cost_matrix_terms -> (n_rows, n_gt) fp32: sum(classification terms) + sum(DisCostV2 terms), each in list order.
+    terms: dicts with 'kind' (a MATCH_COST_KINDS key) and 'weight', plus 'alpha', 'gamma', 'eps' (FocalLossCost) or 'p',
+    'norm_with_img_wh' (DisCostV2), as assigners.match_cost_terms makes them.  cls_logits (Q, num_cols): the softmax term normalises
+    over all num_cols columns.  fx, fy: the image width and height DisCostV2 divides by when norm_with_img_wh is set."""
+    lib = _lib.load()
+    _chk(cls_logits, torch.float32, 'cls_logits'); _chk(gts, torch.float32, 'gts'); _chk(gt_labels, torch.int32, 'gt_labels')
+    if pts.stride(-1) != 1 or pts.dtype != torch.float32:
+        raise ValueError('pts must be fp32 with unit inner stride')
+    if row_idx is not None:
+        _chk(row_idx, torch.int32, 'row_idx')
+    n_rows = row_idx.shape[0] if row_idx is not None else cls_logits.shape[0]
+    n_gt = gts.shape[0]
+    if out is None:
+        cost = torch.empty((n_rows, n_gt), dtype=torch.float32, device=cls_logits.device)
+    else:
+        _chk(out, torch.float32, 'out')
+        if out.numel() != n_rows * n_gt:
+            raise ValueError('out must hold n_rows*n_gt elements')
+        cost = out.view(n_rows, n_gt)
+    arr = (_lib.MatchCost * max(len(terms), 1))(*[
+        _lib.MatchCost(MATCH_COST_KINDS[t['kind']], float(t['weight']), float(t.get('alpha', 0.0)), float(t.get('gamma', 0.0)),
+                       float(t.get('eps', 0.0)), int(t.get('p', 0)), int(bool(t.get('norm_with_img_wh', False)))) for t in terms])
+    ws = None
+    if any(t['kind'] == 'ClassificationCostV2_softmax' for t in terms):
+        ws = torch.empty(max(int(lib.ptb_p2p_cost_matrix_terms_workspace(n_rows)), 8), dtype=torch.uint8, device=cls_logits.device)
+    check(lib.ptb_p2p_cost_matrix_terms(_ptr(cls_logits), _ptr(pts), pts.stride(0), _ptr(row_idx), n_rows, cls_logits.shape[1],
+                                        _ptr(gts), _ptr(gt_labels), n_gt, arr, len(terms), float(fx), float(fy), _ptr(cost),
+                                        _ptr(ws), ws.numel() if ws is not None else 0, _stream()), 'ptb_p2p_cost_matrix_terms')
+    return cost
+
+
 def rpn_proposals(cls_scores, bbox_preds, base_anchors, strides_wh, img_hw, means, stds, wh_ratio_clip, nms_pre, min_bbox_size, iou_thr,
                   max_per_img, want_candidates=False):
     """ptb_rpn_proposals.  cls_scores[l] (B,A,H,W) / bbox_preds[l] (B,4A,H,W) contiguous NCHW fp32 CUDA tensors, base_anchors (L,A,4),

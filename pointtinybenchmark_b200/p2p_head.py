@@ -1,7 +1,8 @@
 """P2PHead — host-side mirror of the reference's P2PNet-style head over the sm_90a kernels.
 
 reference: TOV_mmdetection/mmdet/models/point/dense_heads/p2p_head.py:18-572 (P2PHead), HungarianAssignerV2
-(core/bbox/assigners/hungarian_assigner.py:149-270), FocalLossCost/DisCostV2 (core/bbox/match_costs/match_cost.py),
+(core/bbox/assigners/hungarian_assigner.py:149-270) with lists of FocalLossCost, ClassificationCostV2, ZeroCost and DisCostV2
+(core/bbox/match_costs/match_cost.py; parsed by assigners.match_cost_terms),
 multiclass_nms (core/post_processing/bbox_nms.py).  Same ctor kwargs / outputs / state_dict keys
 (cls_convs.*, reg_convs.*, cls_out (conv3x3), reg_out (conv3x3)).
 
@@ -19,6 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .assigners import cost_matrix, match_cost_terms
 from .post_processing import check_split_thr
 from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
 from .registry import CfgNode, register_head
@@ -111,16 +113,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             a = dict(self.train_cfg.assigner)
             if a.get('type') != 'HungarianAssignerV2':
                 raise NotImplementedError(f"assigner {a.get('type')}")
-            cc, rc = a.get('cls_costs'), a.get('reg_costs')
-            cc = cc[0] if isinstance(cc, (list, tuple)) else cc
-            rc = rc[0] if isinstance(rc, (list, tuple)) else rc
-            if cc.get('type') != 'FocalLossCost' or rc.get('type') != 'DisCostV2':
-                raise NotImplementedError('only FocalLossCost + DisCostV2 match costs are implemented')
-            self.assign = dict(w_cls=cc.get('weight', 1.0), alpha=cc.get('alpha', 0.25), gamma=cc.get('gamma', 2),
-                               eps=cc.get('eps', 1e-12), w_dis=rc.get('weight', 1.0),
-                               norm_wh=rc.get('norm_with_img_wh', True), p=rc.get('p', 1), topk_k=a.get('topk_k', 1))
-            if self.assign['p'] != 1:
-                raise NotImplementedError('DisCostV2 p != 1')
+            self.assign = dict(terms=match_cost_terms(a.get('cls_costs'), a.get('reg_costs')), topk_k=a.get('topk_k', 1))
         self._init_packed_hooks()
         self.check_assign_status = True      # read the (B,) status of the matching kernel each step (scipy's ValueErrors)
 
@@ -225,10 +218,9 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             gpts_l.append(gpts)
             if shapes[b][0] == 0 or shapes[b][1] == 0:
                 continue
-            fx, fy = (img_metas[b]['img_shape'][1], img_metas[b]['img_shape'][0]) if a['norm_wh'] else (1.0, 1.0)
-            ops.p2p_cost_matrix(cls[b].detach().contiguous(), prop[b], ridx_flat[ridx_off[b]:ridx_off[b + 1]], gpts,
-                                gt_labels[b].to(dev).int().contiguous(), a['w_cls'], a['alpha'], a['gamma'], a['eps'], a['w_dis'], fx, fy,
-                                out=cost_flat[cost_off[b]:cost_off[b + 1]])
+            cost_matrix(cls[b].detach().contiguous(), prop[b], ridx_flat[ridx_off[b]:ridx_off[b + 1]], gpts,
+                        gt_labels[b].to(dev).int().contiguous(), a['terms'], img_metas[b]['img_shape'],
+                        out=cost_flat[cost_off[b]:cost_off[b + 1]])
         gi_all = torch.zeros((B, Q), dtype=torch.int64, device=dev)
         status = ops.hungarian_v2_batch(cost_flat, shapes, a['topk_k'], gi_all, [b * Q for b in range(B)], ridx_flat, ridx_off[:-1])
         if self.check_assign_status:                          # one (B,) int32 read per batch: scipy's two ValueErrors
