@@ -517,6 +517,25 @@ int ptb_conv_tc_f16x2(const void* x_h, const void* x_l, const void* w_h, const v
                       void* stream);
 int ptb_gn_relu_apply_f16(const float* y, const double* gn_stats, const float* gamma, const float* beta, int B, int HW, int C,
                           int groups, float eps, int relu, void* out_h, void* out_l, int* overflow_flag, void* stream);
+/* Half-precision feature maps (the fp16 / bf16 FPN output of a backbone under autocast) are operand pairs without an fp32 copy:
+ *   fp16  the tensor is its own h with l == 0 and scale 1.  ptb_conv_tc_f16x1a is ptb_conv_tc_f16x2 without x_l: the l * w_h product
+ *         and the l activation loads are dropped (8 MMAs per K-block instead of 12, half the activation bytes); the result has the
+ *         bits of ptb_conv_tc_f16x2 given the same x_h and an all-zero x_l.  gn_stats (optional, zero-initialised, [B][32][2] fp64)
+ *         as in ptb_conv3x3_c256_f16x2: needs n_out == n_mma == 256.
+ *   bf16  ptb_split_f16_from_bf16: x (void* = __nv_bfloat16*, n % 8 == 0, 16-byte aligned) -> (h, l, *dev_inv_scale), bit for bit
+ *         what ptb_split_f16(auto_scale = 1) gives on the tensor converted to fp32, reading 2 bytes per element (workspace: 4 bytes).
+ *   ptb_conv_tc_f16x2_half_out: ptb_conv_tc_f16x2 storing y as fp16 / bf16 (y_dtype = PTB_DTYPE_*, ldy in elements), each value the
+ *         fp32 result rounded to nearest even (overflow to +-inf), i.e. the cast of the fp32 output without a second pass: the input
+ *         gradient (dgrad) of a half-precision feature map.  n_mma > 64 (128-channel slices). */
+#define PTB_DTYPE_F16 1
+#define PTB_DTYPE_BF16 2
+int ptb_split_f16_from_bf16(const void* x, int64_t n, void* hi, void* lo, float* dev_inv_scale, void* workspace, void* stream);
+int ptb_conv_tc_f16x1a(const void* x_h, const void* w_h, const void* w_l, int B, int H, int W, int Cin, int taps, int n_out, int n_mma,
+                       float out_scale, const float* dev_out_scale, const float* bias, float* y, int ldy, double* gn_stats /*or NULL*/,
+                       void* stream);
+int ptb_conv_tc_f16x2_half_out(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin, int taps,
+                               int n_out, int n_mma, float out_scale, const float* dev_out_scale, const float* bias, void* y, int y_dtype,
+                               int ldy, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-anchor assignment (SURVEY.md §8f rank 4, BASELINE.json configs[3]): MaxIoUAssigner.assign

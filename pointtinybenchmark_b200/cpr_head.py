@@ -486,6 +486,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
             return cls_o
         return cls_o, (cls_o if self.ins_out is self.cls_out else self.ins_out(x).reshape(*shape[:-1], -1))
 
+    @torch.autocast('cuda', enabled=False)          # fp32 Linear / softmax also inside a caller's autocast region
     def _loss_generic(self, fmap, gt, hp, gt_weights):
         """CPRHead.loss0 (cpr_head.py:1131-1229) + MILLoss.forward (multi_instance_learning_loss.py:153-203), R = 1."""
         B, H, W, C = fmap.shape
@@ -555,6 +556,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
             torch.backends.cuda.matmul.allow_tf32 = tf32
 
     @torch.no_grad()
+    @torch.autocast('cuda', enabled=False)
     def _refine_generic(self, fmap, gt, not_refine=None, want_chosen=False, want_bag_pts=False):
         """refine for the variants: bag features (CUDA gather) -> FC stack / cls_out / get_cls_prob (torch) -> ptb_cpr_refine (staged)."""
         pr = self.point_refiner
@@ -574,12 +576,14 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         return (o_pts, o_sc, o_nr, o_ch, pts[..., :2]) if want_bag_pts else (o_pts, o_sc, o_nr, o_ch)
 
     def forward(self, feats):
-        """cpr_head.py:1030-1043: returns feature maps (not logits)."""
+        """cpr_head.py:1030-1043: returns feature maps (not logits).  feats[i]: fp32, or the fp16 / bf16 map of a backbone under
+        torch.autocast, taken as it is (layers.input_plan; no .float() in front of the head).  The returned maps are fp32, as are
+        the logits, losses and detections computed from them, inside an autocast region too; `last_input_path` names the path."""
         cls_feats, ins_feats = [], []
         info = {}
         for x in feats:
             c = tower(self.cls_convs, x, info)
-            self.last_tower_backend = info.get('backend')
+            self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
             cls_feats.append(c)
             ins_feats.append(c)
         return cls_feats, ins_feats
@@ -596,14 +600,15 @@ class CPRHead(PackedWeightsMixin, nn.Module):
     def simple_test(self, feats, img_metas, rescale=False, **kwargs):
         """dense_test_mixins.py:15-36 (forward -> get_bboxes).  Inference fast path: the towers hand their output over
         as the fp16 operand pair and the class-logit map comes from the same wgmma kernel (1 tap, N = num_classes),
-        so neither the fp32 feature map nor an FFMA GEMM appears in the step; results are identical within 1e-4."""
+        so neither the fp32 feature map nor an FFMA GEMM appears in the step; results are identical within 1e-4.
+        An fp16 / bf16 feats[0] takes the same path (see forward); the detections are fp32."""
         x = feats[0]
         if len(feats) == 1 and self._default_variant() and tc_enabled(x, self.cls_convs, self.cls_out) and not torch.is_grad_enabled() \
                 and self.in_channels % 32 == 0 and self.feat_channels == 256:
             info = {}
             pair = tower(self.cls_convs, x, info, want='f16pair')
             if pair is not None:
-                self.last_tower_backend = info.get('backend')
+                self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
                 self.last_overflow_flag = info.get('overflow_flag')
                 if self.debug and self.last_overflow_flag is not None and int(self.last_overflow_flag) != 0:    # host sync: debug only
                     raise FloatingPointError('CPRHead: a GroupNorm output exceeded the fp16 operand range (|x| > 6e4) and was clamped')

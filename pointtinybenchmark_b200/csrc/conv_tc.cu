@@ -36,7 +36,13 @@
 //   * epilogue: straight from the accumulator registers (add, scale, bias) to global memory (8-byte stores, 32 contiguous bytes per
 //     row and quad); GroupNorm sum / sum of squares per (image, group of 8 channels) by a halving butterfly over the 32 lanes of a
 //     warp + one fp64 atomic per lane.
+//   * half-precision activations (an autocast backbone's fp16 / bf16 feature map) are operand pairs already.  An fp16 tensor is its
+//     own hi with lo == 0 and scale 1: A_LO_ZERO drops the lo * W_hi MMA (8 MMAs per K-block instead of 12) and the lo activation
+//     box (half the activation TMA bytes); the ring keeps its layout, the lo half of a slot stays unused.  A bf16 tensor goes
+//     through split_f16_from_bf16_kernel (2 B / element read) and the ordinary three-MMA kernel.  OutT = __half / __nv_bfloat16
+//     stores the epilogue's fp32 value rounded to nearest even: the input gradient of such a tensor, in its dtype.
 #include "tc_ptx.cuh"
+#include <cuda_bf16.h>
 #include <stdlib.h>
 #include <type_traits>
 
@@ -102,11 +108,15 @@ __device__ __forceinline__ TileAt tile_at(const ConvShape& cs, int tile) {
 // F16 = false: 3xTF32 (operands fp32 hi/lo).  F16 = true: 2-term fp16 split (x = h + l, 22 significant bits): h*h + l*h + h*l,
 // the same three MMAs per k-step but K = 16 per MMA, i.e. half the tensor-pipe time and half the operand bytes.  out_scale undoes
 // the power-of-two scaling of the fp16 operands (exact).  NT: output channels per item (16, 32, 64 or 128; 128 in TF32 mode).
-template <bool F16, int NT>
+// A_LO_ZERO: the activation's lo term is identically zero (an fp16 input): its box is not loaded and its MMA not issued; the result
+// has the bits of the full kernel fed an explicit all-zero lo.  OutT: element type of y (float, or __half / __nv_bfloat16 rounded
+// to nearest even from the same fp32 value; cs.ldy counts elements of OutT).
+template <bool F16, int NT, bool A_LO_ZERO = false, typename OutT = float>
 __global__ void __launch_bounds__(CV_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restrict__ y, double* __restrict__ stats /*[B][32][2] or NULL*/,
+conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, OutT* __restrict__ y, double* __restrict__ stats /*[B][32][2] or NULL*/,
                float out_scale, const float* __restrict__ dev_out_scale, const float* __restrict__ bias) {
   static_assert(F16 || NT == 128, "the TF32 mode runs 128-channel slices");
+  static_assert(F16 || (!A_LO_ZERO && std::is_same<OutT, float>::value), "half-precision inputs and outputs belong to the fp16 mode");
   constexpr int KBC = F16 ? CV_KB_F16 : CV_KB;      // channels per K-block
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // swizzle atoms need (at least) 512 B alignment
@@ -152,10 +162,10 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
           const int kw = cs.taps == 9 ? ks / kblocks_per_tap : 1, cblk = ks - (ks / kblocks_per_tap) * kblocks_per_tap;
           mbar_wait(empty_a(a_st), a_ph ^ 1u);
           const uint32_t sA_hi = sA_base + a_st * CV_A_STAGE_BYTES;
-          mbar_expect_tx(full_a(a_st), 2 * a_bytes);
+          mbar_expect_tx(full_a(a_st), (A_LO_ZERO ? 1 : 2) * a_bytes);
           const int aw = ta.w0 + kw - 1, ah = ta.h0 - (n_kh > 1 ? 1 : 0);
           tma_load_4d(&mp.x[ta.shape][0], full_a(a_st), sA_hi, cblk * KBC, aw, ah, ta.b);
-          tma_load_4d(&mp.x[ta.shape][1], full_a(a_st), sA_hi + CV_A_BYTES, cblk * KBC, aw, ah, ta.b);
+          if constexpr (!A_LO_ZERO) tma_load_4d(&mp.x[ta.shape][1], full_a(a_st), sA_hi + CV_A_BYTES, cblk * KBC, aw, ah, ta.b);
           if (++a_st == CV_A_STAGES) { a_st = 0; a_ph ^= 1u; }
           for (int kh = 0; kh < n_kh; ++kh) {                // the weight rows of taps (kh, kw), kh = 0 .. n_kh - 1
             const int tap = cs.taps == 9 ? 3 * kh + kw : 0;
@@ -207,8 +217,12 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
               const uint32_t first = (ks | kh | k) != 0;
               if constexpr (F16) {
                 wgmma_f16<0, 0>(acc, a_hi, b_hi, first);
-                wgmma_f16<0, 0>(cor, a_lo, b_hi, first);
-                wgmma_f16<0, 0>(cor, a_hi, b_lo, 1u);
+                if constexpr (A_LO_ZERO) {
+                  wgmma_f16<0, 0>(cor, a_hi, b_lo, first);
+                } else {
+                  wgmma_f16<0, 0>(cor, a_lo, b_hi, first);
+                  wgmma_f16<0, 0>(cor, a_hi, b_lo, 1u);
+                }
               } else {
                 wgmma_tf32(acc, a_hi, b_hi, first);
                 wgmma_tf32(cor, a_lo, b_hi, first);
@@ -237,7 +251,7 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
 
       // ---- epilogue: rows r0 and r0 + 8, columns n0 + 8 i + 2 (lane % 4) (+1) ----
       const int h_end = ta.shape == 2 ? cs.right_h : cs.H;   // the right strip stops where the bottom strip begins
-      float* row_ptr[2];
+      OutT* row_ptr[2];
       bool valid[2];
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
@@ -261,8 +275,16 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, float* __restr
             if (col + 1 < cs.n_out) v1 = v1 + __ldg(bias + col + 1);
           }
           if (valid[j]) {
-            if (col + 1 < cs.n_out) *reinterpret_cast<float2*>(row_ptr[j] + col) = make_float2(v0, v1);
-            else if (col < cs.n_out) row_ptr[j][col] = v0;
+            if constexpr (std::is_same<OutT, float>::value) {
+              if (col + 1 < cs.n_out) *reinterpret_cast<float2*>(row_ptr[j] + col) = make_float2(v0, v1);
+              else if (col < cs.n_out) row_ptr[j][col] = v0;
+            } else if constexpr (std::is_same<OutT, __half>::value) {
+              if (col + 1 < cs.n_out) *reinterpret_cast<__half2*>(row_ptr[j] + col) = __halves2half2(__float2half_rn(v0), __float2half_rn(v1));
+              else if (col < cs.n_out) row_ptr[j][col] = __float2half_rn(v0);
+            } else {
+              if (col + 1 < cs.n_out) *reinterpret_cast<__nv_bfloat162*>(row_ptr[j] + col) = __halves2bfloat162(__float2bfloat16_rn(v0), __float2bfloat16_rn(v1));
+              else if (col < cs.n_out) row_ptr[j][col] = __float2bfloat16_rn(v0);
+            }
             s += v0 + v1;
             ss = fmaf(v0, v0, ss);
             ss = fmaf(v1, v1, ss);
@@ -419,6 +441,52 @@ split_f16_kernel(const float4* __restrict__ x, long long n4, const unsigned int*
     split_h2(v.z * scale, h[2], l[2]); split_h2(v.w * scale, h[3], l[3]);
     hi[i] = *reinterpret_cast<uint2*>(h);
     lo[i] = *reinterpret_cast<uint2*>(l);
+  }
+}
+
+// ---- bf16 activations: the same (hi, lo, scale) as split_f16_kernel on the upcast tensor (bf16 -> fp32 is exact, so bit for bit),
+// read at 2 B / element.  8 values (one 16-byte load) per thread and step.
+__device__ __forceinline__ void bf16x8_to_f32(const uint4 v, float4& a, float4& b) {
+  a = make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xFFFF0000u), __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xFFFF0000u));
+  b = make_float4(__uint_as_float(v.z << 16), __uint_as_float(v.z & 0xFFFF0000u), __uint_as_float(v.w << 16), __uint_as_float(v.w & 0xFFFF0000u));
+}
+
+__global__ void __launch_bounds__(256) amax_abs_bf16_kernel(const uint4* __restrict__ x, long long n8, unsigned int* __restrict__ out_bits) {
+  float m = 0.f;
+  const long long step = (long long)gridDim.x * 256;
+  long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  float4 a, b;
+  for (; i + 3 * step < n8; i += 4 * step) {
+    const uint4 v0 = x[i], v1 = x[i + step], v2 = x[i + 2 * step], v3 = x[i + 3 * step];
+    bf16x8_to_f32(v0, a, b); m = amax4(amax4(m, a), b);
+    bf16x8_to_f32(v1, a, b); m = amax4(amax4(m, a), b);
+    bf16x8_to_f32(v2, a, b); m = amax4(amax4(m, a), b);
+    bf16x8_to_f32(v3, a, b); m = amax4(amax4(m, a), b);
+  }
+  for (; i < n8; i += step) { bf16x8_to_f32(x[i], a, b); m = amax4(amax4(m, a), b); }
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));
+}
+
+__global__ void __launch_bounds__(256)
+split_f16_from_bf16_kernel(const uint4* __restrict__ x, long long n8, const unsigned int* __restrict__ dev_amax_bits,
+                           uint4* __restrict__ hi, uint4* __restrict__ lo, float* __restrict__ inv_scale_out) {
+  const float scale = pow2_scale_for(__uint_as_float(*dev_amax_bits));
+  if (blockIdx.x == 0 && threadIdx.x == 0) *inv_scale_out = 1.f / scale;
+  const long long step = (long long)gridDim.x * 256;
+  long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  float4 a, b;
+  uint4 ph, pl;
+  for (; i + step < n8; i += 2 * step) {
+    const uint4 v0 = __ldcs(x + i), v1 = __ldcs(x + i + step);
+    bf16x8_to_f32(v0, a, b); split8(a, b, scale, ph, pl);
+    hi[i] = ph; lo[i] = pl;
+    bf16x8_to_f32(v1, a, b); split8(a, b, scale, ph, pl);
+    hi[i + step] = ph; lo[i + step] = pl;
+  }
+  for (; i < n8; i += step) {
+    bf16x8_to_f32(__ldcs(x + i), a, b); split8(a, b, scale, ph, pl);
+    hi[i] = ph; lo[i] = pl;
   }
 }
 
@@ -613,21 +681,22 @@ extern "C" int ptb_conv3x3_pack_weight(const float* w_oihw, int Cout, int Cin, f
   return check_launch("ptb_conv3x3_pack_weight");
 }
 
-template <bool F16, int NT>
-static int conv_launch_nt(const ConvMaps& mp, const ConvShape& cs, float* y, double* gn_stats, float out_scale, const float* dev_out_scale,
+template <bool F16, int NT, bool A_LO_ZERO = false, typename OutT = float>
+static int conv_launch_nt(const ConvMaps& mp, const ConvShape& cs, OutT* y, double* gn_stats, float out_scale, const float* dev_out_scale,
                           const float* bias, void* stream) {
   // a function attribute is per DEVICE and a process may drive several: set it on every call (a few hundred ns)
-  if (cudaFuncSetAttribute(conv_tc_kernel<F16, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess)
+  if (cudaFuncSetAttribute(conv_tc_kernel<F16, NT, A_LO_ZERO, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess)
     return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the conv kernel");
   int grid = sm_count();                                     // persistent: one CTA per SM
   if (grid > cs.n_tiles * cs.n_slices) grid = cs.n_tiles * cs.n_slices;
-  conv_tc_kernel<F16, NT><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias);
+  conv_tc_kernel<F16, NT, A_LO_ZERO, OutT><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias);
   return 0;
 }
 
-template <bool F16>
+// A_LO_ZERO: x_lo is not read (NULL).  OutT != float runs 128-channel slices only (n_mma > 64: the callers' input gradients).
+template <bool F16, bool A_LO_ZERO = false, typename OutT = float>
 static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, int H, int W, int Cin, int taps,
-                       int n_out, int n_mma, float* y, int ldy, const float* bias, double* gn_stats, float out_scale,
+                       int n_out, int n_mma, OutT* y, int ldy, const float* bias, double* gn_stats, float out_scale,
                        const float* dev_out_scale, void* stream, const char* what) {
   ConvShape cs;
   cs.B = B; cs.H = H; cs.W = W; cs.Cin = Cin;
@@ -657,15 +726,17 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
   int rc;
   for (int sh = 0; sh < 3; ++sh) {
     if ((rc = make_act_map(&mp.x[sh][0], x_hi, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
-    if ((rc = make_act_map(&mp.x[sh][1], x_lo, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
+    if (A_LO_ZERO) mp.x[sh][1] = mp.x[sh][0];            // never used by the kernel
+    else if ((rc = make_act_map(&mp.x[sh][1], x_lo, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
   }
   if ((rc = make_w_map(&mp.w[0], w_hi, n_mma, taps * Cin, F16, nt))) return rc;
   if ((rc = make_w_map(&mp.w[1], w_lo, n_mma, taps * Cin, F16, nt))) return rc;
-  if (!F16) rc = conv_launch_nt<false, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
-  else if (nt == 128) rc = conv_launch_nt<true, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
-  else if (nt == 64) rc = conv_launch_nt<true, 64>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
-  else if (nt == 32) rc = conv_launch_nt<true, 32>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
-  else rc = conv_launch_nt<true, 16>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  if constexpr (!F16) rc = conv_launch_nt<false, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if (nt == 128) rc = conv_launch_nt<true, 128, A_LO_ZERO, OutT>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if constexpr (!std::is_same<OutT, float>::value) return fail("%s: a half-precision output needs more than 64 output channels", what);
+  else if (nt == 64) rc = conv_launch_nt<true, 64, A_LO_ZERO>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else if (nt == 32) rc = conv_launch_nt<true, 32, A_LO_ZERO>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
+  else rc = conv_launch_nt<true, 16, A_LO_ZERO>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
   if (rc) return rc;
   return check_launch(what);
 }
@@ -762,6 +833,59 @@ extern "C" int ptb_conv_tc_f16x2(const void* x_h, const void* x_l, const void* w
                   ((uintptr_t)y % 16 == 0), "16-byte alignment");
   return conv_launch<true>(x_h, x_l, w_h, w_l, B, H, W, Cin, taps, n_out, n_mma, y, ldy, bias, nullptr, out_scale, dev_out_scale, stream,
                            "ptb_conv_tc_f16x2");
+}
+
+// the checks ptb_conv_tc_f16x2 makes on its shape arguments, shared by the half-precision entry points
+static int conv_tc_check_shape(int B, int H, int W, int Cin, int taps, int n_out, int n_mma, int ldy) {
+  PTB_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0 && (taps == 1 || taps == 9), "shape");
+  PTB_REQUIRE(Cin % CV_KB_F16 == 0, "Cin must be a multiple of 32");
+  PTB_REQUIRE(n_out > 0 && n_mma >= n_out && n_mma % 16 == 0 && n_mma <= CV_N_MAX, "n_mma must be a multiple of 16 in [n_out, 512]");
+  PTB_REQUIRE(ldy >= n_out && ldy % 4 == 0, "ldy must be a multiple of 4 and >= n_out");
+  return 0;
+}
+
+extern "C" int ptb_conv_tc_f16x1a(const void* x_h, const void* w_h, const void* w_l, int B, int H, int W, int Cin, int taps, int n_out,
+                                  int n_mma, float out_scale, const float* dev_out_scale, const float* bias, float* y, int ldy,
+                                  double* gn_stats, void* stream) {
+  if (int rc = conv_tc_check_shape(B, H, W, Cin, taps, n_out, n_mma, ldy)) return rc;
+  PTB_REQUIRE(x_h && w_h && w_l && y, "NULL input");
+  PTB_REQUIRE(((uintptr_t)x_h % 16 == 0) && ((uintptr_t)w_h % 16 == 0) && ((uintptr_t)w_l % 16 == 0) && ((uintptr_t)y % 16 == 0),
+              "16-byte alignment");
+  return conv_launch<true, true>(x_h, nullptr, w_h, w_l, B, H, W, Cin, taps, n_out, n_mma, y, ldy, bias, gn_stats, out_scale, dev_out_scale,
+                                 stream, "ptb_conv_tc_f16x1a");
+}
+
+extern "C" int ptb_conv_tc_f16x2_half_out(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin,
+                                          int taps, int n_out, int n_mma, float out_scale, const float* dev_out_scale, const float* bias,
+                                          void* y, int y_dtype, int ldy, void* stream) {
+  if (int rc = conv_tc_check_shape(B, H, W, Cin, taps, n_out, n_mma, ldy)) return rc;
+  PTB_REQUIRE(y_dtype == PTB_DTYPE_F16 || y_dtype == PTB_DTYPE_BF16, "y_dtype must be PTB_DTYPE_F16 or PTB_DTYPE_BF16");
+  PTB_REQUIRE(x_h && x_l && w_h && w_l && y, "NULL input");
+  PTB_REQUIRE(((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) && ((uintptr_t)w_h % 16 == 0) && ((uintptr_t)w_l % 16 == 0) &&
+                  ((uintptr_t)y % 16 == 0), "16-byte alignment");
+  if (y_dtype == PTB_DTYPE_F16)
+    return conv_launch<true, false, __half>(x_h, x_l, w_h, w_l, B, H, W, Cin, taps, n_out, n_mma, reinterpret_cast<__half*>(y), ldy, bias,
+                                            nullptr, out_scale, dev_out_scale, stream, "ptb_conv_tc_f16x2_half_out");
+  return conv_launch<true, false, __nv_bfloat16>(x_h, x_l, w_h, w_l, B, H, W, Cin, taps, n_out, n_mma, reinterpret_cast<__nv_bfloat16*>(y),
+                                                 ldy, bias, nullptr, out_scale, dev_out_scale, stream, "ptb_conv_tc_f16x2_half_out");
+}
+
+extern "C" int ptb_split_f16_from_bf16(const void* x, int64_t n, void* hi, void* lo, float* dev_inv_scale, void* workspace, void* stream) {
+  PTB_REQUIRE(n >= 0 && n % 8 == 0, "n must be a multiple of 8");
+  PTB_REQUIRE(((uintptr_t)x % 16 == 0) && ((uintptr_t)hi % 16 == 0) && ((uintptr_t)lo % 16 == 0), "16-byte alignment");
+  PTB_REQUIRE(workspace && dev_inv_scale, "a 4-byte workspace and dev_inv_scale are required");
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  long long blocks = (n / 8 + 255) / 256;
+  const long long cap = (long long)sm_count() * 16;
+  if (blocks > cap) blocks = cap;
+  unsigned int* amax = reinterpret_cast<unsigned int*>(workspace);
+  if (cudaMemsetAsync(amax, 0, 4, st) != cudaSuccess) return fail("%s", "ptb_split_f16_from_bf16: cudaMemsetAsync failed");
+  amax_abs_bf16_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(x), n / 8, amax);
+  if (int rc = check_launch("ptb_split_f16_from_bf16/amax")) return rc;
+  split_f16_from_bf16_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const uint4*>(x), n / 8, amax, reinterpret_cast<uint4*>(hi),
+                                                              reinterpret_cast<uint4*>(lo), dev_inv_scale);
+  return check_launch("ptb_split_f16_from_bf16");
 }
 
 extern "C" int ptb_gn_relu_apply_f16(const float* y, const double* gn_stats, const float* gamma, const float* beta, int B, int HW,

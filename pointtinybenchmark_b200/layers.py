@@ -5,6 +5,10 @@ Conv towers (SURVEY.md §8f rank 1): at inference they run on the hand-written w
 256 -> 256 geometry runs `_TowerTCFn`: the same forward kernel plus hand-written GroupNorm/ReLU backward, dgrad (the forward
 kernel on transposed, flipped weights) and a wgmma wgrad with MN-major operands.  Other geometries (or PTB_TOWER_TRAIN=cudnn)
 use cuDNN fp32 through torch with TF32 switched off locally (library path).
+
+Input dtype: fp32, or the fp16 / bf16 feature map of a backbone under torch.autocast, taken as it is (`input_plan`): an fp16 tensor is
+the first conv's hi operand itself, a bf16 tensor is split from its 2-byte storage, and the input gradient comes back in that dtype.
+Everything after the first conv, parameters and outputs stay fp32.
 """
 import math
 
@@ -80,12 +84,44 @@ class PackedWeightsMixin:
         invalidate_packed(self)
 
 
+HALF_INPUT_DTYPES = (torch.float16, torch.bfloat16)
+_INPUT_DTYPES = (torch.float32,) + HALF_INPUT_DTYPES
+
+
+def input_plan(dtype, conv_mode='f16x2'):
+    """How a tower takes an input of `dtype` with PTB_CONV_MODE = conv_mode: (input_path, first conv, dtype of the input gradient), a
+    pure function decided on the host (no device flag is read).  None for a dtype the tensor-core towers do not take.
+      fp32  'fp32-split'   the (hi, lo) pair from ptb_split_f16 (or the TF32 pair)    conv 'f16x2' | 'tf32x3'
+      fp16  'fp16-direct'  hi is the tensor's own storage, lo == 0, scale 1           conv 'f16x1a' (no lo MMA, no lo loads)
+      bf16  'bf16-split'   the pair from ptb_split_f16_from_bf16 (2 B / element)      conv 'f16x2'
+    Only the first conv of a tower differs: later layers consume fp32 GroupNorm outputs."""
+    if dtype == torch.float32:
+        return 'fp32-split', 'f16x2' if conv_mode == 'f16x2' else 'tf32x3', torch.float32
+    if dtype in HALF_INPUT_DTYPES:
+        if conv_mode != 'f16x2':
+            raise NotImplementedError(f'PTB_CONV_MODE={conv_mode}: {dtype} feature maps are taken by the fp16-split mode only '
+                                      '(PTB_CONV_MODE=f16x2, the default); convert the input to fp32 for this mode')
+        return ('fp16-direct', 'f16x1a', dtype) if dtype == torch.float16 else ('bf16-split', 'f16x2', dtype)
+    return None
+
+
+def _first_operands(xm):
+    """fp16 operand pair of a channels-last tower input: (hi, lo, device 1/scale); lo and the scale are None for an fp16 input
+    (hi is xm itself, lo == 0, scale 1)."""
+    from . import ops
+    if xm.dtype == torch.float16:
+        return xm, None, None
+    if xm.dtype == torch.bfloat16:
+        return ops.split_f16_from_bf16(xm)
+    return ops.split_f16(xm, auto_scale=True)
+
+
 def _tc_supported(convs, x):
     """the wgmma path covers the shipped head geometry: conv3x3 s1 p1 without bias -> 256 channels, GroupNorm with
-    channels-per-group % 4 == 0, Cin % 32 == 0, fp32 CUDA input, inference (no autograd graph)."""
+    channels-per-group % 4 == 0, Cin % 32 == 0, fp32 / fp16 / bf16 CUDA input, inference (no autograd graph)."""
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in convs for p in m.parameters())):
         return False
-    if not x.is_cuda or x.dtype != torch.float32 or len(convs) == 0:
+    if not x.is_cuda or x.dtype not in _INPUT_DTYPES or len(convs) == 0:
         return False
     for m in convs:
         c = m.conv
@@ -143,9 +179,9 @@ def _packed_tc(module, taps, tag):
 
 
 def tc_enabled(x, *modules):
-    """inference-only tensor-core path: CUDA fp32, no autograd graph, fp16-split mode selected."""
+    """inference-only tensor-core path: CUDA fp32 / fp16 / bf16, no autograd graph, fp16-split mode selected."""
     import os
-    if os.environ.get('PTB_CONV_MODE', 'f16x2') != 'f16x2' or not x.is_cuda or x.dtype != torch.float32:
+    if os.environ.get('PTB_CONV_MODE', 'f16x2') != 'f16x2' or not x.is_cuda or x.dtype not in _INPUT_DTYPES:
         return False
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in modules for p in m.parameters())):
         return False
@@ -154,11 +190,11 @@ def tc_enabled(x, *modules):
 
 def _tc_train_supported(convs, x):
     """the tensor-core TRAINING tower (forward + dgrad + wgrad + GroupNorm backward kernels) covers the shipped head geometry:
-    256 -> 256 conv3x3 s1 p1 without bias, GroupNorm with 8 | channels-per-group, ReLU, fp32 CUDA input."""
+    256 -> 256 conv3x3 s1 p1 without bias, GroupNorm with 8 | channels-per-group, ReLU, fp32 / fp16 / bf16 CUDA input."""
     import os
     if os.environ.get('PTB_CONV_MODE', 'f16x2') != 'f16x2' or os.environ.get('PTB_TOWER_TRAIN', 'tc') != 'tc':
         return False
-    if not x.is_cuda or x.dtype != torch.float32 or len(convs) == 0:
+    if not x.is_cuda or x.dtype not in _INPUT_DTYPES or len(convs) == 0:
         return False
     for m in convs:
         c = m.conv
@@ -174,14 +210,17 @@ class _TowerTCFn(torch.autograd.Function):
     forward  ptb_conv3x3_c256_f16x2 (+ GroupNorm statistics) / ptb_gn_relu_apply[_f16]      (csrc/conv_tc.cu)
     backward ptb_gn_relu_bwd -> ptb_split_f16_amax -> ptb_conv3x3_wgrad_f16x2 (dW) and ptb_conv_tc_f16x2 with the transposed,
              flipped weights (dX)                                                          (csrc/tower_bwd.cu, wgrad_tc.cu)
-    Saved per layer: the fp16 operand pair of its input (re-used as the wgrad operand), the conv output y and the statistics."""
+    Saved per layer: the fp16 operand pair of its input (re-used as the wgrad operand), the conv output y and the statistics.
+    A half-precision input is saved itself instead of a pair (backward derives the pair again as forward did), and its gradient is
+    written in its dtype by the first layer's dgrad epilogue."""
 
     @staticmethod
     def forward(ctx, xm, convs, *params):
         from . import ops
         n_layers = len(convs)
         groups, eps = [m.gn.num_groups for m in convs], [float(m.gn.eps) for m in convs]
-        h, l, dev_inv = ops.split_f16(xm, auto_scale=True)
+        h, l, dev_inv = _first_operands(xm)
+        half_in = xm.dtype != torch.float32
         flag = torch.zeros(1, dtype=torch.int32, device=xm.device)
         saved, out = [], None
         for i in range(n_layers):
@@ -189,13 +228,13 @@ class _TowerTCFn(torch.autograd.Function):
             wh, wl, inv_w = _packed_weight_f16(convs[i])          # cached per parameter version (no host sync per step)
             inv_x = dev_inv if i == 0 else None
             y, stats = ops.conv3x3_c256_f16(h, l, wh, wl, inv_w, inv_x)
-            saved += [h, l, y, stats]
+            saved += [xm, None, y, stats] if i == 0 and half_in else [h, l, y, stats]
             if i == n_layers - 1:
                 out = ops.gn_relu_apply(y, stats, gamma.detach(), beta.detach(), groups[i], eps[i], True, split=False)
             else:
                 h, l = ops.gn_relu_apply_f16(y, stats, gamma.detach(), beta.detach(), groups[i], eps[i], True, flag)
         ctx.n_layers, ctx.groups, ctx.eps, ctx.convs = n_layers, groups, eps, convs
-        ctx.dev_inv = dev_inv
+        ctx.dev_inv, ctx.in_dtype = dev_inv, xm.dtype
         ctx.save_for_backward(*saved, *[p.detach() for p in params])
         return out
 
@@ -209,15 +248,21 @@ class _TowerTCFn(torch.autograd.Function):
         grads = [None] * (3 * n)
         for i in reversed(range(n)):
             h, l, y, stats = acts[4 * i:4 * i + 4]
+            inv_x = ctx.dev_inv if i == 0 else None
+            if i == 0 and ctx.in_dtype != torch.float32:
+                h, l, inv_x = _first_operands(h)
+                if l is None:                                     # the wgrad kernel reads a materialised lo
+                    l = torch.zeros_like(h)
             w, gamma, beta = params[3 * i], params[3 * i + 1], params[3 * i + 2]
             dy, dg, db, amax = ops.gn_relu_bwd(da, y, stats, gamma, beta, ctx.groups[i], ctx.eps[i], True)
             dyh, dyl, inv_dy = ops.split_f16_amax(dy, amax)
             grads[3 * i + 1], grads[3 * i + 2] = dg, db
             if ctx.needs_input_grad[2 + 3 * i]:
-                grads[3 * i] = ops.conv3x3_wgrad_f16(dyh, dyl, h, l, 1.0, inv_dy, ctx.dev_inv if i == 0 else None)
+                grads[3 * i] = ops.conv3x3_wgrad_f16(dyh, dyl, h, l, 1.0, inv_dy, inv_x)
             if i > 0 or ctx.needs_input_grad[0]:
                 # dgrad = the forward kernel with W^T and reversed taps
-                da = ops.conv_tc_f16(dyh, dyl, _packed_weight_f16_t(ctx.convs[i]), 9, w.shape[1], dev_out_scale=inv_dy)
+                da = ops.conv_tc_f16(dyh, dyl, _packed_weight_f16_t(ctx.convs[i]), 9, w.shape[1], dev_out_scale=inv_dy,
+                                     out_dtype=ctx.in_dtype if i == 0 else torch.float32)
             else:
                 da = None
         return (da, None, *grads)
@@ -226,9 +271,14 @@ class _TowerTCFn(torch.autograd.Function):
 def tower(convs, x, info=None, want='fp32'):
     """4 x [conv3x3 + GN + ReLU].  Inference: hand-written wgmma implicit GEMM (fp16 two-term split or 3xTF32) with GroupNorm
     statistics in the epilogue (csrc/conv_tc.cu).  Training (autograd): _TowerTCFn for the shipped 256 -> 256 geometry (same forward
-    kernel + hand-written backward), else cuDNN fp32 through torch."""
+    kernel + hand-written backward), else cuDNN fp32 through torch.
+    x: fp32, or an fp16 / bf16 CUDA feature map on the tensor-core paths (`input_plan`; the output is fp32 either way).
+    info (optional dict) receives 'backend' and, on the tensor-core paths, 'input_path'."""
     import os
     mode = os.environ.get('PTB_CONV_MODE', 'f16x2')
+    if x.dtype in HALF_INPUT_DTYPES and not x.is_cuda:
+        raise RuntimeError(f'tower: expected a CUDA tensor for a {x.dtype} input (pointtinybenchmark_b200 has no CPU path)')
+    plan = input_plan(x.dtype, mode)
     if want == 'f16pair' and not (_tc_supported(convs, x) and mode == 'f16x2' and all(m.conv.in_channels % 32 == 0 for m in convs)):
         return None
     if _tc_supported(convs, x) and mode == 'f16x2' and all(m.conv.in_channels % 32 == 0 for m in convs):
@@ -236,7 +286,7 @@ def tower(convs, x, info=None, want='fp32'):
         # is scaled by a power of two chosen on the device from max|x| (no host sync); later layers consume GroupNorm outputs.
         from . import ops
         xm = ops.to_nhwc(x).contiguous()
-        h, l, dev_inv = ops.split_f16(xm, auto_scale=True)
+        h, l, dev_inv = _first_operands(xm)
         flag = torch.zeros(1, dtype=torch.int32, device=x.device)
         out = None
         for i, m in enumerate(convs):
@@ -248,6 +298,7 @@ def tower(convs, x, info=None, want='fp32'):
                 h, l = ops.gn_relu_apply_f16(y, stats, m.gn.weight.detach(), m.gn.bias.detach(), m.gn.num_groups, m.gn.eps, True, flag)
         if info is not None:
             info['backend'] = 'wgmma-f16x2'
+            info['input_path'] = plan[0]
             info['overflow_flag'] = flag
         if want == 'f16pair':
             return h, l              # (B,H,W,C) fp16 operand pair of the tower output: feeds ptb_conv_tc_f16x2 directly
@@ -269,6 +320,7 @@ def tower(convs, x, info=None, want='fp32'):
                 hi, lo = res
         if info is not None:
             info['backend'] = 'wgmma-3xtf32'
+            info['input_path'] = plan[0]
         return out.permute(0, 3, 1, 2)          # (B,C,H,W) view with channels_last strides
     if want == 'fp32' and torch.is_grad_enabled() and _tc_train_supported(convs, x):
         from . import ops
@@ -278,7 +330,11 @@ def tower(convs, x, info=None, want='fp32'):
         out = _TowerTCFn.apply(ops.to_nhwc(x).contiguous(), convs, *params)
         if info is not None:
             info['backend'] = 'wgmma-f16x2-train'
+            info['input_path'] = plan[0]
         return out.permute(0, 3, 1, 2)
+    if x.dtype in HALF_INPUT_DTYPES:
+        raise NotImplementedError(f'tower: a {x.dtype} input needs the tensor-core geometry (conv3x3 s1 p1 without bias -> 256 channels, '
+                                  'GroupNorm(32), ReLU, Cin % 32 == 0; 256 -> 256 under autograd); convert it to fp32 for the cuDNN path')
     if info is not None:
         info['backend'] = 'cudnn'
     x = x.contiguous(memory_format=torch.channels_last)

@@ -869,6 +869,18 @@ def split_f16(x, auto_scale=False):
     return h, l, inv
 
 
+def split_f16_from_bf16(x):
+    """ptb_split_f16_from_bf16: x bf16 -> (h, l, dev_inv_scale), bit for bit split_f16(x.float(), auto_scale=True) without the fp32 copy."""
+    lib = _lib.load()
+    _chk(x, torch.bfloat16, 'x')
+    h = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+    l = torch.empty_like(h)
+    inv = torch.empty(1, dtype=torch.float32, device=x.device)
+    ws = torch.empty(1, dtype=torch.int32, device=x.device)
+    check(lib.ptb_split_f16_from_bf16(_ptr(x), x.numel(), _ptr(h), _ptr(l), _ptr(inv), _ptr(ws), _stream()), 'ptb_split_f16_from_bf16')
+    return h, l, inv
+
+
 def conv3x3_pack_weight_f16(w):
     """(Cout,Cin,3,3) -> packed fp16 (h, l) of w*scale and 1/scale; scale = power of two with max|w|*scale in [2^9, 2^10)."""
     lib = _lib.load()
@@ -885,13 +897,19 @@ def conv3x3_pack_weight_f16(w):
 
 
 def conv3x3_c256_f16(x_h, x_l, w_h, w_l, out_scale, dev_out_scale=None, want_stats=True):
+    """tower conv3x3 -> 256 channels with GroupNorm statistics.  x_l None: x_h is an fp16 tensor used as is (lo == 0, ptb_conv_tc_f16x1a)."""
     lib = _lib.load()
-    _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l'); _chk(w_h, torch.float16, 'w_h'); _chk(w_l, torch.float16, 'w_l')
+    _chk(x_h, torch.float16, 'x_h'); _chk(w_h, torch.float16, 'w_h'); _chk(w_l, torch.float16, 'w_l')
     B, H, W, Cin = x_h.shape
     if w_h.shape != (256, 9 * Cin):
         raise ValueError('packed weight must be (256, 9*Cin)')
     y = torch.empty((B, H, W, 256), dtype=torch.float32, device=x_h.device)
     stats = torch.zeros((B, 32, 2), dtype=torch.float64, device=x_h.device) if want_stats else None
+    if x_l is None:
+        check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, 9, 256, 256, float(out_scale), _ptr(dev_out_scale), None,
+                                     _ptr(y), 256, _ptr(stats), _stream()), 'ptb_conv_tc_f16x1a')
+        return y, stats
+    _chk(x_l, torch.float16, 'x_l')
     check(lib.ptb_conv3x3_c256_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, float(out_scale), _ptr(dev_out_scale),
                                      _ptr(y), _ptr(stats), _stream()), 'ptb_conv3x3_c256_f16x2')
     return y, stats
@@ -994,14 +1012,33 @@ def conv_tc_pack_weight_f16(w, taps):
     return h, l, 1.0 / scale, n_mma
 
 
-def conv_tc_f16(x_h, x_l, packed, taps, n_out, bias=None, dev_out_scale=None, ldy=None):
-    """general wgmma conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias)."""
+HALF_DTYPES = {torch.float16: 1, torch.bfloat16: 2}      # PTB_DTYPE_F16, PTB_DTYPE_BF16
+
+
+def conv_tc_f16(x_h, x_l, packed, taps, n_out, bias=None, dev_out_scale=None, ldy=None, out_dtype=torch.float32):
+    """general wgmma conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias).  x_l None: x_h is an fp16 tensor used as is
+    (lo == 0: ptb_conv_tc_f16x1a).  out_dtype fp16 / bf16: the fp32 result rounded to nearest even in the epilogue
+    (ptb_conv_tc_f16x2_half_out), the input gradient of a half-precision feature map."""
     lib = _lib.load()
-    _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
+    _chk(x_h, torch.float16, 'x_h')
     w_h, w_l, inv_w, n_mma = packed
     B, H, W, Cin = x_h.shape
     ldy = ldy or (n_out + 3) // 4 * 4
-    y = torch.empty((B, H, W, ldy), dtype=torch.float32, device=x_h.device)
-    check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w),
-                                _ptr(dev_out_scale), _ptr(bias), _ptr(y), ldy, _stream()), 'ptb_conv_tc_f16x2')
+    y = torch.empty((B, H, W, ldy), dtype=out_dtype, device=x_h.device)
+    if x_l is None:
+        if out_dtype != torch.float32:
+            raise NotImplementedError('conv_tc_f16: a half-precision output of the lo == 0 variant')
+        check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w), _ptr(dev_out_scale),
+                                     _ptr(bias), _ptr(y), ldy, None, _stream()), 'ptb_conv_tc_f16x1a')
+        return y
+    _chk(x_l, torch.float16, 'x_l')
+    if out_dtype == torch.float32:
+        check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w),
+                                    _ptr(dev_out_scale), _ptr(bias), _ptr(y), ldy, _stream()), 'ptb_conv_tc_f16x2')
+    else:
+        if out_dtype not in HALF_DTYPES:
+            raise TypeError(f'conv_tc_f16: out_dtype must be float32, float16 or bfloat16, got {out_dtype}')
+        check(lib.ptb_conv_tc_f16x2_half_out(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w),
+                                             _ptr(dev_out_scale), _ptr(bias), _ptr(y), HALF_DTYPES[out_dtype], ldy, _stream()),
+              'ptb_conv_tc_f16x2_half_out')
     return y

@@ -122,7 +122,9 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         """p2p_head.py:104-123.  Inference: towers AND the two conv3x3 output layers run on the wgmma kernel (fp16 two-term
         split, fp32-level accuracy; cls_out has num_points * num_classes <= 512 channels, e.g. 320 at the reference's default 4
         anchors x 80 classes, in one launch); with autograd recording the towers use the tensor-core autograd function of
-        layers.py and the two output convs cuDNN fp32."""
+        layers.py and the two output convs cuDNN fp32 (also inside a caller's autocast region).
+        feats[i]: fp32, or the fp16 / bf16 map of a backbone under torch.autocast, taken as it is (layers.input_plan; no .float() in
+        front of the head).  The outputs are fp32; `last_input_path` names the path the towers took."""
         cls_outs, pts_outs = [], []
         for x in feats:
             if tc_enabled(x, self.cls_convs, self.reg_convs, self.cls_out, self.reg_out) and self.feat_channels == 256 \
@@ -131,7 +133,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
                 pc = tower(self.cls_convs, x, info, want='f16pair')
                 pr = tower(self.reg_convs, x, info, want='f16pair') if pc is not None else None
                 if pc is not None and pr is not None:
-                    self.last_tower_backend = info.get('backend')
+                    self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
                     nc, nr = self.cls_out.out_channels, self.reg_out.out_channels
                     yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9, 'conv'), 9, nc, bias=self.cls_out.bias.detach())
                     yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9, 'conv'), 9, nr, bias=self.reg_out.bias.detach())
@@ -142,9 +144,10 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             # shipped geometry; the two narrow output convs (256 -> C / 2k) stay cuDNN fp32, never TF32 (1e-4 logits)
             info = {}
             fc, fr = tower(self.cls_convs, x, info), tower(self.reg_convs, x, info)
-            self.last_tower_backend = info.get('backend')
+            self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
             with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
-                                            deterministic=torch.backends.cudnn.deterministic, allow_tf32=False):
+                                            deterministic=torch.backends.cudnn.deterministic, allow_tf32=False), \
+                    torch.autocast('cuda', enabled=False):
                 cls_outs.append(self.cls_out(fc))
                 pts_outs.append(self.reg_out(fr))
         return cls_outs, pts_outs
@@ -164,6 +167,7 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         yy = (torch.arange(0., H, device=device) * s).view(-1, 1).repeat(1, W).view(-1)
         return xx, yy
 
+    @torch.autocast('cuda', enabled=False)
     def get_pred_points(self, cls_out, pts_out, img_metas):
         """p2p_head.py:125-170 (single level): differentiable torch elementwise ops on channels-last views."""
         B, _, H, W = cls_out.shape
