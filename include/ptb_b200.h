@@ -536,6 +536,18 @@ int ptb_conv_tc_f16x1a(const void* x_h, const void* w_h, const void* w_l, int B,
 int ptb_conv_tc_f16x2_half_out(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin, int taps,
                                int n_out, int n_mma, float out_scale, const float* dev_out_scale, const float* bias, void* y, int y_dtype,
                                int ldy, void* stream);
+/* One tower layer in one launch: ptb_conv3x3_c256_f16x2 (x_l == NULL: the lo == 0 variant of ptb_conv_tc_f16x1a) followed by
+ * GroupNorm(32 groups) + ReLU, the apply running inside the conv kernel as each image's statistics complete.
+ *   workspace  zero-filled by the caller, 8-byte aligned: B * 32 * 2 doubles (the statistics [B][32][2], as gn_stats of
+ *              ptb_conv3x3_c256_f16x2) followed by B int32 completion counters.
+ *   out_l != NULL: out / out_l = the fp16 (h, l) pair ptb_gn_relu_apply_f16 writes (|value| > 60000 clamped, *overflow_flag raised
+ *              when given);  out_l == NULL: out = fp32 relu(GroupNorm(y)) as ptb_gn_relu_apply writes it (out_lo == NULL).
+ * y (fp32 [B][H][W][256]) and the statistics are written as by ptb_conv3x3_c256_f16x2.  Outputs have the bits of the two kernels
+ * run one after the other on this y and these statistics.  The launch is cooperative (the CTAs wait on each other's images); when
+ * the grid cannot be co-resident it runs as those two kernels. */
+int ptb_conv3x3_c256_f16_gn(const void* x_h, const void* x_l /*or NULL*/, const void* w_h, const void* w_l, int B, int H, int W, int Cin,
+                            float out_scale, const float* dev_out_scale, float* y, void* workspace, const float* gamma, const float* beta,
+                            float eps, void* out, void* out_l /*or NULL*/, int* overflow_flag /*or NULL*/, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-anchor assignment (SURVEY.md §8f rank 4, BASELINE.json configs[3]): MaxIoUAssigner.assign

@@ -105,6 +105,7 @@ SIGNATURES = {
     'ptb_split_f16_from_bf16': (c_int, [P, c_i64, P, P, P, P, P]),
     'ptb_conv_tc_f16x1a': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, c_int, P, P]),
     'ptb_conv_tc_f16x2_half_out': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, c_int, c_int, P]),
+    'ptb_conv3x3_c256_f16_gn': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, P, P, P, P, P, c_float, P, P, P, P]),
     'ptb_max_iou_assign_workspace': (c_u64, [c_int, c_int]),
     'ptb_max_iou_assign': (c_int, [P, c_int, P, c_int, P, P, c_int, c_float, c_float, c_float, c_float, c_int, c_int, c_float, c_int,
                                    P, P, P, P, c_u64, P]),

@@ -1,8 +1,9 @@
 // Dense convolutions of the head on the Hopper tensor cores (wgmma + TMA + mbarrier), fp32-accurate by operand splitting:
 // conv3x3 (stride 1, pad 1) and conv1x1 / per-cell Linear, Cin % 32 == 0 (fp16 mode) or Cin % 16 == 0 (TF32 mode), up to 512
 // output channels (fp16 mode; 256 in TF32 mode and whenever GroupNorm statistics are requested), optional bias, optional
-// GroupNorm statistics in the epilogue; GroupNorm-apply + ReLU + operand split is a
-// second, HBM-bound kernel.  Replaces the cuDNN / cuBLAS calls behind CPRHead.forward_single / P2PHead.forward_single
+// GroupNorm statistics in the epilogue; GroupNorm-apply + ReLU + operand split runs either inside the conv kernel, in warps that
+// are idle otherwise, as each image's statistics complete (GnFuse, ptb_conv3x3_c256_f16_gn: what the towers run), or as a second,
+// HBM-bound kernel.  Replaces the cuDNN / cuBLAS calls behind CPRHead.forward_single / P2PHead.forward_single
 // (cpr_head.py:1033-1043, p2p_head.py:113-123: 4 x ConvModule(conv3x3 + GN(32) + ReLU), 79.3 GFLOP per image), the
 // per-sample cls_out / ins_out Linear of CPRHead.get_pts_outs (cpr_head.py:1045-1078, applied once per map cell here) and
 // P2PHead's cls_out / reg_out conv3x3 (k * num_classes channels: 320 at the reference's default 4 anchors x 80 classes).
@@ -27,7 +28,8 @@
 //   * The tensor core adds into its fp32 accumulator without round-to-nearest, i.e. every accumulate step costs up to ~0.5 ulp of
 //     the accumulator.  The two small correction products therefore go to their OWN accumulator (their error is 2^-11 smaller in
 //     absolute terms); the epilogue adds the two in fp32 (round-to-nearest).
-//   * warp roles (384 threads, 1 CTA / SM, persistent over (tile, channel slice) items): warpgroup 0 = TMA producer (one thread),
+//   * warp roles (384 threads, 1 CTA / SM, persistent over (tile, channel slice) items): warpgroup 0 = TMA producer (one thread;
+//     with GnFuse its warps 1-3 apply GroupNorm + ReLU to the CTA's finished items),
 //     warpgroups 1 and 2 = MMA + epilogue for pixel rows 0-63 / 64-127 of the tile, each holding two 64 x NT fp32 accumulators in
 //     registers (128 per thread at NT = 128).  Two mbarrier full / empty rings in shared memory: 4 x 24 KB activation boxes,
 //     released after their last K-block, and 8 x 16 KB weight boxes, released after every K-block, so the weight loads of the
@@ -64,7 +66,7 @@ constexpr uint32_t CV_B_STAGE_BYTES = 2 * CV_B_BYTES;       // 16 KB
 constexpr uint32_t CV_RING_BYTES = CV_A_STAGES * CV_A_STAGE_BYTES + CV_B_STAGES * CV_B_STAGE_BYTES;   // 224 KB
 constexpr uint32_t CV_SMEM_BYTES = CV_RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 static_assert(CV_SMEM_BYTES <= 227 * 1024, "the conv rings must fit the 227 KB of opt-in shared memory");
-static_assert(2 * 8 * (CV_A_STAGES + CV_B_STAGES) <= 256, "the conv barriers must fit their 256 B");
+static_assert(2 * 8 * (CV_A_STAGES + CV_B_STAGES) + 8 <= 256, "the conv barriers and the item counter must fit their 256 B");
 constexpr int CV_THREADS = 384;
 
 // Output tiling.  A tile is always 128 pixels; the main region uses 8 x 16 tiles and the two edge strips that 8 x 16 tiles would
@@ -105,18 +107,148 @@ __device__ __forceinline__ TileAt tile_at(const ConvShape& cs, int tile) {
   return t;
 }
 
+// ---- GroupNorm + ReLU applied inside the conv kernel (GN != CV_GN_NONE) ----
+// The statistics of image b are complete once every item of b has been stored by all 8 MMA warps of the CTA that computed it.  After
+// its epilogue stores and statistics atomics an MMA warp only counts the item in shared memory (a CTA-scope release: no wait for its
+// stores to reach L2).  Warp 1 publishes them: once the MMA warps have counted all of the CTA's items of image b it adds them to
+// done[b] with a gpu-scope release, which makes those stores visible to the whole GPU (the release is cumulative) off the MMA warps'
+// critical path.  Warps 1-3 of warpgroup 0 (idle besides the TMA producer thread) walk the CTA's own items behind the MMA
+// warpgroups, wait for done[b] (gpu-scope acquire) and write
+// relu(GroupNorm(y)) of the item's 128 pixels x 128 channels, read back through L2: while the tensor cores run image b + 1.  The MMA
+// warps join the apply of the last image, which has nothing left to hide behind.  Only the wait crosses CTAs, so the launch is
+// cooperative (every CTA resident).  The arithmetic is gn_relu_apply_f16_v8_kernel's (CV_GN_F16) or gn_relu_apply_kernel's
+// (CV_GN_F32), element by element: the same bits.
+constexpr int CV_GN_NONE = 0, CV_GN_F16 = 1, CV_GN_F32 = 2;
+constexpr int CV_APPLY_WARPS = 3;                // warps 1-3 of warpgroup 0
+constexpr int CV_MMA_WARPS = 8;
+struct GnFuse {             // by-value kernel argument (unused when GN == CV_GN_NONE)
+  const float* gamma;
+  const float* beta;
+  float eps;
+  void* out;                // CV_GN_F16: __half h [B][H][W][256]; CV_GN_F32: float [B][H][W][256]
+  __half* out_l;            // CV_GN_F16: __half l
+  int* overflow_flag;       // optional, CV_GN_F16: raised when |GN output| > 60000 was clamped
+  int* done;                // [B] (item, MMA warp) completions, zero on entry
+};
+constexpr uint32_t CV_CNT_OFFSET = 2 * 8 * (CV_A_STAGES + CV_B_STAGES);   // shared item counters of MMA warpgroups 1, 2 (4 B each)
+
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ int ld_acquire_cta_shared(uint32_t a) {
+  int v;
+  asm volatile("ld.acquire.cta.shared::cta.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_cta_shared_add(uint32_t a, int v) {
+  asm volatile("red.release.cta.shared::cta.add.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+// lane 0 polls with backoff, then the warp proceeds (bounded: a protocol bug must not hang the GPU — trap after > 10 s)
+__device__ __forceinline__ void wait_count(const int* p, int target, int lane) {
+  if (lane == 0) {
+    uint32_t ns = 32, polls = 0;
+    while (ld_acquire_gpu(p) < target) {
+      __nanosleep(ns);
+      if (ns < 1024) ns <<= 1;
+      if (++polls > (1u << 24)) __trap();
+    }
+  }
+  __syncwarp();
+}
+// warp 1: publish this CTA's items of image b (item = its first one, last = the image's last item overall) to done[b], once the MMA
+// warps have counted them in shared memory (cnt, cnt + 4: (item, warp) completions of MMA warpgroup 1 / 2, in the CTA's walk order;
+// one counter per warpgroup, as the two may be an item apart)
+__device__ __forceinline__ void publish_image(uint32_t cnt, int* done_b, int item, int last, int lane) {
+  if (lane == 0) {
+    const int n = (last - item) / (int)gridDim.x + 1;                          // the CTA's items of the image
+    const int through = (item - (int)blockIdx.x) / (int)gridDim.x + n;         // CTA items up to and including the image's last
+    uint32_t ns = 32, polls = 0;
+    while (ld_acquire_cta_shared(cnt) < through * (CV_MMA_WARPS / 2) || ld_acquire_cta_shared(cnt + 4) < through * (CV_MMA_WARPS / 2)) {
+      __nanosleep(ns);
+      if (ns < 1024) ns <<= 1;
+      if (++polls > (1u << 24)) __trap();
+    }
+    red_release_gpu_add(done_b, n * CV_MMA_WARPS);
+  }
+  __syncwarp();
+}
+
+// relu(GroupNorm(y)) of one item (128 pixels x 128 channels at n0) by member `member` of a team of `team` warps: lane L owns channels
+// n0 + 4 L .. + 3 (one group of 8 per lane pair), a warp one pixel row (512 B of y) per step, four rows in flight.
+template <int GN>
+__device__ __forceinline__ void gn_apply_item(const ConvShape& cs, const GnFuse& gf, const float* __restrict__ y,
+                                              const double* __restrict__ stats, int item, int member, int team, int lane,
+                                              bool& clamped) {
+  const int tile = item / cs.n_slices, n0 = (item - tile * cs.n_slices) * CV_NT;
+  const TileAt ta = tile_at(cs, tile);
+  const int c = n0 + 4 * lane, g = c >> 3;
+  const int HW = cs.H * cs.W, cpg = CV_N / 32;
+  const double inv_n = 1.0 / ((double)HW * cpg);
+  const double s = __ldcg(stats + ((size_t)ta.b * 32 + g) * 2), ss = __ldcg(stats + ((size_t)ta.b * 32 + g) * 2 + 1);
+  const double mean = s * inv_n;
+  double var = ss * inv_n - mean * mean;
+  var = var < 0.0 ? 0.0 : var;
+  const float rstd = (float)(1.0 / sqrt(var + (double)gf.eps));
+  const float mu = (float)mean;
+  const float4 ga = __ldg(reinterpret_cast<const float4*>(gf.gamma + c)), be = __ldg(reinterpret_cast<const float4*>(gf.beta + c));
+  const int h_end = ta.shape == 2 ? cs.right_h : cs.H;     // the epilogue's edge rules
+  const int tw_mask = (1 << ta.twl) - 1;
+  const size_t img = (size_t)ta.b * HW * CV_N + c;           // element offsets below are relative to (image b, channel c)
+  const float* __restrict__ yb = y + img;
+  constexpr int U = 4;
+  for (int p0 = member; p0 < CV_BM; p0 += U * team) {
+    float4 v[U];
+    int at[U];                                                 // < H * W * 256 elements: one image
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int p = p0 + u * team;
+      const int h = ta.h0 + (p >> ta.twl), w = ta.w0 + (p & tw_mask);
+      at[u] = p < CV_BM && h < h_end && w < cs.W ? (h * cs.W + w) * CV_N : -1;
+      if (at[u] >= 0) v[u] = __ldcg(reinterpret_cast<const float4*>(yb + at[u]));
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (at[u] < 0) continue;
+      float o[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+      o[0] = fmaf((o[0] - mu) * rstd, ga.x, be.x); o[1] = fmaf((o[1] - mu) * rstd, ga.y, be.y);
+      o[2] = fmaf((o[2] - mu) * rstd, ga.z, be.z); o[3] = fmaf((o[3] - mu) * rstd, ga.w, be.w);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) o[j] = fmaxf(o[j], 0.f);
+      if constexpr (GN == CV_GN_F16) {
+        __align__(8) __half h[4], l[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          if (fabsf(o[j]) > 60000.f) { o[j] = copysignf(60000.f, o[j]); clamped = true; }
+          split_h2(o[j], h[j], l[j]);
+        }
+        *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(gf.out) + img + at[u]) = *reinterpret_cast<uint2*>(h);
+        *reinterpret_cast<uint2*>(gf.out_l + img + at[u]) = *reinterpret_cast<uint2*>(l);
+      } else {
+        *reinterpret_cast<float4*>(reinterpret_cast<float*>(gf.out) + img + at[u]) = make_float4(o[0], o[1], o[2], o[3]);
+      }
+    }
+  }
+}
+
 // F16 = false: 3xTF32 (operands fp32 hi/lo).  F16 = true: 2-term fp16 split (x = h + l, 22 significant bits): h*h + l*h + h*l,
 // the same three MMAs per k-step but K = 16 per MMA, i.e. half the tensor-pipe time and half the operand bytes.  out_scale undoes
 // the power-of-two scaling of the fp16 operands (exact).  NT: output channels per item (16, 32, 64 or 128; 128 in TF32 mode).
 // A_LO_ZERO: the activation's lo term is identically zero (an fp16 input): its box is not loaded and its MMA not issued; the result
 // has the bits of the full kernel fed an explicit all-zero lo.  OutT: element type of y (float, or __half / __nv_bfloat16 rounded
 // to nearest even from the same fp32 value; cs.ldy counts elements of OutT).
-template <bool F16, int NT, bool A_LO_ZERO = false, typename OutT = float>
+// GN: CV_GN_NONE, or GroupNorm + ReLU applied in the kernel (see GnFuse; fp16 mode, NT = 128, fp32 y, statistics on, no bias).
+template <bool F16, int NT, bool A_LO_ZERO = false, typename OutT = float, int GN = CV_GN_NONE>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, OutT* __restrict__ y, double* __restrict__ stats /*[B][32][2] or NULL*/,
-               float out_scale, const float* __restrict__ dev_out_scale, const float* __restrict__ bias) {
+               float out_scale, const float* __restrict__ dev_out_scale, const float* __restrict__ bias, GnFuse gf) {
   static_assert(F16 || NT == 128, "the TF32 mode runs 128-channel slices");
   static_assert(F16 || (!A_LO_ZERO && std::is_same<OutT, float>::value), "half-precision inputs and outputs belong to the fp16 mode");
+  static_assert(GN == CV_GN_NONE || (F16 && NT == 128 && std::is_same<OutT, float>::value), "the fused GroupNorm apply runs on fp32 y, NT 128");
   constexpr int KBC = F16 ? CV_KB_F16 : CV_KB;      // channels per K-block
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // swizzle atoms need (at least) 512 B alignment
@@ -142,13 +274,33 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, OutT* __restri
       mbar_init(full_b(s), 1);
       mbar_init(empty_b(s), 8);
     }
+    if constexpr (GN != CV_GN_NONE) asm volatile("st.shared.v2.u32 [%0], {0, 0};" ::"r"(bar_base + CV_CNT_OFFSET) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (wg == 0) {
-    // =============================== TMA producer ===============================
-    regs_dealloc<40>();
+    // =============================== TMA producer (+ GroupNorm apply: warps 1-3) ===============================
+    if constexpr (GN != CV_GN_NONE) {
+      regs_dealloc<72>();
+      const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+      if (warp >= 1) {
+        const int items_per_img = cs.per_img * cs.n_slices;      // items are image-major
+        bool clamped = false;
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+          const int b = item / items_per_img;
+          if (b == cs.B - 1) break;                          // the last image: the tail below, with the MMA warps
+          // the image's first item in this CTA's walk: warp 1 publishes the CTA's items of it
+          if (warp == 1 && item - (int)gridDim.x < b * items_per_img)
+            publish_image(bar_base + CV_CNT_OFFSET, gf.done + b, item, (b + 1) * items_per_img - 1, lane);
+          wait_count(gf.done + b, items_per_img * CV_MMA_WARPS, lane);
+          gn_apply_item<GN>(cs, gf, y, stats, item, warp - 1, CV_APPLY_WARPS, lane, clamped);
+        }
+        if (clamped && gf.overflow_flag) *gf.overflow_flag = 1;
+      }
+    } else {
+      regs_dealloc<40>();
+    }
     if (threadIdx.x == 0) {
       int a_st = 0, b_st = 0;
       uint32_t a_ph = 0, b_ph = 0;
@@ -182,8 +334,9 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, OutT* __restri
     }
   } else {
     // =============================== MMA + epilogue (warpgroups 1, 2) ===============================
-    regs_alloc<232>();
-    const int cw = wg - 1;                                   // pixel rows 64 cw .. 64 cw + 63 of the tile
+    if constexpr (GN != CV_GN_NONE) regs_alloc<216>();       // 128 x 72 + 256 x 216 <= 64 K registers
+    else regs_alloc<232>();
+    const int cw = wg - 1;                                  // pixel rows 64 cw .. 64 cw + 63 of the tile
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     const float sc = F16 ? (dev_out_scale ? __fmul_rn(out_scale, *dev_out_scale) : out_scale) : 1.f;   // powers of two: exact
     float acc[NT / 2], cor[NT / 2];
@@ -310,6 +463,27 @@ conv_tc_kernel(const __grid_constant__ ConvMaps mp, ConvShape cs, OutT* __restri
           atomicAdd(stats + ((size_t)ta.b * 32 + (n0 >> 3) + (lane >> 1)) * 2 + (lane & 1), (double)part[0]);
         }
       }
+      if constexpr (GN != CV_GN_NONE) {      // this warp's stores and statistics of the item are done: count them (warp 1 publishes)
+        __syncwarp();
+        if (lane == 0) red_release_cta_shared_add(bar_base + CV_CNT_OFFSET + 4u * cw, 1);
+      }
+    }
+  }
+  if constexpr (GN != CV_GN_NONE) {
+    // tail: the apply warps and the 8 MMA warps (11 warps, once each has run out of items) share this CTA's items of the last image,
+    // which has no MMA work left to hide behind.  One copy of this code serves both roles, so it fits the apply warps' registers.
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp >= 1) {
+      const int items_per_img = cs.per_img * cs.n_slices, last0 = (cs.B - 1) * items_per_img;
+      bool clamped = false;
+      int item = (int)blockIdx.x;
+      if (item < last0) item += (last0 - item + (int)gridDim.x - 1) / (int)gridDim.x * (int)gridDim.x;   // first item of the last image
+      if (warp == 1 && item < n_items) publish_image(bar_base + CV_CNT_OFFSET, gf.done + cs.B - 1, item, n_items - 1, lane);
+      for (; item < n_items; item += gridDim.x) {
+        wait_count(gf.done + cs.B - 1, items_per_img * CV_MMA_WARPS, lane);
+        gn_apply_item<GN>(cs, gf, y, stats, item, warp - 1, CV_APPLY_WARPS + CV_MMA_WARPS, lane, clamped);
+      }
+      if (clamped && gf.overflow_flag) *gf.overflow_flag = 1;
     }
   }
 }
@@ -689,16 +863,51 @@ static int conv_launch_nt(const ConvMaps& mp, const ConvShape& cs, OutT* y, doub
     return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the conv kernel");
   int grid = sm_count();                                     // persistent: one CTA per SM
   if (grid > cs.n_tiles * cs.n_slices) grid = cs.n_tiles * cs.n_slices;
-  conv_tc_kernel<F16, NT, A_LO_ZERO, OutT><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias);
+  conv_tc_kernel<F16, NT, A_LO_ZERO, OutT><<<grid, CV_THREADS, CV_SMEM_BYTES, (cudaStream_t)stream>>>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias,
+                                                                                                    GnFuse{});
   return 0;
 }
 
-// A_LO_ZERO: x_lo is not read (NULL).  OutT != float runs 128-channel slices only (n_mma > 64: the callers' input gradients).
-template <bool F16, bool A_LO_ZERO = false, typename OutT = float>
-static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, int H, int W, int Cin, int taps,
-                       int n_out, int n_mma, OutT* y, int ldy, const float* bias, double* gn_stats, float out_scale,
-                       const float* dev_out_scale, void* stream, const char* what) {
-  ConvShape cs;
+// the fused GroupNorm-apply conv: a cooperative launch, as its CTAs wait on each other's items.  *launched = false (nothing enqueued,
+// no error) when the grid cannot be co-resident or the device refuses the cooperative launch: the caller runs the two kernels.
+template <bool A_LO_ZERO, int GN>
+static int conv_gn_launch(const ConvMaps& mp, const ConvShape& cs, float* y, double* stats, float out_scale, const float* dev_out_scale,
+                          const GnFuse& gf, cudaStream_t st, bool* launched) {
+  *launched = false;
+  auto kern = conv_tc_kernel<true, CV_NT, A_LO_ZERO, float, GN>;
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CV_SMEM_BYTES) != cudaSuccess)
+    return fail("%s", "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed for the fused conv kernel");
+  const int n_items = cs.n_tiles * cs.n_slices;
+  const int grid = sm_count() < n_items ? sm_count() : n_items;
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CV_THREADS, CV_SMEM_BYTES) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  if (per_sm * sm_count() < grid) return 0;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(CV_THREADS);
+  cfg.dynamicSmemBytes = CV_SMEM_BYTES;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  const float* no_bias = nullptr;
+  if (cudaLaunchKernelEx(&cfg, kern, mp, cs, y, stats, out_scale, dev_out_scale, no_bias, gf) != cudaSuccess) {
+    (void)cudaGetLastError();          // a refused launch is not sticky: clear it and let the caller run the two kernels
+    return 0;
+  }
+  *launched = true;
+  return 0;
+}
+
+// tile plan, output-channel slice width (*nt) and tensor maps of one conv launch.  A_LO_ZERO: x_lo is not read (NULL).
+template <bool F16, bool A_LO_ZERO>
+static int conv_prepare(ConvShape& cs, ConvMaps& mp, int* nt_out, const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo,
+                        int B, int H, int W, int Cin, int taps, int n_out, int n_mma, int ldy, const double* gn_stats) {
   cs.B = B; cs.H = H; cs.W = W; cs.Cin = Cin;
   {   // tile plan (see ConvShape)
     const int rh = H % 8, rw = W % 16;
@@ -722,7 +931,6 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
   PTB_REQUIRE(!gn_stats || (n_out == CV_N && n_mma == CV_N && nt == CV_NT), "GroupNorm statistics need 256 output channels (32 groups of 8)");
   cs.n_slices = (n_mma + nt - 1) / nt;
   cs.taps = taps; cs.n_out = n_out; cs.ldy = ldy;
-  ConvMaps mp;
   int rc;
   for (int sh = 0; sh < 3; ++sh) {
     if ((rc = make_act_map(&mp.x[sh][0], x_hi, B, H, W, Cin, F16, sh, taps == 9 ? 2 : 0))) return rc;
@@ -731,6 +939,20 @@ static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, con
   }
   if ((rc = make_w_map(&mp.w[0], w_hi, n_mma, taps * Cin, F16, nt))) return rc;
   if ((rc = make_w_map(&mp.w[1], w_lo, n_mma, taps * Cin, F16, nt))) return rc;
+  *nt_out = nt;
+  return 0;
+}
+
+// A_LO_ZERO: x_lo is not read (NULL).  OutT != float runs 128-channel slices only (n_mma > 64: the callers' input gradients).
+template <bool F16, bool A_LO_ZERO = false, typename OutT = float>
+static int conv_launch(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, int B, int H, int W, int Cin, int taps,
+                       int n_out, int n_mma, OutT* y, int ldy, const float* bias, double* gn_stats, float out_scale,
+                       const float* dev_out_scale, void* stream, const char* what) {
+  ConvShape cs;
+  ConvMaps mp;
+  int nt = 0;
+  int rc = conv_prepare<F16, A_LO_ZERO>(cs, mp, &nt, x_hi, x_lo, w_hi, w_lo, B, H, W, Cin, taps, n_out, n_mma, ldy, gn_stats);
+  if (rc) return rc;
   if constexpr (!F16) rc = conv_launch_nt<false, 128>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
   else if (nt == 128) rc = conv_launch_nt<true, 128, A_LO_ZERO, OutT>(mp, cs, y, gn_stats, out_scale, dev_out_scale, bias, stream);
   else if constexpr (!std::is_same<OutT, float>::value) return fail("%s: a half-precision output needs more than 64 output channels", what);
@@ -853,6 +1075,46 @@ extern "C" int ptb_conv_tc_f16x1a(const void* x_h, const void* w_h, const void* 
               "16-byte alignment");
   return conv_launch<true, true>(x_h, nullptr, w_h, w_l, B, H, W, Cin, taps, n_out, n_mma, y, ldy, bias, gn_stats, out_scale, dev_out_scale,
                                  stream, "ptb_conv_tc_f16x1a");
+}
+
+extern "C" int ptb_conv3x3_c256_f16_gn(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin,
+                                       float out_scale, const float* dev_out_scale, float* y, void* workspace, const float* gamma,
+                                       const float* beta, float eps, void* out, void* out_l, int* overflow_flag, void* stream) {
+  PTB_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0, "shape");
+  PTB_REQUIRE(Cin % CV_KB_F16 == 0, "Cin must be a multiple of 32");
+  PTB_REQUIRE(x_h && w_h && w_l && y && workspace && gamma && beta && out, "NULL input");
+  PTB_REQUIRE(((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) && ((uintptr_t)w_h % 16 == 0) && ((uintptr_t)w_l % 16 == 0) &&
+                  ((uintptr_t)y % 16 == 0) && ((uintptr_t)workspace % 8 == 0) && ((uintptr_t)gamma % 16 == 0) && ((uintptr_t)beta % 16 == 0) &&
+                  ((uintptr_t)out % 16 == 0) && ((uintptr_t)out_l % 16 == 0), "alignment");
+  cudaStream_t st = (cudaStream_t)stream;
+  double* stats = reinterpret_cast<double*>(workspace);
+  GnFuse gf;
+  gf.gamma = gamma; gf.beta = beta; gf.eps = eps; gf.out = out; gf.out_l = reinterpret_cast<__half*>(out_l);
+  gf.overflow_flag = overflow_flag;
+  gf.done = reinterpret_cast<int*>(stats + (size_t)B * 32 * 2);
+  ConvShape cs;
+  ConvMaps mp;
+  int nt = 0, rc;
+  bool launched = false;
+  if (x_l) {
+    if ((rc = conv_prepare<true, false>(cs, mp, &nt, x_h, x_l, w_h, w_l, B, H, W, Cin, 9, CV_N, CV_N, CV_N, stats))) return rc;
+    rc = out_l ? conv_gn_launch<false, CV_GN_F16>(mp, cs, y, stats, out_scale, dev_out_scale, gf, st, &launched)
+               : conv_gn_launch<false, CV_GN_F32>(mp, cs, y, stats, out_scale, dev_out_scale, gf, st, &launched);
+  } else {
+    if ((rc = conv_prepare<true, true>(cs, mp, &nt, x_h, nullptr, w_h, w_l, B, H, W, Cin, 9, CV_N, CV_N, CV_N, stats))) return rc;
+    rc = out_l ? conv_gn_launch<true, CV_GN_F16>(mp, cs, y, stats, out_scale, dev_out_scale, gf, st, &launched)
+               : conv_gn_launch<true, CV_GN_F32>(mp, cs, y, stats, out_scale, dev_out_scale, gf, st, &launched);
+  }
+  if (rc) return rc;
+  if (launched) return check_launch("ptb_conv3x3_c256_f16_gn");
+  // the grid cannot be co-resident: the conv and the apply as two kernels (the same bits)
+  if (x_l) rc = conv_launch<true>(x_h, x_l, w_h, w_l, B, H, W, Cin, 9, CV_N, CV_N, y, CV_N, nullptr, stats, out_scale, dev_out_scale, stream,
+                                  "ptb_conv3x3_c256_f16_gn/conv");
+  else rc = conv_launch<true, true>(x_h, nullptr, w_h, w_l, B, H, W, Cin, 9, CV_N, CV_N, y, CV_N, nullptr, stats, out_scale, dev_out_scale,
+                                    stream, "ptb_conv3x3_c256_f16_gn/conv");
+  if (rc) return rc;
+  if (out_l) return ptb_gn_relu_apply_f16(y, stats, gamma, beta, B, H * W, CV_N, 32, eps, 1, out, out_l, overflow_flag, stream);
+  return ptb_gn_relu_apply(y, stats, gamma, beta, B, H * W, CV_N, 32, eps, 1, reinterpret_cast<float*>(out), nullptr, stream);
 }
 
 extern "C" int ptb_conv_tc_f16x2_half_out(const void* x_h, const void* x_l, const void* w_h, const void* w_l, int B, int H, int W, int Cin,

@@ -207,7 +207,8 @@ def _tc_train_supported(convs, x):
 
 class _TowerTCFn(torch.autograd.Function):
     """[conv3x3 -> GroupNorm -> ReLU] x n on the tensor cores with a hand-written backward:
-    forward  ptb_conv3x3_c256_f16x2 (+ GroupNorm statistics) / ptb_gn_relu_apply[_f16]      (csrc/conv_tc.cu)
+    forward  ptb_conv3x3_c256_f16_gn: the conv with GroupNorm statistics and the GroupNorm + ReLU apply in one launch
+             (the next layer's fp16 pair, fp32 after the last layer)                         (csrc/conv_tc.cu)
     backward ptb_gn_relu_bwd -> ptb_split_f16_amax -> ptb_conv3x3_wgrad_f16x2 (dW) and ptb_conv_tc_f16x2 with the transposed,
              flipped weights (dX)                                                          (csrc/tower_bwd.cu, wgrad_tc.cu)
     Saved per layer: the fp16 operand pair of its input (re-used as the wgrad operand), the conv output y and the statistics.
@@ -227,12 +228,14 @@ class _TowerTCFn(torch.autograd.Function):
             gamma, beta = params[3 * i + 1], params[3 * i + 2]
             wh, wl, inv_w = _packed_weight_f16(convs[i])          # cached per parameter version (no host sync per step)
             inv_x = dev_inv if i == 0 else None
-            y, stats = ops.conv3x3_c256_f16(h, l, wh, wl, inv_w, inv_x)
+            last = i == n_layers - 1
+            a, b, y, stats = ops.conv3x3_c256_f16_gn(h, l, wh, wl, inv_w, inv_x, gamma.detach(), beta.detach(), eps[i], flag,
+                                                     out='fp32' if last else 'f16pair')
             saved += [xm, None, y, stats] if i == 0 and half_in else [h, l, y, stats]
-            if i == n_layers - 1:
-                out = ops.gn_relu_apply(y, stats, gamma.detach(), beta.detach(), groups[i], eps[i], True, split=False)
+            if last:
+                out = a
             else:
-                h, l = ops.gn_relu_apply_f16(y, stats, gamma.detach(), beta.detach(), groups[i], eps[i], True, flag)
+                h, l = a, b
         ctx.n_layers, ctx.groups, ctx.eps, ctx.convs = n_layers, groups, eps, convs
         ctx.dev_inv, ctx.in_dtype = dev_inv, xm.dtype
         ctx.save_for_backward(*saved, *[p.detach() for p in params])
@@ -291,11 +294,14 @@ def tower(convs, x, info=None, want='fp32'):
         out = None
         for i, m in enumerate(convs):
             wh, wl, inv_w = _packed_weight_f16(m)
-            y, stats = ops.conv3x3_c256_f16(h, l, wh, wl, inv_w, dev_inv if i == 0 else None)
-            if i == len(convs) - 1 and want == 'fp32':
-                out = ops.gn_relu_apply(y, stats, m.gn.weight.detach(), m.gn.bias.detach(), m.gn.num_groups, m.gn.eps, True, split=False)
+            # conv + GroupNorm + ReLU in one launch: the apply runs inside the conv kernel (ptb_conv3x3_c256_f16_gn)
+            fp32_out = i == len(convs) - 1 and want == 'fp32'
+            a, b, _, _ = ops.conv3x3_c256_f16_gn(h, l, wh, wl, inv_w, dev_inv if i == 0 else None, m.gn.weight.detach(),
+                                                 m.gn.bias.detach(), m.gn.eps, flag, out='fp32' if fp32_out else 'f16pair')
+            if fp32_out:
+                out = a
             else:
-                h, l = ops.gn_relu_apply_f16(y, stats, m.gn.weight.detach(), m.gn.bias.detach(), m.gn.num_groups, m.gn.eps, True, flag)
+                h, l = a, b
         if info is not None:
             info['backend'] = 'wgmma-f16x2'
             info['input_path'] = plan[0]

@@ -915,6 +915,35 @@ def conv3x3_c256_f16(x_h, x_l, w_h, w_l, out_scale, dev_out_scale=None, want_sta
     return y, stats
 
 
+def conv3x3_c256_f16_gn(x_h, x_l, w_h, w_l, out_scale, dev_out_scale, gamma, beta, eps=1e-5, overflow_flag=None, out='f16pair'):
+    """ptb_conv3x3_c256_f16_gn: conv3x3_c256_f16 and GroupNorm(32) + ReLU in one launch.  out='f16pair' -> (h, l, y, stats), what
+    gn_relu_apply_f16 gives on y and stats; out='fp32' -> (relu(GN(y)), None, y, stats), what gn_relu_apply(split=False) gives.
+    x_l None: x_h is an fp16 tensor used as is (lo == 0)."""
+    lib = _lib.load()
+    _chk(x_h, torch.float16, 'x_h'); _chk(w_h, torch.float16, 'w_h'); _chk(w_l, torch.float16, 'w_l')
+    _chk(gamma, torch.float32, 'gamma'); _chk(beta, torch.float32, 'beta')
+    if x_l is not None:
+        _chk(x_l, torch.float16, 'x_l')
+    if out not in ('f16pair', 'fp32'):
+        raise ValueError(f"out must be 'f16pair' or 'fp32', got {out!r}")
+    B, H, W, Cin = x_h.shape
+    if w_h.shape != (256, 9 * Cin) or gamma.shape != (256,) or beta.shape != (256,):
+        raise ValueError('packed weight must be (256, 9*Cin), gamma and beta (256,)')
+    dev = x_h.device
+    y = torch.empty((B, H, W, 256), dtype=torch.float32, device=dev)
+    ws = torch.zeros(B * 64 + (B + 1) // 2, dtype=torch.float64, device=dev)     # statistics [B][32][2], then B int32 counters
+    stats = ws[:B * 64].view(B, 32, 2)
+    if out == 'f16pair':
+        a = torch.empty((B, H, W, 256), dtype=torch.float16, device=dev)
+        b = torch.empty_like(a)
+    else:
+        a, b = torch.empty_like(y), None
+    check(lib.ptb_conv3x3_c256_f16_gn(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, float(out_scale), _ptr(dev_out_scale),
+                                      _ptr(y), _ptr(ws), _ptr(gamma), _ptr(beta), float(eps), _ptr(a), _ptr(b), _ptr(overflow_flag),
+                                      _stream()), 'ptb_conv3x3_c256_f16_gn')
+    return a, b, y, stats
+
+
 def gn_relu_apply_f16(y, stats, gamma, beta, groups=32, eps=1e-5, relu=True, overflow_flag=None):
     lib = _lib.load()
     _chk(y, torch.float32, 'y'); _chk(stats, torch.float64, 'stats')

@@ -87,8 +87,12 @@ def main():
     pk_p2p = ops.conv_tc_pack_weight_f16((torch.randn(320, C, 3, 3, generator=g) * 0.02).reshape(320, C, 9).to(dev), 9)
     pk_lin = ops.conv_tc_pack_weight_f16((torch.randn(80, C, generator=g) * 0.05).to(dev), 1)
     bias = torch.zeros(320, device=dev)
+    gamma, beta = torch.ones(C, device=dev), torch.zeros(C, device=dev)
     launches = [
         ('tower conv3x3 256->256 fp16x2 (+GN stats)', lambda: ops.conv3x3_c256_f16(h16, l16, wh16, wl16, invw, dinv), 9, 256, True),
+        # the launch the towers make: the same conv with GroupNorm + ReLU applied in the kernel, written as the next layer's fp16 pair
+        ('tower conv3x3 256->256 fp16x2 + GN apply in the kernel (fp16 pair out)',
+         lambda: ops.conv3x3_c256_f16_gn(h16, l16, wh16, wl16, invw, dinv, gamma, beta), 9, 256, True),
         ('tower conv3x3 256->256 3xTF32 (+GN stats)', lambda: ops.conv3x3_c256(xh, xl, wh, wl), 9, 256, False),
         ('tower dgrad conv3x3 256->256 fp16x2', lambda: ops.conv_tc_f16(h16, l16, pk_dgrad, 9, C, dev_out_scale=dinv), 9, 256, True),
         ('P2P cls_out conv3x3 256->320 fp16x2', lambda: ops.conv_tc_f16(h16, l16, pk_p2p, 9, 320, bias=bias, dev_out_scale=dinv), 9, 320, True),
