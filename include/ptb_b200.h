@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define PTB_ABI_VERSION 1
+#define PTB_ABI_VERSION 2
 
 int ptb_abi_version(void);
 const char* ptb_last_error(void);
@@ -162,36 +162,27 @@ int ptb_cpr_refine_fused(const float* logit_map /*[B][H][W][ld]*/, int B, int H,
  * ins at column ins_off).  weight[g][k] = valid * gt_weight (cpr_head.py:1211).
  *   out_bag_prob[g][c] = sum_k sigmoid(cls) * normalize_L1(softmax_k(ins) * weight)
  *       (the buffer must hold G*num_classes + 3*G floats: the trailing 3*G are per-bag loss / weight / hit scratch)
- *   out_loss_sum[0]   += sum_g gfocal(bag_prob[g], onehot(labels[g])) * (any_k weight>0)      (un-normalised)
+ *   out_loss_sum[0]   += sum_g term(bag_prob[g], onehot(labels[g])) * (any_k weight>0)      (un-normalised; term below)
  *   out_stats[0] += #bags with any weight>0 ; out_stats[1] += #bags whose argmax == label
  * bwd: d(loss_sum)/d(cls logits), d/d(ins logits) scaled by `scale` (= loss_weight / num_sample).
+ * loss_kind selects the loss term of the positive bags (MILLoss / AllPosLoss `loss_type`, multi_instance_learning_loss.py:187-202, 229-240):
+ *   PTB_LOSS_GFOCAL  gfocal_loss(p, onehot) x label weight (the bag's any-weight flag for MIL, w_k for AllPos)
+ *   PTB_LOSS_BCE     F.binary_cross_entropy(p, onehot) UNWEIGHTED: (t-1) max(log1p(-p), -100) - t max(log p, -100), as ATen on the CPU;
+ *                    a MIL bag whose weights are all zero (prob = 0) still adds 100 at its label column, with zero gradient.
+ *                    A probability above 1 (rounding of saturated sigmoids; ATen raises) gives NaN.
  */
+#define PTB_LOSS_GFOCAL 0
+#define PTB_LOSS_BCE 1
 int ptb_mil_loss_fwd(const float* logits /*[G][Kt][ld]*/, int G, int Kt, int num_classes, int ld, int ins_off,
-                     const float* weight /*[G][Kt]*/, const int32_t* labels, float eps,
+                     const float* weight /*[G][Kt]*/, const int32_t* labels, float eps, int loss_kind,
                      float* out_bag_prob /*[G][num_classes]*/, float* out_loss_sum /*[1]*/, float* out_stats /*[2]*/,
                      float* out_mt /*[G][num_classes][2] = (max_k ins, 1/T or 0 if the L1-normalisation clamp is active) or NULL:
                                      what ptb_cpr_loss_bwd_map needs of the forward*/,
                      void* stream);
 int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off,
-                     const float* weight, const int32_t* labels, float eps, const float* bag_prob,
+                     const float* weight, const int32_t* labels, float eps, int loss_kind, const float* bag_prob,
                      const float* scale /*[1] device scalar*/, float* grad_logits /*[G][Kt][ld], cls+ins columns written*/,
                      void* stream);
-
-/* Loss term of the positive bags (MILLoss / AllPosLoss `loss_type`, multi_instance_learning_loss.py:187-202, 229-240):
- *   PTB_LOSS_GFOCAL  gfocal_loss(p, onehot) x label weight (the bag's any-weight flag for MIL, w_k for AllPos)
- *   PTB_LOSS_BCE     F.binary_cross_entropy(p, onehot) UNWEIGHTED: (t-1) max(log1p(-p), -100) - t max(log p, -100), as ATen on the CPU;
- *                    a MIL bag whose weights are all zero (prob = 0) still adds 100 at its label column, with zero gradient.
- *                    A probability above 1 (rounding of saturated sigmoids; ATen raises) gives NaN.
- * The _kind entry points below are the entry points above with a loss_kind argument; loss_kind = PTB_LOSS_GFOCAL gives their results
- * bit for bit. */
-#define PTB_LOSS_GFOCAL 0
-#define PTB_LOSS_BCE 1
-int ptb_mil_loss_fwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                          const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum, float* out_stats,
-                          float* out_mt, void* stream);
-int ptb_mil_loss_bwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                          const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale, float* grad_logits,
-                          void* stream);
 /* AllPosLoss forward (multi_instance_learning_loss.py:206-243): every bag sample is a row p = sigmoid(logits[g][k][0..num_classes)) with
  * the label of its bag.  aux [3*G] scratch; fixed-order sums (deterministic):
  *   out_loss_sum[0] += sum_{g,k,c} term(p, onehot) (x weight[g][k] for PTB_LOSS_GFOCAL; unweighted over ALL samples for PTB_LOSS_BCE)
@@ -206,13 +197,9 @@ int ptb_cpr_allpos_fwd(const float* logits /*[G][K][ld]*/, int G, int K, int num
  * is written once and never re-read by the forward.  out_bag_prob needs G*num_classes + 3*G floats like ptb_mil_loss_fwd. */
 int ptb_cpr_bag_mil_fwd(const float* logit_map /*[B][H][W][ld]*/, int B, int H, int W, int ld, int num_classes, int ins_off,
                         const float* centers, const int32_t* bag_img, int G, const float* offsets, int K, float stride,
-                        const int32_t* pad_hw, const int32_t* labels, float eps, float* out_bag_logits, float* out_weight,
+                        const int32_t* pad_hw, const int32_t* labels, float eps, int loss_kind, float* out_bag_logits, float* out_weight,
                         float* out_bag_prob, float* out_loss_sum /*[1]*/, float* out_stats /*[2]*/, float* out_mt /*[G][N][2] or NULL*/,
                         void* stream);
-int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off, const float* centers,
-                             const int32_t* bag_img, int G, const float* offsets, int K, float stride, const int32_t* pad_hw,
-                             const int32_t* labels, float eps, int loss_kind, float* out_bag_logits, float* out_weight, float* out_bag_prob,
-                             float* out_loss_sum, float* out_stats, float* out_mt, void* stream);
 
 /* Backward of the whole CPR training loss w.r.t. the LOGIT MAP in one deterministic kernel (gather formulation, no atomics on global
  * memory): replaces autograd of MILLoss (multi_instance_learning_loss.py:153-203), of the gt / neg gfocal terms (cpr_head.py:1159-1184,
@@ -224,53 +211,41 @@ int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, int W, int ld
  * grad_map is written (no zero-init needed).  One CTA per 8x8-cell tile; every sum is formed by one thread in a fixed order, so the
  * result is bit-identical run to run.  ld must be a multiple of 32 and at most 160 (every such ld, 32 to 160, is exact: narrow rows run
  * smaller blocks and rounds of blockDim / 4 samples); K <= 320; reach_px must be at least the largest |offset| component, or samples
- * outside the window are lost. */
-int ptb_cpr_loss_bwd_map(const float* bag_logits /*[G][K][ld]*/, const float* weight /*[G][K]*/, const float* mil_mt /*[G][N][2]*/,
+ * outside the window are lost.
+ * loss_kind is that of the bag term and of the per-sample positive term (AllPosLoss):
+ *   mil_mt == NULL      no MIL term (bag_prob, label_weight, scale_mil unused; the ins columns get no gradient);
+ *   scale_pos != NULL   every sample k of every bag adds scale_pos * w * term'(sigmoid(cls)) * sigmoid'(cls) to its cls columns, with
+ *                       w = weight[g][k] for PTB_LOSS_GFOCAL and w = 1 for PTB_LOSS_BCE (samples outside pad_shape included). */
+int ptb_cpr_loss_bwd_map(const float* bag_logits /*[G][K][ld]*/, const float* weight /*[G][K]*/, const float* mil_mt /*[G][N][2] or NULL*/,
                          const float* bag_prob /*[G][N]*/, const float* label_weight /*[G]*/, const int32_t* labels,
                          const float* centers /*[G][2]*/, const int32_t* img_ptr /*[B+1]*/, const float* offsets /*[K][2]*/,
                          int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld, float stride, float reach_px, float eps,
                          const float* scale_mil /*[1] or NULL*/, const float* scale_gt /*[1] or NULL*/,
                          const float* valid_center /*[G] or NULL*/, const float* logit_map /*[B][H][W][ld] or NULL*/,
                          const uint8_t* neg_mask /*[B][H][W][N]*/, const float* scale_neg /*[1]*/,
+                         int loss_kind, const float* scale_pos /*[1] or NULL*/,
                          void* workspace /*ptb_cpr_loss_bwd_map_workspace(G, N) bytes, 16-byte aligned*/,
                          float* grad_map /*[B][H][W][ld]*/, void* stream);
 uint64_t ptb_cpr_loss_bwd_map_workspace(int G, int num_classes);
 /* Scatter form of the MIL + gt part of the same gradient (fastest; fp32 vector atomics, so NOT bit-reproducible): one CTA per bag adds
  * w_tap * dLoss/d bag_logits straight into grad_map, which the caller has initialised (zeros, or the neg-loss term written by
- * ptb_gfocal_sigmoid_bwd).  Same inputs as ptb_cpr_loss_bwd_map except bag_img [G] instead of img_ptr; workspace as above. */
+ * ptb_sigmoid_loss_bwd).  Same inputs as ptb_cpr_loss_bwd_map except bag_img [G] instead of img_ptr; workspace as above. */
 int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
                              const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
                              const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
                              float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
+                             int loss_kind, const float* scale_pos /*[1] or NULL*/,
                              void* workspace, float* grad_map /*[B][H][W][ld], accumulated into*/, void* stream);
-/* The two map backwards with the loss kind of the bag term and a per-sample positive term (AllPosLoss):
- *   mil_mt == NULL      no MIL term (bag_prob, label_weight, scale_mil unused; the ins columns get no gradient);
- *   scale_pos != NULL   every sample k of every bag adds scale_pos * w * term'(sigmoid(cls)) * sigmoid'(cls) to its cls columns, with
- *                       w = weight[g][k] for PTB_LOSS_GFOCAL and w = 1 for PTB_LOSS_BCE (samples outside pad_shape included). */
-int ptb_cpr_loss_bwd_map_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                              const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
-                              const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                              float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
-                              const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
-                              int loss_kind, const float* scale_pos /*[1] or NULL*/, void* workspace, float* grad_map, void* stream);
-int ptb_cpr_loss_bwd_scatter_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                  const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
-                                  const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                  float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
-                                  int loss_kind, const float* scale_pos /*[1] or NULL*/, void* workspace, float* grad_map, void* stream);
 
 /* gfocal on sigmoid(logits) vs a one-hot / all-zero target with per-element weights — replaces
  * MILLoss.gfocal_loss (multi_instance_learning_loss.py:148-151) as used for gt_loss and neg_loss
  * (cpr_head.py:1159-1184, 1219-1228).  rows: logits[m*row_stride + c], c<num_classes;
  * target_label[m] in [0,num_classes) or -1 (all-zero target); weight is uint8 [M][num_classes] (wmode 0),
- * float [M] (wmode 1) or NULL (all ones).  loss_sum[0] += sum.   bwd: grad = scale[0] * dloss/dlogit (overwrite or add). */
+ * float [M] (wmode 1) or NULL (all ones).  loss_sum[0] += sum.   bwd: grad = scale[0] * dloss/dlogit (overwrite or add), where the loss
+ * is this gfocal for PTB_LOSS_GFOCAL and weight * BCE(sigmoid(logit), target) for PTB_LOSS_BCE. */
 int ptb_gfocal_sigmoid_fwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
                            const int32_t* target_label, const void* weight, int wmode, float eps,
                            float* loss_sum, void* stream);
-int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
-                           const int32_t* target_label, const void* weight, int wmode, float eps,
-                           const float* scale, float* grad, int64_t grad_row_stride, int accumulate, void* stream);
-/* ptb_gfocal_sigmoid_bwd with the loss kind: PTB_LOSS_BCE gives scale * weight * d BCE(sigmoid(logit), target) / d logit. */
 int ptb_sigmoid_loss_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride, const int32_t* target_label,
                          const void* weight, int wmode, float eps, int loss_kind, const float* scale, float* grad,
                          int64_t grad_row_stride, int accumulate, void* stream);

@@ -44,25 +44,17 @@ SIGNATURES = {
     'ptb_cpr_refine': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, RefineCfg, P, P, P, P, P, P]),
     'ptb_cpr_refine_fused': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, P, c_int, P, c_int, c_float, c_float, P, P, P, P, P,
                                      P, RefineCfg, P, P, P, P, P]),
-    'ptb_mil_loss_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, P, P, P, P, P]),
-    'ptb_cpr_bag_mil_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, P, P, c_float, P, P, P, P, P, P, P]),
+    'ptb_mil_loss_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P, P]),
+    'ptb_cpr_bag_mil_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, P, P, c_float, c_int,
+                                    P, P, P, P, P, P, P]),
     'ptb_cpr_loss_bwd_map': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
-                                     P, P, P, P, P, P, P, P, P]),
+                                     P, P, P, P, P, P, c_int, P, P, P, P]),
     'ptb_cpr_loss_bwd_map_workspace': (c_u64, [c_int, c_int]),
     'ptb_cpr_loss_bwd_scatter': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
-                                         P, P, P, P, P, P]),
-    'ptb_mil_loss_bwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, P, P, P, P]),
+                                         P, P, P, c_int, P, P, P, P]),
+    'ptb_mil_loss_bwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P]),
     'ptb_gfocal_sigmoid_fwd': (c_int, [P, c_i64, c_int, c_i64, P, P, c_int, c_float, P, P]),
-    'ptb_gfocal_sigmoid_bwd': (c_int, [P, c_i64, c_int, c_i64, P, P, c_int, c_float, P, P, c_i64, c_int, P]),
-    'ptb_mil_loss_fwd_kind': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P, P]),
-    'ptb_mil_loss_bwd_kind': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P]),
     'ptb_cpr_allpos_fwd': (c_int, [P, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P]),
-    'ptb_cpr_bag_mil_fwd_kind': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, P, P, c_float, c_int,
-                                         P, P, P, P, P, P, P]),
-    'ptb_cpr_loss_bwd_map_kind': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
-                                          c_float, P, P, P, P, P, P, c_int, P, P, P, P]),
-    'ptb_cpr_loss_bwd_scatter_kind': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
-                                              c_float, P, P, P, c_int, P, P, P, P]),
     'ptb_sigmoid_loss_bwd': (c_int, [P, c_i64, c_int, c_i64, P, P, c_int, c_float, c_int, P, P, c_i64, c_int, P]),
     'ptb_p2p_decode_topk': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, c_float, c_float, P, P, c_int, P, P, P, P,
                                     c_u64, P]),
@@ -143,7 +135,7 @@ def load():
         fn.argtypes = args
     global MISSING
     MISSING = missing      # tests/test_capi_symbols.py requires this to be empty
-    if lib.ptb_abi_version() != 1:
+    if lib.ptb_abi_version() != 2:
         raise RuntimeError('libptb_b200.so ABI version mismatch')
     _lib = lib
     return lib

@@ -383,12 +383,12 @@ extern "C" uint64_t ptb_cpr_loss_bwd_map_workspace(int G, int num_classes) {
   return (uint64_t)(G > 0 ? G : 1) * (uint64_t)(num_classes > 0 ? num_classes : 1) * sizeof(float4);
 }
 
-extern "C" int ptb_cpr_loss_bwd_map_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                         const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
-                                         const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                         float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
-                                         const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
-                                         int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
+extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                    const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
+                                    const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                    float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
+                                    const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
+                                    int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 32 * LB_NIT, "shape (num_classes <= 256)");
   PTB_REQUIRE(ld >= ins_off + num_classes && ins_off >= num_classes && stride > 0.f && reach_px >= 0.f, "ld / ins_off / stride");
   PTB_REQUIRE(ld % 32 == 0 && ld <= 512, "ld must be a multiple of 32 (32-channel register groups), at most 512");
@@ -427,23 +427,11 @@ extern "C" int ptb_cpr_loss_bwd_map_kind(const float* bag_logits, const float* w
   return check_launch("ptb_cpr_loss_bwd_map");
 }
 
-extern "C" int ptb_cpr_loss_bwd_map(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                    const float* label_weight, const int32_t* labels, const float* centers, const int32_t* img_ptr,
-                                    const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                    float stride, float reach_px, float eps, const float* scale_mil, const float* scale_gt,
-                                    const float* valid_center, const float* logit_map, const uint8_t* neg_mask, const float* scale_neg,
-                                    void* workspace, float* grad_map, void* stream) {
-  PTB_REQUIRE(G == 0 || mil_mt, "NULL input");
-  return ptb_cpr_loss_bwd_map_kind(bag_logits, weight, mil_mt, bag_prob, label_weight, labels, centers, img_ptr, offsets, B, H, W, G, K,
-                                   num_classes, ins_off, ld, stride, reach_px, eps, scale_mil, scale_gt, valid_center, logit_map, neg_mask,
-                                   scale_neg, LOSS_GFOCAL, nullptr, workspace, grad_map, stream);
-}
-
-extern "C" int ptb_cpr_loss_bwd_scatter_kind(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                             const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
-                                             const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                             float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
-                                             int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
+extern "C" int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
+                                        const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
+                                        const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
+                                        float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
+                                        int loss_kind, const float* scale_pos, void* workspace, float* grad_map, void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 4 * LS_THREADS, "shape");
   PTB_REQUIRE(ld >= ins_off + num_classes && ins_off >= num_classes && ins_off % 4 == 0 && ld % 4 == 0 && stride > 0.f, "ld / ins_off / stride");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
@@ -471,15 +459,4 @@ extern "C" int ptb_cpr_loss_bwd_scatter_kind(const float* bag_logits, const floa
     return fail("%s", "ptb_cpr_loss_bwd_scatter: shared memory opt-in failed");
   cpr_loss_bwd_scatter_kernel<<<G, LS_THREADS, smem, st>>>(a, bag_img);
   return check_launch("ptb_cpr_loss_bwd_scatter");
-}
-
-extern "C" int ptb_cpr_loss_bwd_scatter(const float* bag_logits, const float* weight, const float* mil_mt, const float* bag_prob,
-                                        const float* label_weight, const int32_t* labels, const float* centers, const int32_t* bag_img,
-                                        const float* offsets, int B, int H, int W, int G, int K, int num_classes, int ins_off, int ld,
-                                        float stride, float eps, const float* scale_mil, const float* scale_gt, const float* valid_center,
-                                        void* workspace, float* grad_map, void* stream) {
-  PTB_REQUIRE(G == 0 || mil_mt, "NULL input");
-  return ptb_cpr_loss_bwd_scatter_kind(bag_logits, weight, mil_mt, bag_prob, label_weight, labels, centers, bag_img, offsets, B, H, W, G, K,
-                                       num_classes, ins_off, ld, stride, eps, scale_mil, scale_gt, valid_center, LOSS_GFOCAL, nullptr,
-                                       workspace, grad_map, stream);
 }

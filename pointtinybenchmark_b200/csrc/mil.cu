@@ -449,9 +449,9 @@ static int with_term(int kind, float eps, F&& f) {
   return f(GfocalTerm{eps});
 }
 
-extern "C" int ptb_mil_loss_fwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                     const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum,
-                                     float* out_stats, float* out_mt, void* stream) {
+extern "C" int ptb_mil_loss_fwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum,
+                                float* out_stats, float* out_mt, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
   PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
@@ -471,16 +471,9 @@ extern "C" int ptb_mil_loss_fwd_kind(const float* logits, int G, int Kt, int num
   return check_launch("ptb_mil_loss_fwd/finish");
 }
 
-extern "C" int ptb_mil_loss_fwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                const int32_t* labels, float eps, float* out_bag_prob, float* out_loss_sum, float* out_stats,
-                                float* out_mt, void* stream) {
-  return ptb_mil_loss_fwd_kind(logits, G, Kt, num_classes, ld, ins_off, weight, labels, eps, LOSS_GFOCAL, out_bag_prob, out_loss_sum,
-                               out_stats, out_mt, stream);
-}
-
-extern "C" int ptb_mil_loss_bwd_kind(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                     const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale,
-                                     float* grad_logits, void* stream) {
+extern "C" int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
+                                const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale,
+                                float* grad_logits, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
   PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
@@ -493,13 +486,6 @@ extern "C" int ptb_mil_loss_bwd_kind(const float* logits, int G, int Kt, int num
     return 0;
   });
   return check_launch("ptb_mil_loss_bwd");
-}
-
-extern "C" int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_classes, int ld, int ins_off, const float* weight,
-                                const int32_t* labels, float eps, const float* bag_prob, const float* scale, float* grad_logits,
-                                void* stream) {
-  return ptb_mil_loss_bwd_kind(logits, G, Kt, num_classes, ld, ins_off, weight, labels, eps, LOSS_GFOCAL, bag_prob, scale, grad_logits,
-                               stream);
 }
 
 extern "C" int ptb_cpr_allpos_fwd(const float* logits, int G, int K, int num_classes, int ld, const float* weight, const int32_t* labels,
@@ -546,21 +532,14 @@ extern "C" int ptb_sigmoid_loss_bwd(const float* logits, int64_t M, int num_clas
                                                                         wmode, term, scale, grad, grad_row_stride, accumulate);
     return 0;
   });
-  return check_launch("ptb_gfocal_sigmoid_bwd");
+  return check_launch("ptb_sigmoid_loss_bwd");
 }
 
-extern "C" int ptb_gfocal_sigmoid_bwd(const float* logits, int64_t M, int num_classes, int64_t row_stride,
-                                      const int32_t* target_label, const void* weight, int wmode, float eps, const float* scale,
-                                      float* grad, int64_t grad_row_stride, int accumulate, void* stream) {
-  return ptb_sigmoid_loss_bwd(logits, M, num_classes, row_stride, target_label, weight, wmode, eps, LOSS_GFOCAL, scale, grad,
-                              grad_row_stride, accumulate, stream);
-}
-
-extern "C" int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off,
-                                        const float* centers, const int32_t* bag_img, int G, const float* offsets, int K, float stride,
-                                        const int32_t* pad_hw, const int32_t* labels, float eps, int loss_kind, float* out_bag_logits,
-                                        float* out_weight, float* out_bag_prob, float* out_loss_sum, float* out_stats, float* out_mt,
-                                        void* stream) {
+extern "C" int ptb_cpr_bag_mil_fwd(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off,
+                                   const float* centers, const int32_t* bag_img, int G, const float* offsets, int K, float stride,
+                                   const int32_t* pad_hw, const int32_t* labels, float eps, int loss_kind, float* out_bag_logits,
+                                   float* out_weight, float* out_bag_prob, float* out_loss_sum, float* out_stats, float* out_mt,
+                                   void* stream) {
   PTB_REQUIRE(B > 0 && H > 0 && W > 0 && G >= 0 && K > 0 && num_classes > 0 && num_classes <= 128 && stride > 0.f, "shape (num_classes <= 128)");
   PTB_REQUIRE(ld % 4 == 0 && ins_off % 4 == 0 && ins_off >= num_classes && ld >= ins_off + ((num_classes + 3) / 4) * 4, "ld / ins_off");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
@@ -586,12 +565,4 @@ extern "C" int ptb_cpr_bag_mil_fwd_kind(const float* logit_map, int B, int H, in
   if (rc) return rc;
   mil_finish_kernel<<<1, 1024, 0, st>>>(aux, G, out_loss_sum, out_stats);
   return check_launch("ptb_cpr_bag_mil_fwd/finish");
-}
-
-extern "C" int ptb_cpr_bag_mil_fwd(const float* logit_map, int B, int H, int W, int ld, int num_classes, int ins_off, const float* centers,
-                                   const int32_t* bag_img, int G, const float* offsets, int K, float stride, const int32_t* pad_hw,
-                                   const int32_t* labels, float eps, float* out_bag_logits, float* out_weight, float* out_bag_prob,
-                                   float* out_loss_sum, float* out_stats, float* out_mt, void* stream) {
-  return ptb_cpr_bag_mil_fwd_kind(logit_map, B, H, W, ld, num_classes, ins_off, centers, bag_img, G, offsets, K, stride, pad_hw, labels, eps,
-                                  LOSS_GFOCAL, out_bag_logits, out_weight, out_bag_prob, out_loss_sum, out_stats, out_mt, stream);
 }

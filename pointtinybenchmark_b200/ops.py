@@ -302,7 +302,7 @@ LOSS_KINDS = {'gfocal_loss': 0, 'binary_cross_entropy': 1}      # PTB_LOSS_GFOCA
 
 
 def mil_loss_fwd(logits, num_classes, ins_off, weight, labels, eps, want_aux=False, loss_kind=0):
-    """ptb_mil_loss_fwd (ptb_mil_loss_fwd_kind for loss_kind != 0).  logits (G,Kt,ld) [cls | ins]; weight (G,Kt) fp32; labels (G,) int32.
+    """ptb_mil_loss_fwd.  logits (G,Kt,ld) [cls | ins]; weight (G,Kt) fp32; labels (G,) int32.
     returns bag_prob (G,C), loss_sum (1,), stats (2,) = [#bags with weight, #top-1 hits]."""
     lib = _lib.load()
     _chk(logits, torch.float32, 'logits'); _chk(weight, torch.float32, 'weight'); _chk(labels, torch.int32, 'labels')
@@ -311,12 +311,8 @@ def mil_loss_fwd(logits, num_classes, ins_off, weight, labels, eps, want_aux=Fal
     loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
     stats = torch.zeros(2, dtype=torch.float32, device=logits.device)
     mt = torch.empty((G, num_classes, 2), dtype=torch.float32, device=logits.device) if want_aux else None
-    if loss_kind == 0:
-        check(lib.ptb_mil_loss_fwd(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps),
-                                   _ptr(buf), _ptr(loss), _ptr(stats), _ptr(mt), _stream()), 'ptb_mil_loss_fwd')
-    else:
-        check(lib.ptb_mil_loss_fwd_kind(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps), int(loss_kind),
-                                        _ptr(buf), _ptr(loss), _ptr(stats), _ptr(mt), _stream()), 'ptb_mil_loss_fwd_kind')
+    check(lib.ptb_mil_loss_fwd(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps), int(loss_kind),
+                               _ptr(buf), _ptr(loss), _ptr(stats), _ptr(mt), _stream()), 'ptb_mil_loss_fwd')
     bag_prob = buf[:G * num_classes].view(G, num_classes)
     if want_aux:         # (max ins, 1/T) per (bag, class) and the per-bag label weight: inputs of ptb_cpr_loss_bwd_map
         return bag_prob, loss, stats, mt, buf[G * num_classes + G:G * num_classes + 2 * G]
@@ -339,14 +335,9 @@ def bag_mil_fwd(lmap, num_classes, ins_off, centers, bag_img, offsets, stride, p
     loss = torch.zeros(1, dtype=torch.float32, device=dev)
     stats = torch.zeros(2, dtype=torch.float32, device=dev)
     mt = torch.empty((G, num_classes, 2), dtype=torch.float32, device=dev)
-    if loss_kind == 0:
-        check(lib.ptb_cpr_bag_mil_fwd(_ptr(lmap), B, H, W, ld, num_classes, ins_off, _ptr(centers), _ptr(bag_img), G, _ptr(offsets), K,
-                                      float(stride), _ptr(pad_hw), _ptr(labels), float(eps), _ptr(bl), _ptr(weight), _ptr(buf), _ptr(loss),
-                                      _ptr(stats), _ptr(mt), _stream()), 'ptb_cpr_bag_mil_fwd')
-    else:
-        check(lib.ptb_cpr_bag_mil_fwd_kind(_ptr(lmap), B, H, W, ld, num_classes, ins_off, _ptr(centers), _ptr(bag_img), G, _ptr(offsets), K,
-                                           float(stride), _ptr(pad_hw), _ptr(labels), float(eps), int(loss_kind), _ptr(bl), _ptr(weight),
-                                           _ptr(buf), _ptr(loss), _ptr(stats), _ptr(mt), _stream()), 'ptb_cpr_bag_mil_fwd_kind')
+    check(lib.ptb_cpr_bag_mil_fwd(_ptr(lmap), B, H, W, ld, num_classes, ins_off, _ptr(centers), _ptr(bag_img), G, _ptr(offsets), K,
+                                  float(stride), _ptr(pad_hw), _ptr(labels), float(eps), int(loss_kind), _ptr(bl), _ptr(weight), _ptr(buf),
+                                  _ptr(loss), _ptr(stats), _ptr(mt), _stream()), 'ptb_cpr_bag_mil_fwd')
     return (bl, weight, buf[:G * num_classes].view(G, num_classes), loss, stats, mt, buf[G * num_classes + G:G * num_classes + 2 * G])
 
 
@@ -356,12 +347,8 @@ def mil_loss_bwd(logits, num_classes, ins_off, weight, labels, eps, bag_prob, sc
     grad = grad_out if grad_out is not None else torch.zeros_like(logits)
     _chk(scale, torch.float32, 'scale')
     bp = bag_prob.contiguous()
-    if loss_kind == 0:
-        check(lib.ptb_mil_loss_bwd(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps), _ptr(bp),
-                                   _ptr(scale), _ptr(grad), _stream()), 'ptb_mil_loss_bwd')
-    else:
-        check(lib.ptb_mil_loss_bwd_kind(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps), int(loss_kind),
-                                        _ptr(bp), _ptr(scale), _ptr(grad), _stream()), 'ptb_mil_loss_bwd_kind')
+    check(lib.ptb_mil_loss_bwd(_ptr(logits), G, Kt, num_classes, ld, ins_off, _ptr(weight), _ptr(labels), float(eps), int(loss_kind),
+                               _ptr(bp), _ptr(scale), _ptr(grad), _stream()), 'ptb_mil_loss_bwd')
     return grad
 
 
@@ -383,25 +370,19 @@ def allpos_fwd(bag_logits, num_classes, weight, labels, eps, loss_kind):
 def cpr_loss_bwd_map(bag_logits, weight, mil_mt, bag_prob, label_weight, labels, centers, img_ptr, offsets, map_shape, num_classes, ins_off,
                      stride, reach_px, eps, scale_mil=None, scale_gt=None, valid_center=None, logit_map=None, neg_mask=None, scale_neg=None,
                      loss_kind=0, scale_pos=None):
-    """ptb_cpr_loss_bwd_map: d loss / d logit map (B,H,W,ld), deterministic, every element written.  With loss_kind != 0 or scale_pos
-    (ptb_cpr_loss_bwd_map_kind): mil_mt None drops the MIL term, scale_pos adds the per-sample positive term of AllPosLoss."""
+    """ptb_cpr_loss_bwd_map: d loss / d logit map (B,H,W,ld), deterministic, every element written.  mil_mt None drops the MIL term,
+    scale_pos adds the per-sample positive term of AllPosLoss."""
     lib = _lib.load()
     _chk(bag_logits, torch.float32, 'bag_logits'); _chk(weight, torch.float32, 'weight'); _chk(centers, torch.float32, 'centers')
     B, H, W, ld = map_shape
     G, K, _ = bag_logits.shape
     out = torch.empty((B, H, W, ld), dtype=torch.float32, device=bag_logits.device)
     ws = torch.empty(int(lib.ptb_cpr_loss_bwd_map_workspace(G, num_classes)) // 4, dtype=torch.float32, device=bag_logits.device)
-    if loss_kind == 0 and scale_pos is None and mil_mt is not None:
-        check(lib.ptb_cpr_loss_bwd_map(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
-                                       _ptr(centers), _ptr(img_ptr), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld, float(stride),
-                                       float(reach_px), float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), _ptr(logit_map),
-                                       _ptr(neg_mask), _ptr(scale_neg), _ptr(ws), _ptr(out), _stream()), 'ptb_cpr_loss_bwd_map')
-    else:
-        check(lib.ptb_cpr_loss_bwd_map_kind(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
-                                            _ptr(centers), _ptr(img_ptr), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld, float(stride),
-                                            float(reach_px), float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), _ptr(logit_map),
-                                            _ptr(neg_mask), _ptr(scale_neg), int(loss_kind), _ptr(scale_pos), _ptr(ws), _ptr(out), _stream()),
-              'ptb_cpr_loss_bwd_map_kind')
+    check(lib.ptb_cpr_loss_bwd_map(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
+                                   _ptr(centers), _ptr(img_ptr), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld, float(stride),
+                                   float(reach_px), float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), _ptr(logit_map),
+                                   _ptr(neg_mask), _ptr(scale_neg), int(loss_kind), _ptr(scale_pos), _ptr(ws), _ptr(out), _stream()),
+          'ptb_cpr_loss_bwd_map')
     return out
 
 
@@ -413,16 +394,10 @@ def cpr_loss_bwd_scatter(bag_logits, weight, mil_mt, bag_prob, label_weight, lab
     B, H, W, ld = grad_map.shape
     G, K, _ = bag_logits.shape
     ws = torch.empty(int(lib.ptb_cpr_loss_bwd_map_workspace(G, num_classes)) // 4, dtype=torch.float32, device=bag_logits.device)
-    if loss_kind == 0 and scale_pos is None and mil_mt is not None:
-        check(lib.ptb_cpr_loss_bwd_scatter(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
-                                           _ptr(centers), _ptr(bag_img), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld, float(stride),
-                                           float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), _ptr(ws), _ptr(grad_map),
-                                           _stream()), 'ptb_cpr_loss_bwd_scatter')
-    else:
-        check(lib.ptb_cpr_loss_bwd_scatter_kind(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
-                                                _ptr(centers), _ptr(bag_img), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld,
-                                                float(stride), float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), int(loss_kind),
-                                                _ptr(scale_pos), _ptr(ws), _ptr(grad_map), _stream()), 'ptb_cpr_loss_bwd_scatter_kind')
+    check(lib.ptb_cpr_loss_bwd_scatter(_ptr(bag_logits), _ptr(weight), _ptr(mil_mt), _ptr(bag_prob), _ptr(label_weight), _ptr(labels),
+                                       _ptr(centers), _ptr(bag_img), _ptr(offsets), B, H, W, G, K, num_classes, ins_off, ld, float(stride),
+                                       float(eps), _ptr(scale_mil), _ptr(scale_gt), _ptr(valid_center), int(loss_kind), _ptr(scale_pos),
+                                       _ptr(ws), _ptr(grad_map), _stream()), 'ptb_cpr_loss_bwd_scatter')
     return grad_map
 
 
@@ -438,18 +413,13 @@ def gfocal_fwd(logits, M, num_classes, row_stride, target_label, weight, eps, lo
 
 
 def gfocal_bwd(logits, M, num_classes, row_stride, target_label, weight, eps, scale, grad, grad_row_stride, accumulate, loss_kind=0):
-    """grad (+)= scale * weight * d term(sigmoid(logits), target) / d logits; term = gfocal (ptb_gfocal_sigmoid_bwd) or, with loss_kind 1,
-    binary cross-entropy (ptb_sigmoid_loss_bwd)."""
+    """ptb_sigmoid_loss_bwd: grad (+)= scale * weight * d term(sigmoid(logits), target) / d logits; term = gfocal or, with loss_kind 1,
+    binary cross-entropy."""
     lib = _lib.load()
     wmode = 0 if (weight is not None and weight.dtype == torch.uint8) else 1
-    if loss_kind == 0:
-        check(lib.ptb_gfocal_sigmoid_bwd(_ptr(logits), M, num_classes, row_stride, _ptr(target_label), _ptr(weight), wmode,
-                                         float(eps), _ptr(scale), _ptr(grad), grad_row_stride, 1 if accumulate else 0, _stream()),
-              'ptb_gfocal_sigmoid_bwd')
-    else:
-        check(lib.ptb_sigmoid_loss_bwd(_ptr(logits), M, num_classes, row_stride, _ptr(target_label), _ptr(weight), wmode, float(eps),
-                                       int(loss_kind), _ptr(scale), _ptr(grad), grad_row_stride, 1 if accumulate else 0, _stream()),
-              'ptb_sigmoid_loss_bwd')
+    check(lib.ptb_sigmoid_loss_bwd(_ptr(logits), M, num_classes, row_stride, _ptr(target_label), _ptr(weight), wmode, float(eps),
+                                   int(loss_kind), _ptr(scale), _ptr(grad), grad_row_stride, 1 if accumulate else 0, _stream()),
+          'ptb_sigmoid_loss_bwd')
     return grad
 
 

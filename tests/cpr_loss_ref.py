@@ -1,6 +1,6 @@
 """float64 reference of the fused CPR training loss as a function of the [cls | ins] logit map (test infrastructure, CPU).
 
-The loss kernels (ptb_cpr_bag_mil_fwd, ptb_mil_loss_fwd, ptb_gfocal_sigmoid_fwd/bwd, ptb_cpr_loss_bwd_map, ptb_cpr_loss_bwd_scatter) see
+The loss kernels (ptb_cpr_bag_mil_fwd, ptb_mil_loss_fwd, ptb_gfocal_sigmoid_fwd, ptb_sigmoid_loss_bwd, ptb_cpr_loss_bwd_map, ptb_cpr_loss_bwd_scatter) see
 the head only through its logit map lmap (B,H,W,LD): class logits in columns [0, N), instance logits in [NP, NP+N), padding elsewhere.
 This module restates what they compute from that map:
 

@@ -31,14 +31,14 @@ def test_header_is_plain_c(tmp_path):
     assert r.returncode == 0, r.stderr
 
 
-def test_library_exports_every_declared_symbol(lib_path):
+def test_library_exports_every_declared_symbol_at_abi_version_2(lib_path):
     syms = declared_symbols()
     assert len(syms) >= 25
     lib = ctypes.CDLL(lib_path)
     missing = [s for s in syms if not hasattr(lib, s)]
     assert not missing, missing
     lib.ptb_abi_version.restype = ctypes.c_int
-    assert lib.ptb_abi_version() == 1
+    assert lib.ptb_abi_version() == 2
 
 
 def test_ctypes_binding_covers_the_header(lib_path):

@@ -4,7 +4,7 @@ and bag sizes the head dispatches on (cpr_head.loss_bwd_plan):
   tiles    ptb_cpr_bag_mil_fwd -> ptb_cpr_loss_bwd_map              NP = ceil16(N): LD = 32 .. 160, K = 1 .. 320
   scatter  ptb_cpr_bag_mil_fwd -> ptb_cpr_loss_bwd_scatter          NP = ceil8(N), N <= 128, K up to 361
            ptb_cpr_bag_gather + ptb_mil_loss_fwd -> scatter          N = 129 .. 256
-  staged   ptb_mil_loss_bwd + ptb_gfocal_sigmoid_bwd + ptb_cpr_bag_gather_bwd
+  staged   ptb_mil_loss_bwd + ptb_sigmoid_loss_bwd + ptb_cpr_bag_gather_bwd
 
 Every case runs on 3 images of 13 x 21 cells (not a multiple of the 8 x 8 tile), one of them without GTs, with centres outside the padded
 image (label weight 0), exactly at (0, 0) and at the pad edge, and a duplicated centre; the pad columns of the logit map hold 50.
