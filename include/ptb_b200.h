@@ -315,6 +315,21 @@ int ptb_multiclass_soft_nms(const float* pts /*[B][P][2] or NULL*/, const float*
                             void* workspace, uint64_t workspace_bytes, void* stream);
 uint64_t ptb_multiclass_soft_nms_workspace(int B, int P, int num_classes);
 
+/* class-specific boxes [B][P][C][4] (x1,y1,x2,y2): candidate (p, c) uses boxes[b][p][c] - the RoI head's multiclass_nms with
+ * bboxes (n, 4*C).  Everything else as ptb_multiclass_nms_boxes / ptb_multiclass_soft_nms with boxes: the candidate list, the
+ * `keep` ranks (box-major, class-minor), max_coord over the candidates' own boxes, the `slow` test over every candidate box and
+ * the exact global path below 10000 candidates, the per-class kernels and the merge from 10000 on.  Limits as there: P <= 4096
+ * boxes per image, max_per_img in [1, 1024]; the workspaces are ptb_multiclass_nms_workspace(B, P, C) and
+ * ptb_multiclass_soft_nms_workspace(B, P, C).  Gaussian soft-NMS refuses an image on its candidates' own boxes. */
+int ptb_multiclass_nms_cls_boxes(const float* boxes /*[B][P][C][4]*/, const float* scores /*[B][P][C]*/, int B, int P, int num_classes,
+                                 float score_thr, float iou_thr, int max_per_img,
+                                 int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count,
+                                 void* workspace, uint64_t workspace_bytes, void* stream);
+int ptb_multiclass_soft_nms_cls_boxes(const float* boxes /*[B][P][C][4]*/, const float* scores /*[B][P][C]*/, int B, int P,
+                                      int num_classes, float score_thr, float iou_thr, float sigma, float min_score, int method,
+                                      int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep,
+                                      int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Hungarian cost matrix — replaces FocalLossCost + DisCostV2 (mmdet/core/bbox/match_costs/match_cost.py:94-99,
  * 197-214) as summed by HungarianAssignerV2.assign (hungarian_assigner.py:222-227).

@@ -68,6 +68,9 @@ SIGNATURES = {
                                         P, P, P, P, P, P, c_u64, P]),
     'ptb_multiclass_soft_nms_workspace': (c_u64, [c_int, c_int, c_int]),
     'ptb_multiclass_nms_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_int, P, P, P, P, P, P, c_u64, P]),
+    'ptb_multiclass_nms_cls_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_int, P, P, P, P, P, P, c_u64, P]),
+    'ptb_multiclass_soft_nms_cls_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, c_int,
+                                                  P, P, P, P, P, P, c_u64, P]),
     'ptb_p2p_cost_matrix': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, c_float, c_float, c_float, c_float, c_float,
                                     c_float, c_float, P, P]),
     'ptb_p2p_cost_matrix_terms': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, P, c_int, c_float, c_float, P, P, c_u64, P]),

@@ -20,6 +20,9 @@ constexpr int NMS_T0 = 1024;
 // mmcv batched_nms's default split_thr: from this many candidates on it runs NMS class by class and sorts the kept entries by
 // score, so the classes never interact whatever the offset does - the per-class kernels and the merge are that branch exactly
 constexpr int NMS_SPLIT_THR = 10000;
+// The 1024-thread kernels are templates over the box layout (cs = 1: class-specific boxes).  Their cs = 1 forms state one CTA per
+// SM, which lets ptxas use the full 64 registers per thread instead of spilling; the shared-box forms keep their plain bounds.
+#define NMS_T0_BOUNDS(cs) __launch_bounds__(NMS_T0, (cs) ? 1 : 0)
 
 struct NmsImg {       // per-image header in the workspace
   float max_coord;
@@ -47,7 +50,8 @@ __device__ __forceinline__ bool iou_gt(const Box& a, const Box& b, float thr) {
   return ovr > thr;
 }
 
-// un-offset box of point / proposal p: either given explicitly (boxes [P][4]) or the pseudo box pts[p] -/+ (hw, hh)
+// un-offset box of point / proposal p: either given explicitly (row p of the image's boxes, see box_row) or the pseudo box
+// pts[p] -/+ (hw, hh)
 struct RawBox {
   float x1, y1, x2, y2;
 };
@@ -61,6 +65,12 @@ __device__ __forceinline__ RawBox raw_box(const float* __restrict__ pp, const fl
   }
   return r;
 }
+// image b's boxes: [P][4] shared by the classes, or [P][C][4] with one box per (point, class) (cs = 1, class-specific boxes);
+// candidate (p, c) uses row box_row(p, c) of them
+__device__ __forceinline__ const float* img_boxes(const float* boxes, int b, int P, int C, int cs) {
+  return boxes ? boxes + (size_t)b * P * (cs ? C : 1) * 4 : nullptr;
+}
+__device__ __forceinline__ int box_row(int p, int c, int C, int cs) { return cs ? p * C + c : p; }
 __device__ __forceinline__ Box offset_box(const RawBox& r, float off) {
   Box b;   // + label*(max_coord+1) on every coordinate (mmcv batched_nms)
   b.x1 = __fadd_rn(r.x1, off); b.y1 = __fadd_rn(r.y1, off); b.x2 = __fadd_rn(r.x2, off); b.y2 = __fadd_rn(r.y2, off);
@@ -68,7 +78,8 @@ __device__ __forceinline__ Box offset_box(const RawBox& r, float off) {
   return b;
 }
 
-__global__ void __launch_bounds__(NMS_T0)
+template <int cs>
+__global__ void NMS_T0_BOUNDS(cs)
 nms_prepare_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                    float score_thr, NmsImg* __restrict__ hdr, int32_t* __restrict__ base /*[B][P]*/,
                    int32_t* __restrict__ out_cand_count) {
@@ -79,17 +90,25 @@ nms_prepare_kernel(const float* __restrict__ pts, const float* __restrict__ boxe
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const float* sc = scores + (size_t)b * P * C;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   float mx = -CUDART_INF_F;
   float ax = CUDART_INF_F, ay = CUDART_INF_F;   // min x1 / y1 over candidate boxes in the negative corner zone
   // warp per point: count classes over threshold
   for (int p = wid; p < P; p += NMS_T0 / 32) {
     int cnt = 0;
-    for (int c = lane; c < C; c += 32) cnt += sc[(size_t)p * C + c] > score_thr;
+    for (int c = lane; c < C; c += 32) {
+      const bool is = sc[(size_t)p * C + c] > score_thr;
+      cnt += is;
+      if (cs && is) {  // class-specific boxes: every candidate brings its own box
+        const RawBox rb = raw_box(pp, bx, box_row(p, c, C, cs), hw, hh);
+        mx = fmaxf(mx, fmaxf(fmaxf(rb.x1, rb.y1), fmaxf(rb.x2, rb.y2)));
+        if (rb.x1 < -0.95f && rb.y1 < -0.95f) { ax = fminf(ax, rb.x1); ay = fminf(ay, rb.y1); }
+      }
+    }
     cnt = (int)warp_sum((float)cnt);
     if (lane == 0) {
       s_cnt[p] = cnt;
-      if (cnt > 0) {   // boxes.max() over the candidate boxes = max over (x2, y2)
+      if (!cs && cnt > 0) {   // boxes.max() over the candidate boxes = max over (x2, y2)
         const RawBox rb = raw_box(pp, bx, p, hw, hh);
         mx = fmaxf(mx, fmaxf(fmaxf(rb.x1, rb.y1), fmaxf(rb.x2, rb.y2)));
         if (rb.x1 < -0.95f && rb.y1 < -0.95f) { ax = fminf(ax, rb.x1); ay = fminf(ay, rb.y1); }
@@ -112,10 +131,21 @@ nms_prepare_kernel(const float* __restrict__ pts, const float* __restrict__ boxe
     for (int w = 1; w < NMS_T0 / 32; ++w) { m = fmaxf(m, s_max[w]); mnx = fminf(mnx, s_ax[w]); mny = fminf(mny, s_ay[w]); }
     if (mnx < CUDART_INF_F) {
       const float m1 = m + 1.f;
-      for (int p = threadIdx.x; p < P; p += NMS_T0) {
-        if (s_cnt[p] <= 0) continue;
-        const RawBox rb = raw_box(pp, bx, p, hw, hh);
-        if (rb.x2 > mnx + m1 - 0.05f && rb.y2 > mny + m1 - 0.05f) s_slow = 1;
+      if (!cs) {
+        for (int p = threadIdx.x; p < P; p += NMS_T0) {
+          if (s_cnt[p] <= 0) continue;
+          const RawBox rb = raw_box(pp, bx, p, hw, hh);
+          if (rb.x2 > mnx + m1 - 0.05f && rb.y2 > mny + m1 - 0.05f) s_slow = 1;
+        }
+      } else {         // the same test over every candidate's own box, warp per point
+        for (int p = wid; p < P; p += NMS_T0 / 32) {
+          if (s_cnt[p] <= 0) continue;
+          for (int c = lane; c < C; c += 32) {
+            if (!(sc[(size_t)p * C + c] > score_thr)) continue;
+            const RawBox rb = raw_box(pp, bx, box_row(p, c, C, cs), hw, hh);
+            if (rb.x2 > mnx + m1 - 0.05f && rb.y2 > mny + m1 - 0.05f) s_slow = 1;
+          }
+        }
       }
     }
   }
@@ -171,6 +201,7 @@ __device__ __forceinline__ void bitonic_sort_u64_blk(unsigned long long* a, int 
 constexpr int NMS_T1 = 256;
 
 // per (image, class): list[b][c][0..n) = kept point indices in descending score order (n <= max_keep)
+template <int cs>
 __global__ void __launch_bounds__(NMS_T1)
 nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                  float score_thr, float iou_thr, int max_keep, const NmsImg* __restrict__ hdr,
@@ -184,7 +215,7 @@ nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const float* sc = scores + (size_t)b * P * C + c;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   if (threadIdx.x == 0) s_n = 0;
   __syncthreads();
   // ---- compact candidates of this class (order irrelevant: sorted next)
@@ -215,7 +246,7 @@ nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
       const int i = base0 + lane;
       const bool have = i < n;
       const int p = have ? (int)(keys[i] & 0xFFFFFFFFull) : 0;
-      const Box me = offset_box(raw_box(pp, bx, p, hw, hh), off);
+      const Box me = offset_box(raw_box(pp, bx, box_row(p, c, C, cs), hw, hh), off);
       bool alive = have;
       for (int t = 0; t < nk && alive; ++t) {
         Box kb;
@@ -250,6 +281,7 @@ nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
 }
 
 // one warp per image: merge
+template <int cs>
 __global__ void __launch_bounds__(32)
 nms_merge_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                  float score_thr, int max_keep, const NmsImg* __restrict__ hdr, const int32_t* __restrict__ base,
@@ -267,7 +299,7 @@ nms_merge_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
   __syncwarp();
   const float* sc = scores + (size_t)b * P * C;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   int r = 0;
   for (; r < max_keep; ++r) {
     unsigned long long best = 0xFFFFFFFFFFFFFFFFull;   // (~score bits, flat id) : smaller is better
@@ -292,7 +324,7 @@ nms_merge_kernel(const float* __restrict__ pts, const float* __restrict__ boxes,
       const float sv = cls_score ? cls_score[((size_t)b * C + c) * max_keep + head[c]] : sc[(size_t)p * C + c];
       head[c] += 1;
       float* d = out_det + ((size_t)b * max_keep + r) * 5;
-      const RawBox rb = raw_box(pp, bx, p, hw, hh);
+      const RawBox rb = raw_box(pp, bx, box_row(p, c, C, cs), hw, hh);
       d[0] = rb.x1; d[1] = rb.y1; d[2] = rb.x2; d[3] = rb.y2;
       d[4] = sv;
       out_label[(size_t)b * max_keep + r] = c;
@@ -328,6 +360,7 @@ __device__ __forceinline__ float soft_weight(float ovr, float iou_thr, float sig
 }
 
 
+template <int cs>
 __global__ void __launch_bounds__(SNMS_T)
 soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C,
                       float hw, float hh, float score_thr, float iou_thr, float sigma, float min_score, int method, int max_keep,
@@ -345,7 +378,7 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
   if (hdr[b].slow) return;
   const float* sc = scores + (size_t)b * P * C + c;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   const float off = __fmul_rn((float)c, __fadd_rn(hdr[b].max_coord, 1.f));
   // ---- ordered compaction of this class's candidates
   int n = 0;
@@ -360,7 +393,7 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
     for (int w = 0; w < SNMS_T / 32; ++w) { if (w < wid) before += s_wcnt[w]; total += s_wcnt[w]; }
     if (is) {
       const int slot = n + before + __popc(bal & ((1u << lane) - 1u));
-      const Box me = offset_box(raw_box(pp, bx, p, hw, hh), off);
+      const Box me = offset_box(raw_box(pp, bx, box_row(p, c, C, cs), hw, hh), off);
       bx1[slot] = me.x1; by1[slot] = me.y1; bx2[slot] = me.x2; by2[slot] = me.y2; bar[slot] = me.area;
       bsc[slot] = s; bidx[slot] = p; alive[slot] = 1;
     }
@@ -423,7 +456,8 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
 
 // soft-NMS over ALL candidates of a flagged image (class offsets applied, classes may interact): state[e] = current score of
 // candidate (p, c) = e / C, e % C, or -1 when dead / selected / not a candidate.  One CTA per flagged image.
-__global__ void __launch_bounds__(NMS_T0)
+template <int cs>
+__global__ void NMS_T0_BOUNDS(cs)
 soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C,
                        float hw, float hh, float score_thr, float iou_thr, float sigma, float min_score, int method, int max_keep,
                        const NmsImg* __restrict__ hdr, const int32_t* __restrict__ base, float* __restrict__ state /*[B][P*C]*/,
@@ -436,7 +470,7 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const float* sc = scores + (size_t)b * P * C;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   float* st = state + (size_t)b * P * C;
   const float m1 = __fadd_rn(hdr[b].max_coord, 1.f);
   const int N = P * C;
@@ -448,7 +482,7 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
     st[e] = sc[e] > score_thr ? sc[e] : -1.f;
     if (method == 2 && sc[e] > score_thr) {
       const int p = e / C, c = e - p * C;
-      deg += degenerate_weight(offset_box(raw_box(pp, bx, p, hw, hh), __fmul_rn((float)c, m1)).area);
+      deg += degenerate_weight(offset_box(raw_box(pp, bx, box_row(p, c, C, cs), hw, hh), __fmul_rn((float)c, m1)).area);
     }
   }
   if (deg) atomicAdd(&s_deg, deg);
@@ -484,7 +518,7 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
     if (best == 0xFFFFFFFFFFFFFFFFull) break;
     const int e0 = (int)(best & 0xFFFFFFFFull);
     const int p0 = e0 / C, c0 = e0 - p0 * C;
-    const RawBox rb0 = raw_box(pp, bx, p0, hw, hh);
+    const RawBox rb0 = raw_box(pp, bx, box_row(p0, c0, C, cs), hw, hh);
     const Box b0 = offset_box(rb0, __fmul_rn((float)c0, m1));
     if (threadIdx.x == 0) {
       float* d = out_det + ((size_t)b * max_keep + nk) * 5;
@@ -502,7 +536,7 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
       if (e == e0) { st[e] = -1.f; continue; }
       if (v < 0.f) continue;
       const int p = e / C, c = e - p * C;
-      const Box me = offset_box(raw_box(pp, bx, p, hw, hh), __fmul_rn((float)c, m1));
+      const Box me = offset_box(raw_box(pp, bx, box_row(p, c, C, cs), hw, hh), __fmul_rn((float)c, m1));
       const float w = fmaxf(0.f, __fsub_rn(fminf(b0.x2, me.x2), fmaxf(b0.x1, me.x1)));
       const float h = fmaxf(0.f, __fsub_rn(fminf(b0.y2, me.y2), fmaxf(b0.y1, me.y1)));
       const float inter = __fmul_rn(w, h);
@@ -520,7 +554,8 @@ soft_nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ 
 // walks the candidates in descending (score, flat id) order - one block-wide arg-min per examined candidate - and
 // tests each against the <= max_keep kept boxes of ALL classes on the offset coordinates, i.e. the reference's
 // batched_nms literally, stopping at max_keep.
-__global__ void __launch_bounds__(NMS_T0)
+template <int cs>
+__global__ void NMS_T0_BOUNDS(cs)
 nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                   float score_thr, float iou_thr, int max_keep, const NmsImg* __restrict__ hdr,
                   const int32_t* __restrict__ base, int32_t* __restrict__ out_count, float* __restrict__ out_det,
@@ -533,7 +568,7 @@ nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ boxes
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const float* sc = scores + (size_t)b * P * C;
   const float* pp = pts ? pts + (size_t)b * P * 2 : nullptr;
-  const float* bx = boxes ? boxes + (size_t)b * P * 4 : nullptr;
+  const float* bx = img_boxes(boxes, b, P, C, cs);
   const float m1 = __fadd_rn(hdr[b].max_coord, 1.f);
   const int N = P * C;
   unsigned long long prev = 0ull;
@@ -567,7 +602,7 @@ nms_global_kernel(const float* __restrict__ pts, const float* __restrict__ boxes
     first = false;
     const int flat = (int)(best & 0xFFFFFFFFull);
     const int p = flat / C, c = flat - p * C;
-    const RawBox rb = raw_box(pp, bx, p, hw, hh);
+    const RawBox rb = raw_box(pp, bx, box_row(p, c, C, cs), hw, hh);
     const Box me = offset_box(rb, __fmul_rn((float)c, m1));
     int sup = 0;
     for (int t = threadIdx.x; t < nk; t += NMS_T0) {
@@ -605,6 +640,11 @@ extern "C" uint64_t ptb_multiclass_nms_workspace(int B, int P, int num_classes) 
   return nms_hdr_bytes(B) + ((uint64_t)B * P + (uint64_t)B * num_classes + (uint64_t)B * num_classes * 1024) * 4;
 }
 
+// class-specific boxes index row p * C + c of a [P][C][4] image: keep 4 * P * C within int
+#define NMS_REQUIRE_CS_ROWS(cs, P, C) \
+  PTB_REQUIRE(!(cs) || (uint64_t)(P) * (uint64_t)(C) * 4 <= 0x7fffffffull, "class-specific boxes: 4 * P * num_classes must fit in int")
+
+template <int cs>
 static int nms_run(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes, float pseudo_w,
                    float pseudo_h, float score_thr, float iou_thr, int max_per_img, int32_t* out_count, float* out_det,
                    int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
@@ -615,6 +655,7 @@ static int nms_run(const float* pts, const float* boxes, const float* scores, in
   PTB_REQUIRE(iou_thr >= 0.f, "iou_thr must be >= 0 (per-class decomposition)");
   PTB_REQUIRE((pts || boxes) && scores && out_count && out_det && out_label && out_keep && out_cand_count, "NULL input");
   PTB_REQUIRE(workspace && workspace_bytes >= ptb_multiclass_nms_workspace(B, P, num_classes), "workspace too small");
+  NMS_REQUIRE_CS_ROWS(cs, P, num_classes);
   NmsImg* hdr = reinterpret_cast<NmsImg*>(workspace);
   int32_t* base = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(workspace) + nms_hdr_bytes(B));
   int32_t* cls_cnt = base + (size_t)B * P;
@@ -622,21 +663,21 @@ static int nms_run(const float* pts, const float* boxes, const float* scores, in
   const float hw = pseudo_w * 0.5f, hh = pseudo_h * 0.5f;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  nms_prepare_kernel<<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
+  nms_prepare_kernel<cs><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
   if ((rc = check_launch("ptb_multiclass_nms/prepare"))) return rc;
   // keys (32 KB static) + kept list (dynamic) can exceed the 48 KB default; the attribute is per device -> set on every call
-  if (cudaFuncSetAttribute(nms_class_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess ||
-      cudaFuncSetAttribute(nms_global_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess)
+  if (cudaFuncSetAttribute(nms_class_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess ||
+      cudaFuncSetAttribute(nms_global_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess)
     return fail("%s", "ptb_multiclass_nms: shared memory opt-in failed");
   dim3 g1(num_classes, B);
-  nms_class_kernel<<<g1, NMS_T1, (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
+  nms_class_kernel<cs><<<g1, NMS_T1, (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
                                                                               iou_thr, max_per_img, hdr, cls_cnt, cls_list);
   if ((rc = check_launch("ptb_multiclass_nms/class"))) return rc;
-  nms_merge_kernel<<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
+  nms_merge_kernel<cs><<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
                                                                    hdr, base, cls_cnt, cls_list, out_count, out_det, out_label,
                                                                    out_keep, nullptr);
   if ((rc = check_launch("ptb_multiclass_nms/merge"))) return rc;
-  nms_global_kernel<<<B, NMS_T0, (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
+  nms_global_kernel<cs><<<B, NMS_T0, (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
                                                                                 iou_thr, max_per_img, hdr, base, out_count,
                                                                                 out_det, out_label, out_keep);
   return check_launch("ptb_multiclass_nms/global");
@@ -647,7 +688,7 @@ extern "C" int ptb_multiclass_nms(const float* pts, const float* scores, int B, 
                                   float* out_det, int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count,
                                   void* workspace, uint64_t workspace_bytes, void* stream) {
   PTB_REQUIRE(pts, "NULL pts");
-  return nms_run(pts, nullptr, scores, B, P, num_classes, pseudo_w, pseudo_h, score_thr, iou_thr, max_per_img, out_count, out_det,
+  return nms_run<0>(pts, nullptr, scores, B, P, num_classes, pseudo_w, pseudo_h, score_thr, iou_thr, max_per_img, out_count, out_det,
                  out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
 }
 
@@ -656,7 +697,16 @@ extern "C" int ptb_multiclass_nms_boxes(const float* boxes, const float* scores,
                                         int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
                                         void* stream) {
   PTB_REQUIRE(boxes, "NULL boxes");
-  return nms_run(nullptr, boxes, scores, B, P, num_classes, 0.f, 0.f, score_thr, iou_thr, max_per_img, out_count, out_det,
+  return nms_run<0>(nullptr, boxes, scores, B, P, num_classes, 0.f, 0.f, score_thr, iou_thr, max_per_img, out_count, out_det,
+                 out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ptb_multiclass_nms_cls_boxes(const float* boxes, const float* scores, int B, int P, int num_classes, float score_thr,
+                                            float iou_thr, int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label,
+                                            int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
+                                            void* stream) {
+  PTB_REQUIRE(boxes, "NULL boxes");
+  return nms_run<1>(nullptr, boxes, scores, B, P, num_classes, 0.f, 0.f, score_thr, iou_thr, max_per_img, out_count, out_det,
                  out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
 }
 
@@ -666,11 +716,11 @@ extern "C" uint64_t ptb_multiclass_soft_nms_workspace(int B, int P, int num_clas
          ((uint64_t)B * P + (uint64_t)B * num_classes + 2 * (uint64_t)B * num_classes * 1024 + (uint64_t)B * P * num_classes) * 4;
 }
 
-extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes,
-                                       float pseudo_w, float pseudo_h, float score_thr, float iou_thr, float sigma, float min_score,
-                                       int method, int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label,
-                                       int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
-                                       void* stream) {
+template <int cs>
+static int soft_nms_run(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes,
+                        float pseudo_w, float pseudo_h, float score_thr, float iou_thr, float sigma, float min_score, int method,
+                        int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep,
+                        int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes, void* stream) {
   PTB_REQUIRE(B > 0 && P > 0 && num_classes > 0, "shape");
   PTB_REQUIRE(P <= NMS_MAXP, "more than 4096 points per image not supported");
   PTB_REQUIRE(max_per_img > 0 && max_per_img <= 1024, "max_per_img must be in [1,1024]");
@@ -681,6 +731,7 @@ extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, con
   PTB_REQUIRE((pts != nullptr) != (boxes != nullptr), "give either pts (pseudo boxes) or boxes");
   PTB_REQUIRE(scores && out_count && out_det && out_label && out_keep && out_cand_count, "NULL input");
   PTB_REQUIRE(workspace && workspace_bytes >= ptb_multiclass_soft_nms_workspace(B, P, num_classes), "workspace too small");
+  NMS_REQUIRE_CS_ROWS(cs, P, num_classes);
   NmsImg* hdr = reinterpret_cast<NmsImg*>(workspace);
   int32_t* base = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(workspace) + nms_hdr_bytes(B));
   int32_t* cls_cnt = base + (size_t)B * P;
@@ -690,22 +741,41 @@ extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, con
   const float hw = pseudo_w * 0.5f, hh = pseudo_h * 0.5f;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  nms_prepare_kernel<<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
+  nms_prepare_kernel<cs><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
   if ((rc = check_launch("ptb_multiclass_soft_nms/prepare"))) return rc;
   const size_t smem = (size_t)P * (7 * sizeof(float) + 1) + 16;
   // the kernel's own 104 B of static shared memory count against the 48 KB default too (P = 1691..1694 have smem <= 48 KB but fail
   // to launch without the opt-in): set the per-device attribute on every call (a process may drive several devices)
-  if (cudaFuncSetAttribute(soft_nms_class_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+  if (cudaFuncSetAttribute(soft_nms_class_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return fail("%s", "ptb_multiclass_soft_nms: shared memory opt-in failed");
   dim3 g1(num_classes, B);
-  soft_nms_class_kernel<<<g1, SNMS_T, smem, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
+  soft_nms_class_kernel<cs><<<g1, SNMS_T, smem, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
                                                 max_per_img, hdr, cls_cnt, cls_list, cls_score);
   if ((rc = check_launch("ptb_multiclass_soft_nms/class"))) return rc;
-  nms_merge_kernel<<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
+  nms_merge_kernel<cs><<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
                                                                    hdr, base, cls_cnt, cls_list, out_count, out_det, out_label,
                                                                    out_keep, cls_score);
   if ((rc = check_launch("ptb_multiclass_soft_nms/merge"))) return rc;
-  soft_nms_global_kernel<<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
+  soft_nms_global_kernel<cs><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
                                              max_per_img, hdr, base, state, out_count, out_det, out_label, out_keep);
   return check_launch("ptb_multiclass_soft_nms/global");
+}
+
+extern "C" int ptb_multiclass_soft_nms(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes,
+                                       float pseudo_w, float pseudo_h, float score_thr, float iou_thr, float sigma, float min_score,
+                                       int method, int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label,
+                                       int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
+                                       void* stream) {
+  return soft_nms_run<0>(pts, boxes, scores, B, P, num_classes, pseudo_w, pseudo_h, score_thr, iou_thr, sigma, min_score, method,
+                      max_per_img, out_count, out_det, out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ptb_multiclass_soft_nms_cls_boxes(const float* boxes, const float* scores, int B, int P, int num_classes,
+                                                 float score_thr, float iou_thr, float sigma, float min_score, int method,
+                                                 int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label,
+                                                 int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
+                                                 void* stream) {
+  PTB_REQUIRE(boxes, "NULL boxes");
+  return soft_nms_run<1>(nullptr, boxes, scores, B, P, num_classes, 0.f, 0.f, score_thr, iou_thr, sigma, min_score, method,
+                      max_per_img, out_count, out_det, out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
 }

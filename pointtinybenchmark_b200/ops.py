@@ -489,11 +489,23 @@ def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img):
     return cnt, det, lab, keep, cc
 
 
+def _cls_boxes(boxes, scores):
+    """True for class-specific boxes (B,P,C,4), False for boxes shared by the classes (B,P,4)."""
+    if boxes.dim() == 3:
+        return False
+    if tuple(boxes.shape) != tuple(scores.shape) + (4,):
+        raise ValueError(f'class-specific boxes must be (B, P, C, 4) = {tuple(scores.shape) + (4,)}, got {tuple(boxes.shape)}')
+    return True
+
+
 def multiclass_nms_boxes(boxes, scores, score_thr, iou_thr, max_per_img):
-    """ptb_multiclass_nms_boxes. boxes (B,P,4) xyxy, scores (B,P,C) -> count, det (B,max,5), label, keep, cand_count."""
+    """ptb_multiclass_nms_boxes: boxes (B,P,4) xyxy shared by the classes, or ptb_multiclass_nms_cls_boxes: class-specific boxes
+    (B,P,C,4), candidate (p, c) using boxes[b, p, c];  scores (B,P,C) -> count, det (B,max,5), label, keep, cand_count."""
     lib = _lib.load()
     _chk(boxes, torch.float32, 'boxes'); _chk(scores, torch.float32, 'scores')
     B, P, C = scores.shape
+    fn, name = ((lib.ptb_multiclass_nms_cls_boxes, 'ptb_multiclass_nms_cls_boxes') if _cls_boxes(boxes, scores)
+                else (lib.ptb_multiclass_nms_boxes, 'ptb_multiclass_nms_boxes'))
     dev = boxes.device
     cnt = torch.empty((B,), dtype=torch.int32, device=dev)
     det = torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=dev)
@@ -502,9 +514,8 @@ def multiclass_nms_boxes(boxes, scores, score_thr, iou_thr, max_per_img):
     cc = torch.empty((B,), dtype=torch.int32, device=dev)
     nbytes = lib.ptb_multiclass_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    check(lib.ptb_multiclass_nms_boxes(_ptr(boxes), _ptr(scores), B, P, C, float(score_thr), float(iou_thr), int(max_per_img),
-                                       _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes, _stream()),
-          'ptb_multiclass_nms_boxes')
+    check(fn(_ptr(boxes), _ptr(scores), B, P, C, float(score_thr), float(iou_thr), int(max_per_img),
+             _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes, _stream()), name)
     return cnt, det, lab, keep, cc
 
 
@@ -513,6 +524,7 @@ SOFT_NMS_METHODS = {'naive': 0, 'linear': 1, 'gaussian': 2}
 
 def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max_per_img, sigma=0.5, min_score=1e-3, method='linear'):
     """ptb_multiclass_soft_nms.  pts_or_boxes: (B,P,2) points (pseudo boxes of pseudo_wh) or (B,P,4) boxes; scores (B,P,C).
+    Class-specific boxes (B,P,C,4) go to ptb_multiclass_soft_nms_cls_boxes.
     returns count (B,), det (B,max,5) with DECAYED scores, label, keep, cand_count."""
     lib = _lib.load()
     _chk(pts_or_boxes, torch.float32, 'pts_or_boxes'); _chk(scores, torch.float32, 'scores')
@@ -520,6 +532,7 @@ def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max
         raise KeyError(method)
     B, P, C = scores.shape
     dev = scores.device
+    cls_boxes = pts_or_boxes.dim() == 4 and _cls_boxes(pts_or_boxes, scores)
     is_boxes = pts_or_boxes.shape[-1] == 4
     cnt = torch.empty((B,), dtype=torch.int32, device=dev)
     det = torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=dev)
@@ -528,15 +541,22 @@ def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max
     cc = torch.empty((B,), dtype=torch.int32, device=dev)
     nbytes = lib.ptb_multiclass_soft_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    wh = pseudo_wh if pseudo_wh is not None else (0.0, 0.0)
-    check(lib.ptb_multiclass_soft_nms(None if is_boxes else _ptr(pts_or_boxes), _ptr(pts_or_boxes) if is_boxes else None, _ptr(scores),
-                                      B, P, C, float(wh[0]), float(wh[1]), float(score_thr), float(iou_thr), float(sigma),
-                                      float(min_score), SOFT_NMS_METHODS[method], int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab),
-                                      _ptr(keep), _ptr(cc), _ptr(ws), nbytes, _stream()), 'ptb_multiclass_soft_nms')
+    outs = (SOFT_NMS_METHODS[method], int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes,
+            _stream())
+    if cls_boxes:
+        name = 'ptb_multiclass_soft_nms_cls_boxes'
+        check(lib.ptb_multiclass_soft_nms_cls_boxes(_ptr(pts_or_boxes), _ptr(scores), B, P, C, float(score_thr), float(iou_thr),
+                                                    float(sigma), float(min_score), *outs), name)
+    else:
+        name = 'ptb_multiclass_soft_nms'
+        wh = pseudo_wh if pseudo_wh is not None else (0.0, 0.0)
+        check(lib.ptb_multiclass_soft_nms(None if is_boxes else _ptr(pts_or_boxes), _ptr(pts_or_boxes) if is_boxes else None,
+                                          _ptr(scores), B, P, C, float(wh[0]), float(wh[1]), float(score_thr), float(iou_thr),
+                                          float(sigma), float(min_score), *outs), name)
     if method == 'gaussian':              # refused images (count -1): one device read, gaussian only
         bad = torch.nonzero(cnt < 0).flatten().tolist()
         if bad:
-            raise RuntimeError(f'ptb_multiclass_soft_nms: gaussian soft-NMS refused image(s) {bad}: two candidate boxes of zero area '
+            raise RuntimeError(f'{name}: gaussian soft-NMS refused image(s) {bad}: two candidate boxes of zero area '
                                '(or one of negative area) give IoU 0/0 = NaN weights')
     return cnt, det, lab, keep, cc
 
