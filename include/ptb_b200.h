@@ -163,7 +163,8 @@ int ptb_cpr_refine_fused(const float* logit_map /*[B][H][W][ld]*/, int B, int H,
  *   out_bag_prob[g][c] = sum_k sigmoid(cls) * normalize_L1(softmax_k(ins) * weight)
  *       (the buffer must hold G*num_classes + 3*G floats: the trailing 3*G are per-bag loss / weight / hit scratch)
  *   out_loss_sum[0]   += sum_g term(bag_prob[g], onehot(labels[g])) * (any_k weight>0)      (un-normalised; term below)
- *   out_stats[0] += #bags with any weight>0 ; out_stats[1] += #bags whose argmax == label
+ *   out_stats[0] += #bags with any weight>0 ; out_stats[1] += #bags whose argmax (first maximum) == label
+ * num_classes <= 1280; above 256 the classes are processed in chunks of 256 lanes, each per-(bag, class) sum in the same order.
  * bwd: d(loss_sum)/d(cls logits), d/d(ins logits) scaled by `scale` (= loss_weight / num_sample).
  * loss_kind selects the loss term of the positive bags (MILLoss / AllPosLoss `loss_type`, multi_instance_learning_loss.py:187-202, 229-240):
  *   PTB_LOSS_GFOCAL  gfocal_loss(p, onehot) x label weight (the bag's any-weight flag for MIL, w_k for AllPos)
@@ -586,6 +587,11 @@ uint64_t ptb_conv_tc_wgrad_workspace(int B, int H, int W, int taps);
 int ptb_conv_tc_wgrad_f16x2(const void* dy_h, const void* dy_l /*[B][H][W][Cout] fp16*/, const void* x_h, const void* x_l /*[B][H][W][256] fp16*/,
                             int B, int H, int W, int Cout, int Cin, int taps, float scale, const float* dev_scale_dy,
                             const float* dev_scale_x, void* workspace, float* dw, int accumulate, void* stream);
+/* the same with dy rows ld_dy fp16 apart (ld_dy >= Cout, a multiple of 8; dy 16-byte aligned): one column slice [c0, c0 + Cout) of a wider
+ * fp16 pair (dy + c0), e.g. the logit map's gradient of more than 256 columns, without a copy.  dw [Cout][256] as above. */
+int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H, int W,
+                               int Cout, int Cin, int taps, float scale, const float* dev_scale_dy, const float* dev_scale_x,
+                               void* workspace, float* dw, int accumulate, void* stream);
 
 /* column sums of a row-major fp32 matrix: out[n] = sum_m y[m][n] (bias gradient of the logit-map Linear); fixed-order, deterministic */
 uint64_t ptb_col_sum_workspace(int64_t M, int N);

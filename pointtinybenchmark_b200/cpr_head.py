@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc, _packed_tc_cols
 from .registry import register_head
 
 _SUPPORTED_POS = ('CirclePtFeatGenerator', 'GridCirclesPtFeatGenerator')
@@ -105,9 +105,20 @@ class _GridCircleBags:
 
 def _loss_gemm_on_tc(C, LD):
     """the two GEMMs of the loss that are plain 1x1 convolutions (logit map forward, its input gradient) run on the wgmma kernel
-    when the channel counts fit it (Cin % 32 == 0, N <= 256); PTB_LOSS_GEMM=ffma keeps the fp32 FFMA kernels."""
+    when the channel counts fit it (Cin % 32 == 0, LD <= 256); PTB_LOSS_GEMM=ffma keeps the fp32 FFMA kernels."""
     import os
     return os.environ.get('PTB_LOSS_GEMM', 'tc') == 'tc' and C % 32 == 0 and LD % 32 == 0 and C <= 256 and LD <= 256
+
+
+def _loss_map_sliced_on_tc(N, C):
+    """above 256 classes the training logit map runs as column slices of the wgmma kernel (ops.conv_tc_f16_cols); with 256 input
+    channels its two backward GEMMs run on the tensor cores too (dW in column slices, dX as one conv with Cin = LD).  Up to 256 classes
+    the choice is _loss_gemm_on_tc's."""
+    import os
+    return os.environ.get('PTB_LOSS_GEMM', 'tc') == 'tc' and N > 256 and C % 32 == 0
+
+
+MAX_CLASSES = 1280     # the loss kernels' class limit (ptb_cpr_loss_bwd_scatter: 4 classes x 320 lanes, ptb_mil_loss_fwd / _bwd)
 
 
 class _BagGatherFn(torch.autograd.Function):
@@ -136,14 +147,15 @@ def loss_bwd_plan(N, K, circle_bags, with_mil_loss, env_mode=None, deterministic
     env_mode is PTB_LOSS_BWD (None when unset); deterministic is torch.are_deterministic_algorithms_enabled().  Returns
     (NP, path, reason):
       NP      ins column offset of the logit map, LD = 2 * NP.  ceil8(N) by default; ceil16(N) when bit-reproducible gradients are
-              asked for, so that LD is a multiple of 32 (the tile kernel's channel groups) for every N.
+              asked for, so that LD is a multiple of 32 (the tile kernel's channel groups) for every N, and above 256 classes, so that
+              the tensor-core input gradient (a conv with Cin = LD, Cin % 32 == 0) takes the map.
       path    'tiles'   ptb_cpr_loss_bwd_map: deterministic, ring bags with the MIL loss, LD <= 160 (N <= 80), K <= 320
               'scatter' ptb_cpr_loss_bwd_scatter: fp32 atomics, ring bags with the MIL loss (the default)
               'staged'  mil_loss_bwd + gfocal_bwd + bag_gather_bwd / grid_bag_bwd: fp32 atomics, every configuration
       reason  None, or why bit-reproducible gradients were asked for (PTB_LOSS_BWD=tiles or deterministic mode) but cannot be
               given; `path` is then the atomic path that would run instead.  The caller raises, or warns in warn-only mode."""
     want_tiles = env_mode == 'tiles' or (env_mode is None and deterministic)
-    NP = (N + 15) // 16 * 16 if want_tiles else (N + 7) // 8 * 8
+    NP = (N + 15) // 16 * 16 if (want_tiles or N > 256) else (N + 7) // 8 * 8
     LD = 2 * NP
     circle = circle_bags and with_mil_loss
     fallback = 'scatter' if circle and env_mode in (None, 'scatter', 'tiles') else 'staged'
@@ -189,9 +201,14 @@ class _CPRLossFn(torch.autograd.Function):
         wcat[:N], wcat[NP:NP + N], bcat[:N], bcat[NP:NP + N] = w_cls, w_ins, b_cls, b_ins
         x2d = fmap.reshape(M, C)
         use_tc = _loss_gemm_on_tc(C, LD)
+        sliced = not use_tc and _loss_map_sliced_on_tc(N, C)
         if use_tc:       # logit map on the tensor cores: 1-tap conv of the fp16 operand pair (fp32-accurate two-term split)
             fh, fl, finv = ops.split_f16(fmap, auto_scale=True)
             lmap = ops.conv_tc_f16(fh, fl, ops.conv_tc_pack_weight_f16(wcat, 1), 1, LD, bias=bcat, dev_out_scale=finv, ldy=LD).view(M, LD)
+        elif sliced:
+            fh, fl, finv = ops.split_f16(fmap, auto_scale=True)
+            lmap = ops.conv_tc_f16_cols(fh, fl, ops.conv_tc_pack_weight_f16_cols(wcat, 1), 1, LD, bias=bcat, dev_out_scale=finv,
+                                        ldy=LD).view(M, LD)
         else:
             lmap = ops.linear_rows(x2d, wcat, bcat)                              # (M, LD) fp32 FFMA GEMM
         allpos, kind = hp['allpos'], hp['loss_kind']
@@ -248,7 +265,7 @@ class _CPRLossFn(torch.autograd.Function):
             saved['neg_mask'] = nm
         ctx.hp, ctx.gt, ctx.bags, ctx.aux, ctx.saved = hp, gt, bags, aux, saved
         ctx.num_pos = num_pos
-        ctx.fpair = (fh, fl, finv) if use_tc else None        # fp16 operand pair of the feature map: the wgrad's second operand
+        ctx.fpair = (fh, fl, finv) if (use_tc or sliced) else None    # fp16 operand pair of the feature map: the wgrad's second operand
         ctx.save_for_backward(fmap, wcat, lmap, bl, weight)
         return gt_loss, pos_loss, neg_loss, bag_acc
 
@@ -331,7 +348,15 @@ class _CPRLossFn(torch.autograd.Function):
             dlmap = _CPRLossFn._bwd_map_staged(ctx, g_gt, g_pos, g_neg, bl, weight, lmap, B, H, W, N, NP, LD, M, G, K)
         d2 = dlmap.view(M, LD)
         x2d = fmap.reshape(M, C)
-        if _loss_gemm_on_tc(C, LD) and ctx.fpair is not None and C == 256 and LD % 8 == 0:
+        if ctx.fpair is not None and C == 256 and LD > 256 and LD % 32 == 0:
+            # above 256 classes: dW in column slices of <= 256 of the gradient's fp16 pair (the wgrad's widest output), read in place;
+            # dX as one conv with Cin = LD (loss_bwd_plan pads LD to a multiple of 32 here)
+            dh, dl_, dinv = ops.split_f16(dlmap.view(B, H, W, LD), auto_scale=True)
+            fh, fl, finv = ctx.fpair
+            dw = ops.conv_tc_wgrad_f16_cols(dh, dl_, fh, fl, 1.0, dinv, finv)
+            db = ops.col_sum(d2)
+            dx = ops.conv_tc_f16(dh, dl_, ops.conv_tc_pack_weight_f16(wcat.t().contiguous(), 1), 1, C, dev_out_scale=dinv, ldy=C)
+        elif _loss_gemm_on_tc(C, LD) and ctx.fpair is not None and C == 256 and LD % 8 == 0:
             # both GEMMs of the Linear's backward on the tensor cores (fp16 two-term split, fp32-accurate, deterministic):
             #   dW = dL^T @ X  : K = pixels, MN-major operands (the tower's wgrad kernel with one tap)
             #   dX = dL @ W    : 1-tap conv with W^T (Cin = LD)
@@ -613,7 +638,11 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 if self.debug and self.last_overflow_flag is not None and int(self.last_overflow_flag) != 0:    # host sync: debug only
                     raise FloatingPointError('CPRHead: a GroupNorm output exceeded the fp16 operand range (|x| > 6e4) and was clamped')
                 h, l = pair
-                lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1, 'lin'), 1, self.num_classes, bias=self.cls_out.bias.detach())
+                bias = self.cls_out.bias.detach()
+                if self.num_classes <= ops.CONV_TC_N_MAX:
+                    lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1, 'lin'), 1, self.num_classes, bias=bias)
+                else:            # wider than one wgmma launch: column slices of the same kernel into one map
+                    lmap = ops.conv_tc_f16_cols(h, l, _packed_tc_cols(self.cls_out), 1, self.num_classes, bias=bias)
                 return self._get_bboxes_from_logit_map(lmap, img_metas, rescale=rescale, **kwargs)
         outs = self.forward(feats)
         return self.get_bboxes(*outs, img_metas, rescale=rescale, **kwargs)
@@ -625,6 +654,8 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         feat = cls_feat[0]
         if not feat.is_cuda:
             raise RuntimeError('CPRHead runs on CUDA tensors only; there is no CPU fallback')
+        if self.num_classes > MAX_CLASSES:
+            raise RuntimeError(f'CPRHead.loss: num_classes={self.num_classes} exceeds the {MAX_CLASSES} classes the CUDA loss kernels take')
         gt = _BatchGT(gt_bboxes, gt_labels, img_metas, feat.device)
         pos, neg = self.train_pts_extractor['pos_generator'], self.train_pts_extractor['neg_generator']
         hp = dict(num_classes=self.num_classes, stride=float(self.strides[0]), eps=float(self.loss_mil_cfg.get('eps', 1e-6)),

@@ -2,7 +2,9 @@
 // elementwise loss (:148-151) used for gt_loss / neg_loss (cpr_head.py:1159-1184, 1219-1228) — forward + backward.
 //
 // MIL: one CTA per bag; threads = (class lane, sample slice).  Logit rows are [cls(0..C) | ins(ins_off..ins_off+C)],
-// so for a fixed sample the class lanes read contiguous floats (coalesced).  Per class:
+// so for a fixed sample the class lanes read contiguous floats (coalesced).  Above MIL_MAXCP classes the CTA walks the classes in
+// chunks of MIL_MAXCP lanes; every per-(bag, class) sum has the same order whatever the chunk, and the bag's loss sum and top-1
+// class are merged over the chunks in class order (first maximum wins).  Per class:
 //   m = max_k ins;  e_k = exp(ins_k - m);  Z = sum e;  T = sum e*w;  N = sum sigmoid(cls_k)*e*w
 //   prob = (N/Z) / max(T/Z, 1e-12)                       (softmax over the bag, x valid, F.normalize(p=1), weighted sum)
 // Reductions use fixed-order trees: results are deterministic run to run.
@@ -13,7 +15,8 @@
 namespace ptb {
 
 constexpr int MIL_KS = 4;         // sample slices per bag
-constexpr int MIL_MAXCP = 256;    // padded class lanes supported per pass
+constexpr int MIL_MAXCP = 256;    // class lanes per chunk
+constexpr int MIL_MAX_CLASSES = 1280;   // the class count of ptb_cpr_loss_bwd_scatter (4 x 320 lanes), the head's limit
 
 // the bag loss term of the positive bags: GfocalTerm x label weight, or BceTerm unweighted (cpr_loss_term.cuh)
 template <class Loss>
@@ -28,18 +31,18 @@ struct MilShared {
   float c[MIL_KS][MIL_MAXCP];
 };
 
-// computes per class: m (max ins), Z, T, N for bag g.  cls lane `cl` < C valid. returns via refs (all slices get the totals)
+// computes per class: m (max ins), Z, T, N for bag g at class column `cl` (valid when act) on shared lane `ln`; all slices get the totals
 __device__ __forceinline__ void mil_stats(const float* __restrict__ row0, int Kt, int ld, int ins_off, const float* __restrict__ wrow,
-                                          int cl, int ks, bool act, MilShared& sh, float& m, float& Z, float& T, float& N) {
+                                          int cl, int ln, int ks, bool act, MilShared& sh, float& m, float& Z, float& T, float& N) {
   // pass 1: max
   float mx = -CUDART_INF_F;
   if (act)
     for (int k = ks; k < Kt; k += MIL_KS) mx = fmaxf(mx, row0[(size_t)k * ld + ins_off + cl]);
-  sh.a[ks][cl] = mx;
+  sh.a[ks][ln] = mx;
   __syncthreads();
-  mx = sh.a[0][cl];
+  mx = sh.a[0][ln];
 #pragma unroll
-  for (int s = 1; s < MIL_KS; ++s) mx = fmaxf(mx, sh.a[s][cl]);
+  for (int s = 1; s < MIL_KS; ++s) mx = fmaxf(mx, sh.a[s][ln]);
   __syncthreads();
   // pass 2: sums
   float z = 0.f, t = 0.f, n = 0.f;
@@ -52,11 +55,11 @@ __device__ __forceinline__ void mil_stats(const float* __restrict__ row0, int Kt
       t += e * w;
       n += sg * (e * w);
     }
-  sh.a[ks][cl] = z; sh.b[ks][cl] = t; sh.c[ks][cl] = n;
+  sh.a[ks][ln] = z; sh.b[ks][ln] = t; sh.c[ks][ln] = n;
   __syncthreads();
   z = t = n = 0.f;
 #pragma unroll
-  for (int s = 0; s < MIL_KS; ++s) { z += sh.a[s][cl]; t += sh.b[s][cl]; n += sh.c[s][cl]; }
+  for (int s = 0; s < MIL_KS; ++s) { z += sh.a[s][ln]; t += sh.b[s][ln]; n += sh.c[s][ln]; }
   __syncthreads();
   m = mx; Z = z; T = t; N = n;
 }
@@ -71,12 +74,9 @@ mil_fwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
   __shared__ int s_arg[MIL_MAXCP / 32];
   __shared__ float s_argv[MIL_MAXCP / 32];
   const int g = blockIdx.x;
-  const int cl = threadIdx.x % CP, ks = threadIdx.x / CP;
-  const bool act = cl < C;
+  const int ln = threadIdx.x % CP, ks = threadIdx.x / CP;     // CP lanes per chunk (a multiple of 32, at most MIL_MAXCP)
   const float* row0 = logits + (size_t)g * Kt * ld;
   const float* wrow = weight + (size_t)g * Kt;
-  float m, Z, T, N;
-  mil_stats(row0, Kt, ld, ins_off, wrow, cl, ks, act, sh, m, Z, T, N);
   // label weight: any sample weight > 0  (valid.sum(dim=1) > 0, multi_instance_learning_loss.py:174)
   float wsum = 0.f;
   for (int k = threadIdx.x; k < Kt; k += blockDim.x) wsum += wrow[k];
@@ -88,40 +88,48 @@ mil_fwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
   for (int i = 0; i < (int)(blockDim.x >> 5); ++i) wtot += sh.a[0][i];
   __syncthreads();
   const float lw = wtot > 0.f ? 1.f : 0.f;
-  if (ks != 0) return;   // slice 0 finishes the bag (no further __syncthreads below involve other slices)
-  float prob = 0.f, lossc = 0.f;
   const int l = labels[g];
-  if (act) {
-    const float tn = T / Z;                                   // sum_k softmax*w  (>=0)
-    prob = (N / Z) / fmaxf(tn, 1e-12f);                       // F.normalize(p=1, eps=1e-12)
-    bag_prob[(size_t)g * C + cl] = prob;
-    if (out_mt) {
-      out_mt[((size_t)g * C + cl) * 2] = m;
-      out_mt[((size_t)g * C + cl) * 2 + 1] = (tn >= 1e-12f) ? 1.f / T : 0.f;       // mil_bwd's `degenerate` test
-    }
-    lossc = bag_term(term, prob, cl == l ? 1.f : 0.f, lw);
-  }
-  // reduce over class lanes of slice 0 (threads 0..CP-1; CP is a multiple of 32)
-  float ls = warp_sum(lossc);
-  float bv = act ? prob : -CUDART_INF_F;
-  int bi = act ? cl : 0x7fffffff;
+  float tot = 0.f, best = -CUDART_INF_F;                      // thread 0: bag loss and top-1 class, merged over the chunks in class order
+  int besti = 0x7fffffff;
+  for (int c0 = 0; c0 < C; c0 += CP) {
+    const int cl = c0 + ln;
+    const bool act = cl < C;
+    float m, Z, T, N;
+    mil_stats(row0, Kt, ld, ins_off, wrow, cl, ln, ks, act, sh, m, Z, T, N);
+    if (ks == 0) {                                            // slice 0 finishes the chunk's classes
+      float prob = 0.f, lossc = 0.f;
+      if (act) {
+        const float tn = T / Z;                               // sum_k softmax*w  (>=0)
+        prob = (N / Z) / fmaxf(tn, 1e-12f);                   // F.normalize(p=1, eps=1e-12)
+        bag_prob[(size_t)g * C + cl] = prob;
+        if (out_mt) {
+          out_mt[((size_t)g * C + cl) * 2] = m;
+          out_mt[((size_t)g * C + cl) * 2 + 1] = (tn >= 1e-12f) ? 1.f / T : 0.f;   // mil_bwd's `degenerate` test
+        }
+        lossc = bag_term(term, prob, cl == l ? 1.f : 0.f, lw);
+      }
+      // reduce over the class lanes of slice 0 (threads 0..CP-1)
+      const float ls = warp_sum(lossc);
+      float bv = act ? prob : -CUDART_INF_F;
+      int bi = act ? cl : 0x7fffffff;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-  }
-  const int wid = threadIdx.x >> 5, nw = CP >> 5;
-  if ((threadIdx.x & 31) == 0) { s_red[wid] = ls; s_arg[wid] = bi; s_argv[wid] = bv; }
-  // only slice-0 warps participate: named barrier over CP threads
-  asm volatile("bar.sync 1, %0;" ::"r"(CP));
-  if (threadIdx.x == 0) {
-    float tot = 0.f, best = -CUDART_INF_F;
-    int besti = 0x7fffffff;
-    for (int i = 0; i < nw; ++i) {
-      tot += s_red[i];
-      if (s_argv[i] > best || (s_argv[i] == best && s_arg[i] < besti)) { best = s_argv[i]; besti = s_arg[i]; }
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+      }
+      const int wid = threadIdx.x >> 5;
+      if ((threadIdx.x & 31) == 0) { s_red[wid] = ls; s_arg[wid] = bi; s_argv[wid] = bv; }
     }
+    __syncthreads();
+    // thread 0 reads s_red before its next mil_stats, whose barriers come before slice 0 writes s_red again
+    if (threadIdx.x == 0)
+      for (int i = 0; i < (CP >> 5); ++i) {
+        tot += s_red[i];
+        if (s_argv[i] > best || (s_argv[i] == best && s_arg[i] < besti)) { best = s_argv[i]; besti = s_arg[i]; }
+      }
+  }
+  if (threadIdx.x == 0) {
     aux[g] = tot;                       // bag loss (gfocal: already x label weight)
     aux[(size_t)G + g] = lw;            // bag counted in num_sample
     aux[(size_t)2 * G + g] = (besti == l) ? 1.f : 0.f;   // top-1 hit (accuracy(), losses/accuracy.py)
@@ -135,13 +143,10 @@ mil_bwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
                const float* __restrict__ scale, float* __restrict__ grad) {
   __shared__ MilShared sh;
   const int g = blockIdx.x;
-  const int cl = threadIdx.x % CP, ks = threadIdx.x / CP;
-  const bool act = cl < C;
+  const int ln = threadIdx.x % CP, ks = threadIdx.x / CP;
   const float* row0 = logits + (size_t)g * Kt * ld;
   const float* wrow = weight + (size_t)g * Kt;
   float* grow = grad + (size_t)g * Kt * ld;
-  float m, Z, T, N;
-  mil_stats(row0, Kt, ld, ins_off, wrow, cl, ks, act, sh, m, Z, T, N);
   float wsum = 0.f;
   for (int k = threadIdx.x; k < Kt; k += blockDim.x) wsum += wrow[k];
   wsum = warp_sum(wsum);
@@ -149,18 +154,26 @@ mil_bwd_kernel(const float* __restrict__ logits, int Kt, int C, int CP, int ld, 
   __syncthreads();
   float wtot = 0.f;
   for (int i = 0; i < (int)(blockDim.x >> 5); ++i) wtot += sh.a[0][i];
+  __syncthreads();
   const float lw = wtot > 0.f ? 1.f : 0.f;
-  if (!act) return;
-  const float p = bag_prob[(size_t)g * C + cl];
-  const float q = (cl == labels[g]) ? 1.f : 0.f;
-  const float gp = Loss::label_weighted ? scale[0] * lw * term.dp(p, q) : scale[0] * term.dp(p, q);     // dLoss/dprob
-  const bool degenerate = !(T / Z >= 1e-12f);                 // normalisation clamp active (all weights ~0): prob const
-  for (int k = ks; k < Kt; k += MIL_KS) {
-    const float e = expf(row0[(size_t)k * ld + ins_off + cl] - m);
-    const float pi = degenerate ? 0.f : (e * wrow[k]) / T;    // normalised instance weight
-    const float sg = sigmoidf_acc(row0[(size_t)k * ld + cl]);
-    grow[(size_t)k * ld + cl] = gp * pi * sg * (1.f - sg);
-    grow[(size_t)k * ld + ins_off + cl] = gp * pi * (sg - p);
+  const int l = labels[g];
+  for (int c0 = 0; c0 < C; c0 += CP) {
+    const int cl = c0 + ln;
+    const bool act = cl < C;
+    float m, Z, T, N;
+    mil_stats(row0, Kt, ld, ins_off, wrow, cl, ln, ks, act, sh, m, Z, T, N);
+    if (!act) continue;
+    const float p = bag_prob[(size_t)g * C + cl];
+    const float q = (cl == l) ? 1.f : 0.f;
+    const float gp = Loss::label_weighted ? scale[0] * lw * term.dp(p, q) : scale[0] * term.dp(p, q);     // dLoss/dprob
+    const bool degenerate = !(T / Z >= 1e-12f);               // normalisation clamp active (all weights ~0): prob const
+    for (int k = ks; k < Kt; k += MIL_KS) {
+      const float e = expf(row0[(size_t)k * ld + ins_off + cl] - m);
+      const float pi = degenerate ? 0.f : (e * wrow[k]) / T;  // normalised instance weight
+      const float sg = sigmoidf_acc(row0[(size_t)k * ld + cl]);
+      grow[(size_t)k * ld + cl] = gp * pi * sg * (1.f - sg);
+      grow[(size_t)k * ld + ins_off + cl] = gp * pi * (sg - p);
+    }
   }
 }
 
@@ -440,7 +453,8 @@ gfocal_bwd_kernel(const float* __restrict__ logits, long long M, int C, long lon
 
 using namespace ptb;
 
-static int mil_cp(int C) { return ((C + 31) / 32) * 32; }
+// class lanes per chunk: C rounded up to a warp, at most MIL_MAXCP (one chunk, as before, up to 256 classes)
+static int mil_cp(int C) { return C < MIL_MAXCP ? ((C + 31) / 32) * 32 : MIL_MAXCP; }
 
 // runs f(term) with the loss-term functor of `kind` (LOSS_GFOCAL | LOSS_BCE); the caller has validated kind
 template <class F>
@@ -453,7 +467,7 @@ extern "C" int ptb_mil_loss_fwd(const float* logits, int G, int Kt, int num_clas
                                 const int32_t* labels, float eps, int loss_kind, float* out_bag_prob, float* out_loss_sum,
                                 float* out_stats, float* out_mt, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
-  PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
+  PTB_REQUIRE(num_classes <= MIL_MAX_CLASSES, "num_classes > 1280 not supported");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
   PTB_REQUIRE(logits && weight && labels && out_bag_prob && out_loss_sum && out_stats, "NULL input");
@@ -475,7 +489,7 @@ extern "C" int ptb_mil_loss_bwd(const float* logits, int G, int Kt, int num_clas
                                 const int32_t* labels, float eps, int loss_kind, const float* bag_prob, const float* scale,
                                 float* grad_logits, void* stream) {
   PTB_REQUIRE(G >= 0 && Kt > 0 && num_classes > 0 && ld >= ins_off + num_classes && ins_off >= 0, "shape");
-  PTB_REQUIRE(num_classes <= MIL_MAXCP, "num_classes > 256 not supported");
+  PTB_REQUIRE(num_classes <= MIL_MAX_CLASSES, "num_classes > 1280 not supported");
   PTB_REQUIRE(loss_kind == LOSS_GFOCAL || loss_kind == LOSS_BCE, "loss_kind");
   if (G == 0) return 0;
   PTB_REQUIRE(logits && weight && labels && bag_prob && scale && grad_logits, "NULL input");

@@ -218,11 +218,12 @@ __global__ void __launch_bounds__(256) colsum_reduce_kernel(const float* __restr
   out[n] = s;
 }
 
-static int make_px_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, int C) {
+// C channels of pixel rows `ld` fp16 apart (ld = C: dense); channels past C read as zeros (TMA out-of-bounds fill)
+static int make_px_map(CUtensorMap* tm, const void* ptr, int B, int H, int W, int C, int ld) {
   EncodeTiledFn enc = tc_get_encode();
   if (!enc) return fail("%s", "cuTensorMapEncodeTiled is unavailable (driver too old?)");
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)H * W * ld * 2};
   cuuint32_t box[4] = {64, WG_TW, WG_TH, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
@@ -262,15 +263,15 @@ static uint64_t wgrad_ws_bytes(int B, int H, int W, int taps) {
 extern "C" uint64_t ptb_conv3x3_wgrad_workspace(int B, int H, int W) { return wgrad_ws_bytes(B, H, W, 9); }
 extern "C" uint64_t ptb_conv_tc_wgrad_workspace(int B, int H, int W, int taps) { return wgrad_ws_bytes(B, H, W, taps); }
 
-static int wgrad_run(const void* dy_h, const void* dy_l, const void* x_h, const void* x_l, int B, int H, int W, int Cout, int Cin, int taps,
-                     float scale, const float* dev_scale_dy, const float* dev_scale_x, void* workspace, float* dw, int accumulate,
+static int wgrad_run(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H, int W, int Cout, int Cin,
+                     int taps, float scale, const float* dev_scale_dy, const float* dev_scale_x, void* workspace, float* dw, int accumulate,
                      void* stream, const char* what) {
   CUtensorMap tm_dyh, tm_dyl, tm_xh, tm_xl;
   int rc;
-  if ((rc = make_px_map(&tm_dyh, dy_h, B, H, W, Cout))) return rc;
-  if ((rc = make_px_map(&tm_dyl, dy_l, B, H, W, Cout))) return rc;
-  if ((rc = make_px_map(&tm_xh, x_h, B, H, W, Cin))) return rc;
-  if ((rc = make_px_map(&tm_xl, x_l, B, H, W, Cin))) return rc;
+  if ((rc = make_px_map(&tm_dyh, dy_h, B, H, W, Cout, ld_dy))) return rc;
+  if ((rc = make_px_map(&tm_dyl, dy_l, B, H, W, Cout, ld_dy))) return rc;
+  if ((rc = make_px_map(&tm_xh, x_h, B, H, W, Cin, Cin))) return rc;
+  if ((rc = make_px_map(&tm_xl, x_l, B, H, W, Cin, Cin))) return rc;
   WgradShape ws;
   ws.B = B; ws.H = H; ws.W = W;
   ws.tiles_h = (H + WG_TH - 1) / WG_TH;
@@ -300,7 +301,7 @@ extern "C" int ptb_conv3x3_wgrad_f16x2(const void* dy_h, const void* dy_l, const
   PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
   PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
                   ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
-  return wgrad_run(dy_h, dy_l, x_h, x_l, B, H, W, Cout, Cin, 9, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
+  return wgrad_run(dy_h, dy_l, Cout, x_h, x_l, B, H, W, Cout, Cin, 9, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
                    "ptb_conv3x3_wgrad_f16x2");
 }
 
@@ -312,8 +313,21 @@ extern "C" int ptb_conv_tc_wgrad_f16x2(const void* dy_h, const void* dy_l, const
   PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
   PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
                   ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
-  return wgrad_run(dy_h, dy_l, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
+  return wgrad_run(dy_h, dy_l, Cout, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
                    "ptb_conv_tc_wgrad_f16x2");
+}
+
+extern "C" int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H,
+                                          int W, int Cout, int Cin, int taps, float scale, const float* dev_scale_dy,
+                                          const float* dev_scale_x, void* workspace, float* dw, int accumulate, void* stream) {
+  PTB_REQUIRE(B > 0 && H > 0 && W > 0 && (taps == 1 || taps == 9), "shape");
+  PTB_REQUIRE(Cin == WG_C && Cout > 0 && Cout <= WG_C && Cout % 8 == 0, "Cin must be 256, Cout a multiple of 8 up to 256");
+  PTB_REQUIRE(ld_dy >= Cout && ld_dy % 8 == 0, "ld_dy must be a multiple of 8 and >= Cout");
+  PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
+  PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
+                  ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
+  return wgrad_run(dy_h, dy_l, ld_dy, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
+                   "ptb_conv_tc_wgrad_f16x2_ld");
 }
 
 extern "C" uint64_t ptb_col_sum_workspace(int64_t M, int N) {

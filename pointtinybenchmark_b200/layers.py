@@ -56,7 +56,7 @@ def bias_init_with_prob(p):
     return float(-math.log((1 - p) / p))
 
 
-_PACK_ATTRS = ('_ptb_packed_f16', '_ptb_packed_f16_t', '_ptb_packed', '_ptb_packed_tc')
+_PACK_ATTRS = ('_ptb_packed_f16', '_ptb_packed_f16_t', '_ptb_packed', '_ptb_packed_tc', '_ptb_packed_tc_cols')
 
 
 def invalidate_packed(module):
@@ -176,6 +176,17 @@ def _packed_tc(module, taps, tag):
         w2 = w.detach().reshape(w.shape[0], w.shape[1], -1) if w.dim() == 4 else w.detach()
         module._ptb_packed_tc = (key, ops.conv_tc_pack_weight_f16(w2.contiguous(), taps))
     return module._ptb_packed_tc[1]
+
+
+def _packed_tc_cols(module):
+    """column-slice packing (ops.conv_tc_pack_weight_f16_cols) of a Linear weight wider than one wgmma launch, cached per version."""
+    from . import ops
+    w = module.weight
+    key = (w.data_ptr(), w._version, str(w.device))
+    cache = getattr(module, '_ptb_packed_tc_cols', None)
+    if cache is None or cache[0] != key:
+        module._ptb_packed_tc_cols = (key, ops.conv_tc_pack_weight_f16_cols(w.detach().contiguous(), 1))
+    return module._ptb_packed_tc_cols[1]
 
 
 def tc_enabled(x, *modules):

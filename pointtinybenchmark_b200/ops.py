@@ -1005,6 +1005,24 @@ def conv_tc_wgrad_f16(dy_h, dy_l, x_h, x_l, taps, scale=1.0, dev_scale_dy=None, 
     return dw
 
 
+def conv_tc_wgrad_f16_cols(dy_h, dy_l, x_h, x_l, scale=1.0, dev_scale_dy=None, dev_scale_x=None, width=256):
+    """dW (Cout, 256) of a per-cell Linear whose output gradient dy (B,H,W,Cout) is wider than one tensor-core wgrad (Cout <= 256): one
+    ptb_conv_tc_wgrad_f16x2_ld launch per column slice [c0, c0 + width) of the fp16 pair, read in place (row stride Cout), writing rows
+    [c0, c0 + n) of dW.  Cout a multiple of 8."""
+    lib = _lib.load()
+    _chk(dy_h, torch.float16, 'dy_h'); _chk(dy_l, torch.float16, 'dy_l'); _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
+    B, H, W, Cout = dy_h.shape
+    Cin = x_h.shape[3]
+    ws = torch.empty(int(lib.ptb_conv_tc_wgrad_workspace(B, H, W, 1)), dtype=torch.uint8, device=dy_h.device)
+    dw = torch.empty((Cout, Cin), dtype=torch.float32, device=dy_h.device)
+    for c0 in range(0, Cout, width):
+        n = min(width, Cout - c0)
+        check(lib.ptb_conv_tc_wgrad_f16x2_ld(_ptr(dy_h[..., c0:]), _ptr(dy_l[..., c0:]), Cout, _ptr(x_h), _ptr(x_l), B, H, W, n, Cin, 1,
+                                             float(scale), _ptr(dev_scale_dy), _ptr(dev_scale_x), _ptr(ws), _ptr(dw[c0:]), 0, _stream()),
+              'ptb_conv_tc_wgrad_f16x2_ld')
+    return dw
+
+
 def col_sum(y2d):
     """ptb_col_sum: out[n] = sum_m y[m][n] of a contiguous fp32 (M, N) matrix, fixed order."""
     lib = _lib.load()
@@ -1029,6 +1047,38 @@ def conv_tc_pack_weight_f16(w, taps):
     check(lib.ptb_conv_tc_pack_weight_f16(_ptr(w), n_out, n_mma, Cin, taps, float(scale), _ptr(h), _ptr(l), _stream()),
           'ptb_conv_tc_pack_weight_f16')
     return h, l, 1.0 / scale, n_mma
+
+
+CONV_TC_N_MAX = 512       # widest output of one ptb_conv_tc_f16x2 launch
+
+
+def conv_tc_pack_weight_f16_cols(w, taps, width=CONV_TC_N_MAX):
+    """column slices [c0, c0 + width) of a weight wider than one wgmma launch, each packed by conv_tc_pack_weight_f16 (its own scale):
+    [(c0, n, packed), ...] for conv_tc_f16_cols."""
+    return [(c0, min(width, w.shape[0] - c0), conv_tc_pack_weight_f16(w[c0:c0 + width], taps)) for c0 in range(0, w.shape[0], width)]
+
+
+def conv_tc_f16_cols(x_h, x_l, packs, taps, n_out, bias=None, dev_out_scale=None, ldy=None):
+    """conv_tc_f16 at any n_out: one wgmma launch per column slice of conv_tc_pack_weight_f16_cols, each writing columns
+    [c0, c0 + n) of one (B,H,W,ldy) fp32 map (+bias).  x_l None: x_h is used as is (ptb_conv_tc_f16x1a)."""
+    lib = _lib.load()
+    _chk(x_h, torch.float16, 'x_h')
+    if x_l is not None:
+        _chk(x_l, torch.float16, 'x_l')
+    B, H, W, Cin = x_h.shape
+    ldy = ldy or (n_out + 3) // 4 * 4
+    y = torch.empty((B, H, W, ldy), dtype=torch.float32, device=x_h.device)
+    if packs[-1][0] + packs[-1][1] != n_out:
+        raise ValueError(f'conv_tc_f16_cols: the packed slices cover {packs[-1][0] + packs[-1][1]} columns, not n_out = {n_out}')
+    for c0, n, (w_h, w_l, inv_w, n_mma) in packs:
+        yc, bc = y[..., c0:], (bias[c0:c0 + n] if bias is not None else None)
+        if x_l is None:
+            check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w), _ptr(dev_out_scale),
+                                         _ptr(bc), _ptr(yc), ldy, None, _stream()), 'ptb_conv_tc_f16x1a')
+        else:
+            check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w),
+                                        _ptr(dev_out_scale), _ptr(bc), _ptr(yc), ldy, _stream()), 'ptb_conv_tc_f16x2')
+    return y
 
 
 HALF_DTYPES = {torch.float16: 1, torch.bfloat16: 2}      # PTB_DTYPE_F16, PTB_DTYPE_BF16
