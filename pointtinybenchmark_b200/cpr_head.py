@@ -642,7 +642,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 if self.num_classes <= ops.CONV_TC_N_MAX:
                     lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1, 'lin'), 1, self.num_classes, bias=bias)
                 else:            # wider than one wgmma launch: column slices of the same kernel into one map
-                    lmap = ops.conv_tc_f16_cols(h, l, _packed_tc_cols(self.cls_out), 1, self.num_classes, bias=bias)
+                    lmap = ops.conv_tc_f16_cols(h, l, _packed_tc_cols(self.cls_out, 1), 1, self.num_classes, bias=bias)
                 return self._get_bboxes_from_logit_map(lmap, img_metas, rescale=rescale, **kwargs)
         outs = self.forward(feats)
         return self.get_bboxes(*outs, img_metas, rescale=rescale, **kwargs)

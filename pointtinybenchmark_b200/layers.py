@@ -178,15 +178,95 @@ def _packed_tc(module, taps, tag):
     return module._ptb_packed_tc[1]
 
 
-def _packed_tc_cols(module):
-    """column-slice packing (ops.conv_tc_pack_weight_f16_cols) of a Linear weight wider than one wgmma launch, cached per version."""
+def _packed_tc_cols(module, taps):
+    """column-slice packing (ops.conv_tc_pack_weight_f16_cols) of a Linear (taps 1) / conv3x3 (taps 9) weight wider than one wgmma
+    launch, cached per version."""
     from . import ops
     w = module.weight
-    key = (w.data_ptr(), w._version, str(w.device))
+    key = (w.data_ptr(), w._version, str(w.device), taps)
     cache = getattr(module, '_ptb_packed_tc_cols', None)
     if cache is None or cache[0] != key:
-        module._ptb_packed_tc_cols = (key, ops.conv_tc_pack_weight_f16_cols(w.detach().contiguous(), 1))
+        w2 = w.detach().reshape(w.shape[0], w.shape[1], -1) if w.dim() == 4 else w.detach()
+        module._ptb_packed_tc_cols = (key, ops.conv_tc_pack_weight_f16_cols(w2.contiguous(), taps))
     return module._ptb_packed_tc_cols[1]
+
+
+INT32_MAX = 2 ** 31 - 1
+TMA_STRIDE_LIMIT = 2 ** 40         # bytes: cuTensorMapEncodeTiled's bound on a global stride
+
+
+def wide_out_conv_plan(B, H, W, n_out, k=1, backward=False):
+    """Row stride ldy of the (B,H,W,ldy) fp32 map that a conv3x3 output layer wider than one wgmma launch (n_out > 512) writes, and the
+    refusal of shapes the kernels on that path cannot index.  A pure function of the shape (no device is touched).
+
+    ldy = ceil4(n_out) for a forward alone: the (B,H,W,n_out) view of the map is the whole map when n_out % 4 == 0, so the per-anchor
+    reshape downstream needs no copy.  ldy = ceil32(n_out) when a backward follows: the input gradient is one conv with Cin = ldy, and the
+    conv kernel takes Cin % 32 == 0 (the padded weight rows are zero).
+    Every kernel of the path indexes elements with 64-bit offsets (conv epilogue, ptb_split_f16*, ptb_col_sum, the loss and cost
+    kernels); what stays 32-bit is the proposal index of the decode and top-k (H * W * k per image, int32 indices), and the tensor maps
+    of the conv and wgrad operands (the fp16 pair of the (B,H,W,ldy) gradient) take per-image strides below 2^40 bytes.  Above either bound this raises ValueError."""
+    if min(B, H, W, n_out, k) <= 0:
+        raise ValueError(f'wide output conv: empty shape B={B} H={H} W={W} n_out={n_out} k={k}')
+    ldy = (n_out + 31) // 32 * 32 if backward else (n_out + 3) // 4 * 4
+    if H * W * k > INT32_MAX:
+        raise ValueError(f'wide output conv: {H} x {W} cells x {k} anchors = {H * W * k} proposals per image; the decode indexes them '
+                         f'in 32 bits (at most {INT32_MAX})')
+    if H * W * ldy * 2 >= TMA_STRIDE_LIMIT:
+        raise ValueError(f'wide output conv: an fp16 {H} x {W} x {ldy} gradient is {H * W * ldy * 2} bytes per image; the tensor maps '
+                         f'of the conv and wgrad operands take per-image strides below 2^40 bytes')
+    return ldy
+
+
+class _WideOutConvFn(torch.autograd.Function):
+    """conv3x3 (pad 1, bias) from 256 channels to n_out > 512 on the tensor cores, with a deterministic hand-written backward:
+    forward  ptb_split_f16 of the input, then one ptb_conv_tc_f16x2 launch per column slice of <= 512 into one (B,H,W,ldy) map
+             (ops.conv_tc_f16_cols; the columns from n_out to ldy are not written)
+    backward the (B,H,W,ldy) gradient split once (columns past n_out are zero: the caller takes the [..., :n_out] view), then
+             dW: one ptb_conv_tc_wgrad_f16x2_ld per 256-column slice, read in place; db: ptb_col_sum; dX: ONE 9-tap conv with
+             Cin = ldy on the transposed, flipped weights, zero-padded to ldy rows (ldy % 32 == 0, wide_out_conv_plan).
+    Every sum is formed in a fixed order: two backward passes give the same bits."""
+
+    @staticmethod
+    def forward(ctx, xm, weight, bias, ldy):
+        from . import ops
+        n_out = weight.shape[0]
+        h, l, inv = ops.split_f16(xm, auto_scale=True)
+        packs = ops.conv_tc_pack_weight_f16_cols(weight.detach().reshape(n_out, weight.shape[1], 9).contiguous(), 9)
+        y = ops.conv_tc_f16_cols(h, l, packs, 9, n_out, bias=bias.detach(), dev_out_scale=inv, ldy=ldy)
+        ctx.save_for_backward(h, l, inv, weight.detach())
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        from . import ops
+        h, l, inv, weight = ctx.saved_tensors
+        n_out, C = weight.shape[:2]
+        g = g.contiguous()
+        ldy = g.shape[-1]
+        gh, gl, ginv = ops.split_f16(g, auto_scale=True)
+        dw = db = dx = None
+        if ctx.needs_input_grad[1]:
+            dw = ops.conv_tc_wgrad_f16_cols(gh, gl, h, l, 1.0, ginv, inv, taps=9)[:n_out]
+        if ctx.needs_input_grad[2]:
+            db = ops.col_sum(g.view(-1, ldy))[:n_out]
+        if ctx.needs_input_grad[0]:
+            wt = weight.new_zeros((C, ldy, 3, 3))
+            wt[:, :n_out] = weight.flip(2, 3).transpose(0, 1)
+            dx = ops.conv_tc_f16(gh, gl, ops.conv_tc_pack_weight_f16(wt.reshape(C, ldy, 9), 9), 9, C, dev_out_scale=ginv, ldy=C)
+        return dx, dw, db, None
+
+
+def wide_out_conv(conv, x, k=1):
+    """conv(x) for an nn.Conv2d(256, n_out > 512, 3, padding=1) output layer on the tensor cores (_WideOutConvFn), differentiable in x,
+    weight and bias.  x: fp32 CUDA (B,256,H,W); returns a (B,n_out,H,W) view of the (B,H,W,ldy) map."""
+    from . import ops
+    if not x.is_cuda or x.dtype != torch.float32:
+        raise RuntimeError(f'wide output conv ({conv.out_channels} channels): expected an fp32 CUDA input, got {x.dtype} on {x.device}')
+    B, _, H, W = x.shape
+    backward = torch.is_grad_enabled() and (x.requires_grad or conv.weight.requires_grad or conv.bias.requires_grad)
+    ldy = wide_out_conv_plan(B, H, W, conv.out_channels, k, backward)
+    y = _WideOutConvFn.apply(ops.to_nhwc(x).contiguous(), conv.weight, conv.bias, ldy)
+    return y[..., :conv.out_channels].permute(0, 3, 1, 2)
 
 
 def tc_enabled(x, *modules):

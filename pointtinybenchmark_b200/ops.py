@@ -1005,19 +1005,19 @@ def conv_tc_wgrad_f16(dy_h, dy_l, x_h, x_l, taps, scale=1.0, dev_scale_dy=None, 
     return dw
 
 
-def conv_tc_wgrad_f16_cols(dy_h, dy_l, x_h, x_l, scale=1.0, dev_scale_dy=None, dev_scale_x=None, width=256):
-    """dW (Cout, 256) of a per-cell Linear whose output gradient dy (B,H,W,Cout) is wider than one tensor-core wgrad (Cout <= 256): one
-    ptb_conv_tc_wgrad_f16x2_ld launch per column slice [c0, c0 + width) of the fp16 pair, read in place (row stride Cout), writing rows
-    [c0, c0 + n) of dW.  Cout a multiple of 8."""
+def conv_tc_wgrad_f16_cols(dy_h, dy_l, x_h, x_l, scale=1.0, dev_scale_dy=None, dev_scale_x=None, width=256, taps=1):
+    """dW (Cout, 256) of a per-cell Linear (taps 1), or (Cout, 256, 3, 3) of a conv3x3 (taps 9), whose output gradient dy (B,H,W,Cout)
+    is wider than one tensor-core wgrad (Cout <= 256): one ptb_conv_tc_wgrad_f16x2_ld launch per column slice [c0, c0 + width) of the
+    fp16 pair, read in place (row stride Cout), writing rows [c0, c0 + n) of dW.  Cout a multiple of 8."""
     lib = _lib.load()
     _chk(dy_h, torch.float16, 'dy_h'); _chk(dy_l, torch.float16, 'dy_l'); _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
     B, H, W, Cout = dy_h.shape
     Cin = x_h.shape[3]
-    ws = torch.empty(int(lib.ptb_conv_tc_wgrad_workspace(B, H, W, 1)), dtype=torch.uint8, device=dy_h.device)
-    dw = torch.empty((Cout, Cin), dtype=torch.float32, device=dy_h.device)
+    ws = torch.empty(int(lib.ptb_conv_tc_wgrad_workspace(B, H, W, taps)), dtype=torch.uint8, device=dy_h.device)
+    dw = torch.empty((Cout, Cin, 3, 3) if taps == 9 else (Cout, Cin), dtype=torch.float32, device=dy_h.device)
     for c0 in range(0, Cout, width):
         n = min(width, Cout - c0)
-        check(lib.ptb_conv_tc_wgrad_f16x2_ld(_ptr(dy_h[..., c0:]), _ptr(dy_l[..., c0:]), Cout, _ptr(x_h), _ptr(x_l), B, H, W, n, Cin, 1,
+        check(lib.ptb_conv_tc_wgrad_f16x2_ld(_ptr(dy_h[..., c0:]), _ptr(dy_l[..., c0:]), Cout, _ptr(x_h), _ptr(x_l), B, H, W, n, Cin, taps,
                                              float(scale), _ptr(dev_scale_dy), _ptr(dev_scale_x), _ptr(ws), _ptr(dw[c0:]), 0, _stream()),
               'ptb_conv_tc_wgrad_f16x2_ld')
     return dw

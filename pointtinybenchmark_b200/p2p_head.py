@@ -7,8 +7,9 @@ multiclass_nms (core/post_processing/bbox_nms.py).  Same ctor kwargs / outputs /
 (cls_convs.*, reg_convs.*, cls_out (conv3x3), reg_out (conv3x3)).
 
 What runs where: towers and the two output convs = wgmma implicit GEMMs of libptb_b200.so at inference; under autograd the
-towers use the tensor-core autograd function of layers.py (dgrad / wgrad / GroupNorm backward kernels) and the two narrow output
-convs cuDNN fp32; decode, top-k, NMS / soft-NMS, cost matrix, the Hungarian matching (scipy's shortest-augmenting-path algorithm
+towers use the tensor-core autograd function of layers.py (dgrad / wgrad / GroupNorm backward kernels), the two output convs cuDNN fp32
+up to 512 channels and a cls_out wider than that (257 to 1280 classes: Objects365, LVIS) the tensor-core autograd function
+layers._WideOutConvFn (column-sliced forward, deterministic wgrad / dgrad); decode, top-k, NMS / soft-NMS, cost matrix, the Hungarian matching (scipy's shortest-augmenting-path algorithm
 restated as a one-CTA-per-image kernel, bit-identical assignments incl. ties: csrc/lsap_core.cuh; SURVEY.md §8f rank 2) and the
 losses = libptb_b200.so: FocalLoss or the reference's default CrossEntropyLoss(use_sigmoid=True) for classification, the latter
 also with class_weight (= pos_weight) or in softmax mode (use_sigmoid=False: C+1 outputs per anchor, background last, softmax decode
@@ -22,7 +23,8 @@ import torch.nn as nn
 from . import ops
 from .assigners import cost_matrix, match_cost_terms
 from .post_processing import check_split_thr
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, wide_out_conv, \
+    wide_out_conv_plan, _packed_tc, _packed_tc_cols
 from .registry import CfgNode, register_head
 
 
@@ -54,7 +56,10 @@ class _LossSumFn(torch.autograd.Function):
         return (None, ctx.op(x, *args, scale=scale, want_grad=True)) + (None,) * len(args)
 
 
-MAX_OUT_CHANNELS = 512     # widest output of the wgmma conv (ptb_conv_tc_f16x2): bounds num_points * num_classes
+MAX_OUT_CHANNELS = 512     # widest output of one wgmma conv launch (ptb_conv_tc_f16x2): cls_out beyond it runs in column slices
+MAX_CLASSES = 1280         # CPRHead's limit (cpr_head.MAX_CLASSES): the second stage takes every dataset the first one refines
+WIDE_MIN_CLASSES = 257     # the many-class path (cls_out in column slices) starts above 256 classes, where CPRHead's sliced logit map does;
+                           # up to 256 classes cls_out must fit one launch, as it always had to
 LOSS_CLS_TYPES = ('FocalLoss', 'CrossEntropyLoss')
 LOSS_REG_TYPES = ('SmoothL1Loss', 'MSELoss')
 
@@ -94,10 +99,19 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             raise ValueError(f'P2PHead: CrossEntropyLoss.class_weight has {len(cw)} entries; '
                              f'{"sigmoid" if self.use_sigmoid_cls else "softmax"} classification needs {self.num_cls_out}')
         self.class_weight = None if cw is None else torch.tensor([float(v) for v in cw], dtype=torch.float32)
-        if max(self.num_cls_out * self.num_points, 2 * self.num_points) > MAX_OUT_CHANNELS:
+        if num_classes > MAX_CLASSES:
+            raise NotImplementedError(f'P2PHead: num_classes={num_classes} exceeds the {MAX_CLASSES} classes the CUDA head supports')
+        if self.num_cls_out * self.num_points > MAX_OUT_CHANNELS and num_classes < WIDE_MIN_CLASSES:
             raise NotImplementedError(
                 f'P2PHead: cls_out would have {self.num_cls_out} classes x {self.num_points} anchors = '
-                f'{self.num_cls_out * self.num_points} output channels; the output conv kernel supports at most {MAX_OUT_CHANNELS}')
+                f'{self.num_cls_out * self.num_points} output channels; up to {WIDE_MIN_CLASSES - 1} classes the output conv kernel '
+                f'supports at most {MAX_OUT_CHANNELS} (heads of {WIDE_MIN_CLASSES} to {MAX_CLASSES} classes run it in column slices)')
+        if 2 * self.num_points > MAX_OUT_CHANNELS:
+            raise NotImplementedError(f'P2PHead: reg_out would have 2 x {self.num_points} anchors = {2 * self.num_points} output '
+                                      f'channels; the output conv kernel supports at most {MAX_OUT_CHANNELS}')
+        if self.num_cls_out * self.num_points > MAX_OUT_CHANNELS and feat_channels != 256:
+            raise NotImplementedError(f'P2PHead: a cls_out of {self.num_cls_out * self.num_points} output channels (> {MAX_OUT_CHANNELS}) '
+                                      f'runs on the tensor-core wide conv, which takes feat_channels=256 (got {feat_channels})')
         self.cls_convs, self.reg_convs = nn.ModuleList(), nn.ModuleList()
         for i in range(stacked_convs):
             chn = in_channels if i == 0 else feat_channels
@@ -120,9 +134,10 @@ class P2PHead(PackedWeightsMixin, nn.Module):
     # ------------------------------------------------------------------------------------------------
     def forward(self, feats):
         """p2p_head.py:104-123.  Inference: towers AND the two conv3x3 output layers run on the wgmma kernel (fp16 two-term
-        split, fp32-level accuracy; cls_out has num_points * num_classes <= 512 channels, e.g. 320 at the reference's default 4
-        anchors x 80 classes, in one launch); with autograd recording the towers use the tensor-core autograd function of
-        layers.py and the two output convs cuDNN fp32 (also inside a caller's autocast region).
+        split, fp32-level accuracy; a cls_out of up to 512 channels, e.g. 320 at the reference's default 4 anchors x 80 classes, in one
+        launch, a wider one as column slices of <= 512 into one map, layers.wide_out_conv_plan's ldy); with autograd recording the
+        towers use the tensor-core autograd function of layers.py and the two output convs cuDNN fp32 up to 512 channels, a wider
+        cls_out layers._WideOutConvFn (also inside a caller's autocast region).
         feats[i]: fp32, or the fp16 / bf16 map of a backbone under torch.autocast, taken as it is (layers.input_plan; no .float() in
         front of the head).  The outputs are fp32; `last_input_path` names the path the towers took."""
         cls_outs, pts_outs = [], []
@@ -135,20 +150,29 @@ class P2PHead(PackedWeightsMixin, nn.Module):
                 if pc is not None and pr is not None:
                     self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
                     nc, nr = self.cls_out.out_channels, self.reg_out.out_channels
-                    yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9, 'conv'), 9, nc, bias=self.cls_out.bias.detach())
+                    if nc > MAX_OUT_CHANNELS:      # one launch per 512-column slice; ldy = ceil4(nc): [..., :nc] is the whole map if 4 | nc
+                        B_, H_, W_ = pc[0].shape[:3]
+                        yc = ops.conv_tc_f16_cols(pc[0], pc[1], _packed_tc_cols(self.cls_out, 9), 9, nc, bias=self.cls_out.bias.detach(),
+                                                  ldy=wide_out_conv_plan(B_, H_, W_, nc, self.num_points))
+                    else:
+                        yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9, 'conv'), 9, nc, bias=self.cls_out.bias.detach())
                     yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9, 'conv'), 9, nr, bias=self.reg_out.bias.detach())
                     cls_outs.append(yc[..., :nc].permute(0, 3, 1, 2))
                     pts_outs.append(yr[..., :nr].permute(0, 3, 1, 2))
                     continue
             # autograd path: the towers run layers._TowerTCFn (tensor-core forward + dgrad + wgrad + GroupNorm backward) for the
-            # shipped geometry; the two narrow output convs (256 -> C / 2k) stay cuDNN fp32, never TF32 (1e-4 logits)
+            # shipped geometry; output convs of up to 512 channels stay cuDNN fp32, never TF32 (1e-4 logits); a wider cls_out runs
+            # layers._WideOutConvFn on the tensor cores (selected from the width alone)
             info = {}
             fc, fr = tower(self.cls_convs, x, info), tower(self.reg_convs, x, info)
             self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
             with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
                                             deterministic=torch.backends.cudnn.deterministic, allow_tf32=False), \
                     torch.autocast('cuda', enabled=False):
-                cls_outs.append(self.cls_out(fc))
+                if self.cls_out.out_channels > MAX_OUT_CHANNELS:
+                    cls_outs.append(wide_out_conv(self.cls_out, fc, self.num_points))
+                else:
+                    cls_outs.append(self.cls_out(fc))
                 pts_outs.append(self.reg_out(fr))
         return cls_outs, pts_outs
 
