@@ -278,6 +278,24 @@ int ptb_p2p_decode_topk_softmax(const float* cls_map, const float* reg_map, int 
                                 const int32_t* img_hw, const float* scale_xy /*[B][2] or NULL*/, int nms_pre,
                                 int32_t* out_topk_idx /*[B][P]*/, float* out_pts /*[B][P][2]*/, float* out_scores /*[B][P][C]*/,
                                 void* workspace, uint64_t workspace_bytes, void* stream);
+/* Several FPN levels (P2PHead with strides [s_0, ..., s_{L-1}], p2p_head.py:125-170, 345-381), sigmoid or softmax scores as above.
+ * Level l: cls_maps[l] [B][H_l][W_l][k*C1], reg_maps[l] [B][H_l][W_l][2k], hw[l] = (H_l, W_l), strides[l] (host arrays of L <= 8
+ * entries; the maps are device pointers).  An image's T = sum_l H_l W_l k rows are the levels' proposals, level-major.  As the
+ * reference's _get_bboxes_single, the rows are split into L equal chunks of T / L rows (not into levels: a chunk may straddle
+ * levels), and each chunk keeps its top nms_pre rows by the max foreground score (ties: lower index first), or all of its rows when
+ * nms_pre <= 0 or nms_pre >= T / L.  P = rows kept per chunk; output row r of image b is entry r % P of chunk r / P:
+ *   out_topk_idx[b][r] = the chunk-local row index (reference topk_inds),  out_pts / out_scores as above with the row's own stride.
+ * T % L != 0 is refused (the reference's reshape raises there).  nms_pre <= 4096.  workspace: ptb_p2p_decode_topk_levels_workspace. */
+int ptb_p2p_decode_topk_levels(const float* const* cls_maps, const float* const* reg_maps, int L, const int32_t* hw /*[L][2]*/,
+                               const float* strides /*[L]*/, int B, int num_classes, int k, const float* point_anchor /*[k][2]*/,
+                               float pts_gamma, const int32_t* img_hw, const float* scale_xy /*[B][2] or NULL*/, int nms_pre,
+                               int32_t* out_topk_idx /*[B][L*P]*/, float* out_pts /*[B][L*P][2]*/, float* out_scores /*[B][L*P][C]*/,
+                               void* workspace, uint64_t workspace_bytes, void* stream);
+int ptb_p2p_decode_topk_levels_softmax(const float* const* cls_maps, const float* const* reg_maps, int L, const int32_t* hw,
+                                       const float* strides, int B, int num_classes, int k, const float* point_anchor, float pts_gamma,
+                                       const int32_t* img_hw, const float* scale_xy, int nms_pre, int32_t* out_topk_idx,
+                                       float* out_pts, float* out_scores, void* workspace, uint64_t workspace_bytes, void* stream);
+uint64_t ptb_p2p_decode_topk_levels_workspace(int B, int L, const int32_t* hw /*[L][2]*/, int k);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * multiclass NMS — replaces multiclass_nms (mmdet/core/post_processing/bbox_nms.py:7-94) and the third-party
@@ -330,6 +348,18 @@ int ptb_multiclass_soft_nms_cls_boxes(const float* boxes /*[B][P][C][4]*/, const
                                       int num_classes, float score_thr, float iou_thr, float sigma, float min_score, int method,
                                       int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep,
                                       int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes, void* stream);
+/* ptb_multiclass_nms / ptb_multiclass_soft_nms (point pseudo-boxes or shared boxes) for up to 8192 points per image, e.g. the
+ * multi-level P2P head's L x nms_pre candidates.  Same arguments, workspaces (ptb_multiclass_nms_workspace,
+ * ptb_multiclass_soft_nms_workspace) and results. */
+int ptb_multiclass_nms_wide(const float* pts /*[B][P][2]*/, const float* scores /*[B][P][C]*/, int B, int P, int num_classes,
+                            float pseudo_w, float pseudo_h, float score_thr, float iou_thr, int max_per_img,
+                            int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count,
+                            void* workspace, uint64_t workspace_bytes, void* stream);
+int ptb_multiclass_soft_nms_wide(const float* pts /*[B][P][2] or NULL*/, const float* boxes /*[B][P][4] or NULL*/,
+                                 const float* scores /*[B][P][C]*/, int B, int P, int num_classes, float pseudo_w, float pseudo_h,
+                                 float score_thr, float iou_thr, float sigma, float min_score, int method, int max_per_img,
+                                 int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count,
+                                 void* workspace, uint64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Hungarian cost matrix — replaces FocalLossCost + DisCostV2 (mmdet/core/bbox/match_costs/match_cost.py:94-99,
@@ -462,6 +492,13 @@ int ptb_sigmoid_bce_cw_fwd_bwd(const float* logits /*[M][C]*/, const int64_t* la
 int ptb_softmax_ce_fwd_bwd(const float* logits /*[M][num_cols]*/, const int64_t* labels /*[M]*/, const float* weight /*[M] or NULL*/,
                            const float* class_weight /*[num_cols] or NULL*/, int64_t M, int num_cols, float* loss_sum /*[1]*/,
                            const float* scale /*[1] or NULL*/, float* grad /*[M][num_cols] or NULL*/, void* stream);
+/* ptb_smooth_l1_fwd_bwd / ptb_mse_fwd_bwd with one normalisation per proposal row, row_inv_norm[m] = 1 / (stride_m * reg_norm):
+ * the multi-level P2P head, where each row is divided by its own level's stride (p2p_head.py:234-240). */
+int ptb_smooth_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2]*/, int64_t M,
+                               const float* row_inv_norm /*[M]*/, float beta, float* loss_sum, const float* scale, float* grad,
+                               void* stream);
+int ptb_mse_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
+                         const float* row_inv_norm /*[M]*/, float* loss_sum, const float* scale, float* grad, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Conv towers on the tensor cores — replace the cuDNN calls behind CPRHead.forward_single / P2PHead.forward_single

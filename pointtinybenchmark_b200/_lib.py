@@ -64,6 +64,14 @@ SIGNATURES = {
     'ptb_multiclass_nms': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, P, P, P, P, P, P,
                                    c_u64, P]),
     'ptb_multiclass_nms_workspace': (c_u64, [c_int, c_int, c_int]),
+    'ptb_multiclass_nms_wide': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, P, P, P, P, P, P,
+                                        c_u64, P]),
+    'ptb_multiclass_soft_nms_wide': (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_int,
+                                             c_int, P, P, P, P, P, P, c_u64, P]),
+    'ptb_p2p_decode_topk_levels': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P, c_float, P, P, c_int, P, P, P, P, c_u64, P]),
+    'ptb_p2p_decode_topk_levels_softmax': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P, c_float, P, P, c_int, P, P, P, P, c_u64,
+                                                   P]),
+    'ptb_p2p_decode_topk_levels_workspace': (c_u64, [c_int, c_int, P, c_int]),
     'ptb_multiclass_soft_nms': (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_int, c_int,
                                         P, P, P, P, P, P, c_u64, P]),
     'ptb_multiclass_soft_nms_workspace': (c_u64, [c_int, c_int, c_int]),
@@ -85,6 +93,8 @@ SIGNATURES = {
     'ptb_smooth_l1_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, c_float, P, P, P, P]),
     'ptb_sigmoid_bce_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_mse_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, P, P, P, P]),
+    'ptb_smooth_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, P, P, P, P]),
+    'ptb_mse_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, P, P, P, P]),
     'ptb_sigmoid_bce_cw_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_softmax_ce_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_split_tf32': (c_int, [P, c_i64, P, P, P]),

@@ -16,6 +16,9 @@
 namespace ptb {
 
 constexpr int NMS_MAXP = 4096;      // points per image supported (nms_pre)
+// the *_wide entry points: up to 8192 points per image (nms_pre over several FPN levels, e.g. 5 x 1000).  Their class kernel keeps
+// its sort keys in dynamic shared memory and their soft-NMS class kernel recomputes each box area instead of storing it.
+constexpr int NMS_MAXP_WIDE = 8192;
 constexpr int NMS_T0 = 1024;
 // mmcv batched_nms's default split_thr: from this many candidates on it runs NMS class by class and sorts the kept entries by
 // score, so the classes never interact whatever the offset does - the per-class kernels and the merge are that branch exactly
@@ -78,12 +81,12 @@ __device__ __forceinline__ Box offset_box(const RawBox& r, float off) {
   return b;
 }
 
-template <int cs>
+template <int cs, bool WIDE>
 __global__ void NMS_T0_BOUNDS(cs)
 nms_prepare_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                    float score_thr, NmsImg* __restrict__ hdr, int32_t* __restrict__ base /*[B][P]*/,
                    int32_t* __restrict__ out_cand_count) {
-  __shared__ int s_cnt[NMS_MAXP];
+  __shared__ int s_cnt[WIDE ? NMS_MAXP_WIDE : NMS_MAXP];
   __shared__ float s_max[NMS_T0 / 32];
   __shared__ int s_wsum[NMS_T0 / 32];
   const int b = blockIdx.x;
@@ -201,15 +204,17 @@ __device__ __forceinline__ void bitonic_sort_u64_blk(unsigned long long* a, int 
 constexpr int NMS_T1 = 256;
 
 // per (image, class): list[b][c][0..n) = kept point indices in descending score order (n <= max_keep)
-template <int cs>
+template <int cs, bool WIDE>
 __global__ void __launch_bounds__(NMS_T1)
 nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C, float hw, float hh,
                  float score_thr, float iou_thr, int max_keep, const NmsImg* __restrict__ hdr,
                  int32_t* __restrict__ cls_cnt /*[B][C]*/, int32_t* __restrict__ cls_list /*[B][C][max_keep]*/) {
-  __shared__ unsigned long long keys[NMS_MAXP];
+  __shared__ unsigned long long keys_static[WIDE ? 1 : NMS_MAXP];
   __shared__ int s_n;
   __shared__ int s_wbase[NMS_T1 / 32];
-  extern __shared__ float kept[];     // [max_keep][5]
+  extern __shared__ unsigned long long dyn_sm[];     // WIDE: keys [NMS_MAXP_WIDE], then the kept list; else the kept list
+  unsigned long long* keys = WIDE ? dyn_sm : keys_static;
+  float* kept = reinterpret_cast<float*>(WIDE ? dyn_sm + NMS_MAXP_WIDE : dyn_sm);   // [max_keep][5]
   const int b = blockIdx.y, c = blockIdx.x;
   if (hdr[b].slow) return;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -360,16 +365,21 @@ __device__ __forceinline__ float soft_weight(float ovr, float iou_thr, float sig
 }
 
 
-template <int cs>
+template <int cs, bool WIDE>
 __global__ void __launch_bounds__(SNMS_T)
 soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ boxes, const float* __restrict__ scores, int P, int C,
                       float hw, float hh, float score_thr, float iou_thr, float sigma, float min_score, int method, int max_keep,
                       NmsImg* __restrict__ hdr, int32_t* __restrict__ cls_cnt, int32_t* __restrict__ cls_list,
                       float* __restrict__ cls_score) {
-  extern __shared__ float sm[];                 // x1 | y1 | x2 | y2 | area | score : [P] each, then idx [P] (int), alive [P] (u8)
-  float* bx1 = sm; float* by1 = sm + P; float* bx2 = sm + 2 * P; float* by2 = sm + 3 * P; float* bar = sm + 4 * P; float* bsc = sm + 5 * P;
-  int* bidx = reinterpret_cast<int*>(sm + 6 * P);
-  unsigned char* alive = reinterpret_cast<unsigned char*>(sm + 7 * P);
+  // x1 | y1 | x2 | y2 | area | score : [P] each, then idx [P] (int), alive [P] (u8).  WIDE: no area array (recomputed from the
+  // offset box by offset_box's formula, the same bits), so 8192 candidates fit
+  extern __shared__ float sm[];
+  constexpr int NA = WIDE ? 0 : 1;
+  float* bx1 = sm; float* by1 = sm + P; float* bx2 = sm + 2 * P; float* by2 = sm + 3 * P; float* bar = sm + 4 * P;
+  float* bsc = sm + (4 + NA) * P;
+  int* bidx = reinterpret_cast<int*>(sm + (5 + NA) * P);
+  unsigned char* alive = reinterpret_cast<unsigned char*>(sm + (6 + NA) * P);
+  auto area_of = [&](int j) { return WIDE ? __fmul_rn(__fsub_rn(bx2[j], bx1[j]), __fsub_rn(by2[j], by1[j])) : bar[j]; };
   __shared__ int s_wcnt[SNMS_T / 32];
   __shared__ unsigned long long s_red[SNMS_T / 32];
   __shared__ unsigned long long s_best;
@@ -394,7 +404,8 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
     if (is) {
       const int slot = n + before + __popc(bal & ((1u << lane) - 1u));
       const Box me = offset_box(raw_box(pp, bx, box_row(p, c, C, cs), hw, hh), off);
-      bx1[slot] = me.x1; by1[slot] = me.y1; bx2[slot] = me.x2; by2[slot] = me.y2; bar[slot] = me.area;
+      bx1[slot] = me.x1; by1[slot] = me.y1; bx2[slot] = me.x2; by2[slot] = me.y2;
+      if (!WIDE) bar[slot] = me.area;
       bsc[slot] = s; bidx[slot] = p; alive[slot] = 1;
     }
     n += total;
@@ -402,7 +413,7 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
   }
   if (method == 2) {          // degenerate boxes of the whole image, summed over its classes; the merge refuses the image
     int d = 0;
-    for (int j = threadIdx.x; j < n; j += SNMS_T) d += degenerate_weight(bar[j]);
+    for (int j = threadIdx.x; j < n; j += SNMS_T) d += degenerate_weight(area_of(j));
     if (d) atomicAdd(&hdr[b].degenerate, d);
   }
   int nk = 0;
@@ -437,14 +448,14 @@ soft_nms_class_kernel(const float* __restrict__ pts, const float* __restrict__ b
     if (best == 0xFFFFFFFFFFFFFFFFull) break;
     ++nk;
     const int w0 = (int)(best & 0xFFFFFFFFull);
-    const float ix1 = bx1[w0], iy1 = by1[w0], ix2 = bx2[w0], iy2 = by2[w0], iarea = bar[w0];
+    const float ix1 = bx1[w0], iy1 = by1[w0], ix2 = bx2[w0], iy2 = by2[w0], iarea = area_of(w0);
     // ---- decay every remaining candidate (mmcv's operation order: offset 0)
     for (int j = threadIdx.x; j < n; j += SNMS_T)
       if (alive[j]) {
         const float w = fmaxf(0.f, __fsub_rn(fminf(ix2, bx2[j]), fmaxf(ix1, bx1[j])));
         const float h = fmaxf(0.f, __fsub_rn(fminf(iy2, by2[j]), fmaxf(iy1, by1[j])));
         const float inter = __fmul_rn(w, h);
-        const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(iarea, bar[j]), inter));
+        const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(iarea, area_of(j)), inter));
         const float ns = __fmul_rn(bsc[j], soft_weight(ovr, iou_thr, sigma, method));
         bsc[j] = ns;
         if (ns < min_score) alive[j] = 0;
@@ -644,13 +655,14 @@ extern "C" uint64_t ptb_multiclass_nms_workspace(int B, int P, int num_classes) 
 #define NMS_REQUIRE_CS_ROWS(cs, P, C) \
   PTB_REQUIRE(!(cs) || (uint64_t)(P) * (uint64_t)(C) * 4 <= 0x7fffffffull, "class-specific boxes: 4 * P * num_classes must fit in int")
 
-template <int cs>
+template <int cs, bool WIDE = false>
 static int nms_run(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes, float pseudo_w,
                    float pseudo_h, float score_thr, float iou_thr, int max_per_img, int32_t* out_count, float* out_det,
                    int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
                    void* stream) {
   PTB_REQUIRE(B > 0 && P > 0 && num_classes > 0, "shape");
-  PTB_REQUIRE(P <= NMS_MAXP, "more than 4096 points per image not supported");
+  if (WIDE) PTB_REQUIRE(P <= NMS_MAXP_WIDE, "more than 8192 points per image not supported");
+  else PTB_REQUIRE(P <= NMS_MAXP, "more than 4096 points per image not supported");
   PTB_REQUIRE(max_per_img > 0 && max_per_img <= 1024, "max_per_img must be in [1,1024]");
   PTB_REQUIRE(iou_thr >= 0.f, "iou_thr must be >= 0 (per-class decomposition)");
   PTB_REQUIRE((pts || boxes) && scores && out_count && out_det && out_label && out_keep && out_cand_count, "NULL input");
@@ -663,14 +675,17 @@ static int nms_run(const float* pts, const float* boxes, const float* scores, in
   const float hw = pseudo_w * 0.5f, hh = pseudo_h * 0.5f;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  nms_prepare_kernel<cs><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
+  nms_prepare_kernel<cs, WIDE><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
   if ((rc = check_launch("ptb_multiclass_nms/prepare"))) return rc;
-  // keys (32 KB static) + kept list (dynamic) can exceed the 48 KB default; the attribute is per device -> set on every call
-  if (cudaFuncSetAttribute(nms_class_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess ||
+  // keys (32 KB static, or 64 KB dynamic when WIDE) + kept list (dynamic) can exceed the 48 KB default; the attribute is per device
+  // -> set on every call
+  const int keys_dyn = WIDE ? NMS_MAXP_WIDE * (int)sizeof(unsigned long long) : 0;
+  if (cudaFuncSetAttribute(nms_class_kernel<cs, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           keys_dyn + 1024 * 5 * (int)sizeof(float)) != cudaSuccess ||
       cudaFuncSetAttribute(nms_global_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 * 5 * (int)sizeof(float)) != cudaSuccess)
     return fail("%s", "ptb_multiclass_nms: shared memory opt-in failed");
   dim3 g1(num_classes, B);
-  nms_class_kernel<cs><<<g1, NMS_T1, (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
+  nms_class_kernel<cs, WIDE><<<g1, NMS_T1, keys_dyn + (size_t)max_per_img * 5 * sizeof(float), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr,
                                                                               iou_thr, max_per_img, hdr, cls_cnt, cls_list);
   if ((rc = check_launch("ptb_multiclass_nms/class"))) return rc;
   nms_merge_kernel<cs><<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
@@ -716,13 +731,14 @@ extern "C" uint64_t ptb_multiclass_soft_nms_workspace(int B, int P, int num_clas
          ((uint64_t)B * P + (uint64_t)B * num_classes + 2 * (uint64_t)B * num_classes * 1024 + (uint64_t)B * P * num_classes) * 4;
 }
 
-template <int cs>
+template <int cs, bool WIDE = false>
 static int soft_nms_run(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes,
                         float pseudo_w, float pseudo_h, float score_thr, float iou_thr, float sigma, float min_score, int method,
                         int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep,
                         int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes, void* stream) {
   PTB_REQUIRE(B > 0 && P > 0 && num_classes > 0, "shape");
-  PTB_REQUIRE(P <= NMS_MAXP, "more than 4096 points per image not supported");
+  if (WIDE) PTB_REQUIRE(P <= NMS_MAXP_WIDE, "more than 8192 points per image not supported");
+  else PTB_REQUIRE(P <= NMS_MAXP, "more than 4096 points per image not supported");
   PTB_REQUIRE(max_per_img > 0 && max_per_img <= 1024, "max_per_img must be in [1,1024]");
   PTB_REQUIRE(method >= 0 && method <= 2, "method: 0 naive, 1 linear, 2 gaussian");
   PTB_REQUIRE(method != 2 || sigma > 0.f, "sigma must be > 0 for the gaussian method");
@@ -741,15 +757,15 @@ static int soft_nms_run(const float* pts, const float* boxes, const float* score
   const float hw = pseudo_w * 0.5f, hh = pseudo_h * 0.5f;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  nms_prepare_kernel<cs><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
+  nms_prepare_kernel<cs, WIDE><<<B, NMS_T0, 0, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, hdr, base, out_cand_count);
   if ((rc = check_launch("ptb_multiclass_soft_nms/prepare"))) return rc;
-  const size_t smem = (size_t)P * (7 * sizeof(float) + 1) + 16;
+  const size_t smem = (size_t)P * ((WIDE ? 6 : 7) * sizeof(float) + 1) + 16;
   // the kernel's own 104 B of static shared memory count against the 48 KB default too (P = 1691..1694 have smem <= 48 KB but fail
   // to launch without the opt-in): set the per-device attribute on every call (a process may drive several devices)
-  if (cudaFuncSetAttribute(soft_nms_class_kernel<cs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+  if (cudaFuncSetAttribute(soft_nms_class_kernel<cs, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return fail("%s", "ptb_multiclass_soft_nms: shared memory opt-in failed");
   dim3 g1(num_classes, B);
-  soft_nms_class_kernel<cs><<<g1, SNMS_T, smem, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
+  soft_nms_class_kernel<cs, WIDE><<<g1, SNMS_T, smem, st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, iou_thr, sigma, min_score, method,
                                                 max_per_img, hdr, cls_cnt, cls_list, cls_score);
   if ((rc = check_launch("ptb_multiclass_soft_nms/class"))) return rc;
   nms_merge_kernel<cs><<<B, 32, (size_t)num_classes * sizeof(int), st>>>(pts, boxes, scores, P, num_classes, hw, hh, score_thr, max_per_img,
@@ -778,4 +794,24 @@ extern "C" int ptb_multiclass_soft_nms_cls_boxes(const float* boxes, const float
   PTB_REQUIRE(boxes, "NULL boxes");
   return soft_nms_run<1>(nullptr, boxes, scores, B, P, num_classes, 0.f, 0.f, score_thr, iou_thr, sigma, min_score, method,
                       max_per_img, out_count, out_det, out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
+}
+
+// up to 8192 points per image: the multi-level P2P head's candidates (L levels x nms_pre).  Same arguments, workspaces and results as
+// ptb_multiclass_nms / ptb_multiclass_soft_nms.
+extern "C" int ptb_multiclass_nms_wide(const float* pts, const float* scores, int B, int P, int num_classes, float pseudo_w,
+                                       float pseudo_h, float score_thr, float iou_thr, int max_per_img, int32_t* out_count,
+                                       float* out_det, int32_t* out_label, int32_t* out_keep, int32_t* out_cand_count,
+                                       void* workspace, uint64_t workspace_bytes, void* stream) {
+  PTB_REQUIRE(pts, "NULL pts");
+  return nms_run<0, true>(pts, nullptr, scores, B, P, num_classes, pseudo_w, pseudo_h, score_thr, iou_thr, max_per_img, out_count,
+                          out_det, out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ptb_multiclass_soft_nms_wide(const float* pts, const float* boxes, const float* scores, int B, int P, int num_classes,
+                                            float pseudo_w, float pseudo_h, float score_thr, float iou_thr, float sigma, float min_score,
+                                            int method, int max_per_img, int32_t* out_count, float* out_det, int32_t* out_label,
+                                            int32_t* out_keep, int32_t* out_cand_count, void* workspace, uint64_t workspace_bytes,
+                                            void* stream) {
+  return soft_nms_run<0, true>(pts, boxes, scores, B, P, num_classes, pseudo_w, pseudo_h, score_thr, iou_thr, sigma, min_score, method,
+                               max_per_img, out_count, out_det, out_label, out_keep, out_cand_count, workspace, workspace_bytes, stream);
 }

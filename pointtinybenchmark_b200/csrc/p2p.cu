@@ -101,6 +101,97 @@ p2p_gather_kernel(const float* __restrict__ cls_map, const float* __restrict__ r
 }
 
 // ------------------------------------------------------------------------------------------------
+// decode + top-k over several FPN levels (p2p_head.py:125-170, 355-381).  An image's rows t in [0, T), T = sum_l H_l W_l k, are the
+// levels' proposals concatenated level-major (cell-major, anchor-minor inside a level).  The reference's _get_bboxes_single then
+// reshapes them into L equal chunks of T / L rows - not into levels - and takes the top nms_pre of each chunk, so a chunk may
+// straddle two or more levels.  The key / select / gather steps below reproduce exactly that.
+// ------------------------------------------------------------------------------------------------
+constexpr int P2P_MAX_LEVELS = 8;
+struct P2PLevels {
+  const float* cls[P2P_MAX_LEVELS];      // [B][H_l][W_l][k*C1]
+  const float* reg[P2P_MAX_LEVELS];      // [B][H_l][W_l][2k]
+  int W[P2P_MAX_LEVELS];
+  float stride[P2P_MAX_LEVELS];
+  int row0[P2P_MAX_LEVELS + 1];          // first row of level l in an image; row0[L] = T
+  int L;
+  __device__ __forceinline__ int level_of(int t) const {
+    int l = 0;
+    while (l + 1 < L && t >= row0[l + 1]) ++l;
+    return l;
+  }
+};
+
+// key[b][t] as p2p_score_kernel / p2p_softmax_score_kernel compute it for row t's level.  One warp per row.
+template <bool SOFTMAX>
+__global__ void __launch_bounds__(256)
+p2p_levels_score_kernel(P2PLevels lv, int B, int C, float* __restrict__ key) {
+  const long long wq = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const int T = lv.row0[lv.L];
+  if (wq >= (long long)B * T) return;
+  const int b = (int)(wq / T), t = (int)(wq - (long long)b * T);
+  const int l = lv.level_of(t);
+  const long long q = (long long)b * (lv.row0[l + 1] - lv.row0[l]) + (t - lv.row0[l]);
+  if constexpr (SOFTMAX) {
+    float m, s, e_fg;
+    softmax_row_stats(lv.cls[l] + q * (C + 1), C + 1, lane, m, s, e_fg);
+    if (lane == 0) key[wq] = __fdiv_rn(e_fg, s);
+  } else {
+    const float* row = lv.cls[l] + q * C;
+    float mx = -CUDART_INF_F;
+    for (int c = lane; c < C; c += 32) mx = fmaxf(mx, sigmoidf_acc(row[c]));
+    mx = warp_max(mx);
+    if (lane == 0) key[wq] = mx;
+  }
+}
+
+// gather: output row r of image b is entry r % P of chunk r / P; its image row is t = chunk * (T / L) + the chunk-local index
+// (the select's output, or r itself when every chunk keeps all its rows).  Decode and scores as p2p_gather_kernel, at t's level.
+template <bool SOFTMAX>
+__global__ void __launch_bounds__(256)
+p2p_levels_gather_kernel(P2PLevels lv, int C, int k, const float* __restrict__ point_anchor, float gamma,
+                         const int32_t* __restrict__ img_hw, const float* __restrict__ scale_xy, int P, int identity,
+                         int32_t* __restrict__ topk_idx, float* __restrict__ out_pts, float* __restrict__ out_scores, long long BR) {
+  const long long wr = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (wr >= BR) return;
+  const int LP = lv.L * P, T = lv.row0[lv.L];
+  const int b = (int)(wr / LP);
+  const int r = (int)(wr - (long long)b * LP);
+  const int chunk = r / P;
+  const int local = identity ? r - chunk * P : topk_idx[wr];
+  const int t = chunk * (T / lv.L) + local;
+  const int l = lv.level_of(t);
+  const int Ql = lv.row0[l + 1] - lv.row0[l];
+  const int q = t - lv.row0[l];
+  const int cell = q / k, a = q - cell * k;
+  const int i = cell / lv.W[l], j = cell - i * lv.W[l];
+  const float stride = lv.stride[l];
+  if (lane == 0) {
+    if (identity) topk_idx[wr] = local;
+    const float ax = __fadd_rn(__fmul_rn((float)j, stride), __fmul_rn(point_anchor[2 * a], stride));
+    const float ay = __fadd_rn(__fmul_rn((float)i, stride), __fmul_rn(point_anchor[2 * a + 1], stride));
+    const float* rg = lv.reg[l] + ((size_t)b * (Ql / k) + cell) * (2 * k) + 2 * a;
+    float x = __fadd_rn(ax, __fmul_rn(__fmul_rn(rg[0], gamma), stride));
+    float y = __fadd_rn(ay, __fmul_rn(__fmul_rn(rg[1], gamma), stride));
+    x = fminf(fmaxf(x, 0.f), (float)img_hw[2 * b + 1]);
+    y = fminf(fmaxf(y, 0.f), (float)img_hw[2 * b]);
+    if (scale_xy) { x = __fdiv_rn(x, scale_xy[2 * b]); y = __fdiv_rn(y, scale_xy[2 * b + 1]); }
+    out_pts[wr * 2] = x; out_pts[wr * 2 + 1] = y;
+  }
+  float* orow = out_scores + wr * C;
+  if constexpr (SOFTMAX) {
+    const float* row = lv.cls[l] + ((size_t)b * Ql + q) * (C + 1);
+    float m, s, e_fg;
+    softmax_row_stats(row, C + 1, lane, m, s, e_fg);
+    for (int c = lane; c < C; c += 32) orow[c] = __fdiv_rn(sleef_expf_u10(__fsub_rn(row[c], m)), s);
+  } else {
+    const float* row = lv.cls[l] + ((size_t)b * Ql + q) * C;
+    for (int c = lane; c < C; c += 32) orow[c] = sigmoidf_acc(row[c]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // cost matrix
 // ------------------------------------------------------------------------------------------------
 // FocalLossCost (match_cost.py:94-100) of one logit
@@ -332,6 +423,18 @@ struct SmoothL1Loss {
   }
 };
 
+// The regression losses over several FPN levels: each proposal row m brings its own 1 / (stride_m * reg_norm) (p2p_head.py:234-240
+// divides by the row's own stride), the rest is the single-level functor.
+template <class Loss>
+struct PerRowNorm {
+  Loss base; const float* row_inv_norm;
+  __device__ __forceinline__ float operator()(long long e, bool want_loss, float* grad, float sc) const {
+    Loss l = base;
+    l.inv_norm = row_inv_norm[e >> 1];
+    return l(e, want_loss, grad, sc);
+  }
+};
+
 // CrossEntropyLoss(use_sigmoid=True) = binary_cross_entropy (cross_entropy_loss.py:42-89): labels expanded to one-hot rows
 // (_expand_onehot_labels; a label outside [0, C), e.g. the background label C, is an all-zero row), the per-proposal weight
 // broadcast over the classes, F.binary_cross_entropy_with_logits(reduction='none') in ATen's CPU form
@@ -482,6 +585,79 @@ extern "C" int ptb_p2p_decode_topk_softmax(const float* cls_map, const float* re
                                nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
 }
 
+extern "C" uint64_t ptb_p2p_decode_topk_levels_workspace(int B, int L, const int32_t* hw, int k) {
+  uint64_t T = 0;
+  for (int l = 0; l < L && hw; ++l) T += (uint64_t)hw[2 * l] * hw[2 * l + 1] * k;
+  return (uint64_t)B * T * sizeof(float);
+}
+
+template <bool SOFTMAX>
+static int p2p_decode_topk_levels(const float* const* cls_maps, const float* const* reg_maps, int L, const int32_t* hw,
+                                  const float* strides, int B, int num_classes, int k, const float* point_anchor, float pts_gamma,
+                                  const int32_t* img_hw, const float* scale_xy, int nms_pre, int32_t* out_topk_idx, float* out_pts,
+                                  float* out_scores, void* workspace, uint64_t workspace_bytes, void* stream) {
+  const char* name = SOFTMAX ? "ptb_p2p_decode_topk_levels_softmax" : "ptb_p2p_decode_topk_levels";
+  char what[64];
+  PTB_REQUIRE(L >= 1 && L <= P2P_MAX_LEVELS, "1 to 8 levels");
+  PTB_REQUIRE(B > 0 && num_classes > 0 && k > 0, "shape");
+  PTB_REQUIRE(cls_maps && reg_maps && hw && strides && point_anchor && img_hw && out_topk_idx && out_pts && out_scores, "NULL input");
+  P2PLevels lv = {};
+  lv.L = L;
+  long long T = 0;
+  for (int l = 0; l < L; ++l) {
+    PTB_REQUIRE(cls_maps[l] && reg_maps[l] && hw[2 * l] > 0 && hw[2 * l + 1] > 0 && strides[l] > 0.f, "level shape");
+    lv.cls[l] = cls_maps[l]; lv.reg[l] = reg_maps[l]; lv.W[l] = hw[2 * l + 1]; lv.stride[l] = strides[l];
+    lv.row0[l] = (int)T;
+    T += (long long)hw[2 * l] * hw[2 * l + 1] * k;
+    PTB_REQUIRE(T <= 0x7fffffffLL, "more than 2^31 - 1 proposals per image");
+  }
+  lv.row0[L] = (int)T;
+  // p2p_head.py:357-358 reshapes the rows into L equal chunks, which raises when L does not divide them
+  PTB_REQUIRE(T % L == 0, "the number of proposals per image is not a multiple of the number of levels");
+  const int chunk = (int)(T / L);
+  const bool identity = !(nms_pre > 0 && nms_pre < chunk);
+  const int P = identity ? chunk : nms_pre;
+  PTB_REQUIRE(identity || nms_pre <= TOPK_MAX, "nms_pre > 4096 not supported");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (!identity) {
+    PTB_REQUIRE(workspace && workspace_bytes >= ptb_p2p_decode_topk_levels_workspace(B, L, hw, k), "workspace too small");
+    float* key = reinterpret_cast<float*>(workspace);
+    const long long BT = (long long)B * T;
+    p2p_levels_score_kernel<SOFTMAX><<<(unsigned)((BT * 32 + 255) / 256), 256, 0, st>>>(lv, B, num_classes, key);
+    snprintf(what, sizeof(what), "%s/score", name);
+    if ((rc = check_launch(what))) return rc;
+    // the B * L chunks are consecutive runs of T / L keys: one select CTA each, output row (b, chunk) at (b * L + chunk) * P
+    p2p_select_kernel<<<B * L, SEL_THREADS, 0, st>>>(key, chunk, P, out_topk_idx, P);
+    snprintf(what, sizeof(what), "%s/select", name);
+    if ((rc = check_launch(what))) return rc;
+  }
+  const long long BR = (long long)B * L * P;
+  p2p_levels_gather_kernel<SOFTMAX><<<(unsigned)((BR * 32 + 255) / 256), 256, 0, st>>>(lv, num_classes, k, point_anchor, pts_gamma,
+                                                                                      img_hw, scale_xy, P, identity ? 1 : 0,
+                                                                                      out_topk_idx, out_pts, out_scores, BR);
+  snprintf(what, sizeof(what), "%s/gather", name);
+  return check_launch(what);
+}
+
+extern "C" int ptb_p2p_decode_topk_levels(const float* const* cls_maps, const float* const* reg_maps, int L, const int32_t* hw,
+                                          const float* strides, int B, int num_classes, int k, const float* point_anchor,
+                                          float pts_gamma, const int32_t* img_hw, const float* scale_xy, int nms_pre,
+                                          int32_t* out_topk_idx, float* out_pts, float* out_scores, void* workspace,
+                                          uint64_t workspace_bytes, void* stream) {
+  return p2p_decode_topk_levels<false>(cls_maps, reg_maps, L, hw, strides, B, num_classes, k, point_anchor, pts_gamma, img_hw,
+                                       scale_xy, nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ptb_p2p_decode_topk_levels_softmax(const float* const* cls_maps, const float* const* reg_maps, int L,
+                                                  const int32_t* hw, const float* strides, int B, int num_classes, int k,
+                                                  const float* point_anchor, float pts_gamma, const int32_t* img_hw,
+                                                  const float* scale_xy, int nms_pre, int32_t* out_topk_idx, float* out_pts,
+                                                  float* out_scores, void* workspace, uint64_t workspace_bytes, void* stream) {
+  return p2p_decode_topk_levels<true>(cls_maps, reg_maps, L, hw, strides, B, num_classes, k, point_anchor, pts_gamma, img_hw,
+                                      scale_xy, nms_pre, out_topk_idx, out_pts, out_scores, workspace, workspace_bytes, stream);
+}
+
 static unsigned cost_matrix_blocks(int n_rows, int n_gt) {
   const long long blocks = ((long long)n_rows * n_gt + 255) / 256, cap = (long long)sm_count() * 8;
   return (unsigned)(blocks > cap ? cap : blocks);
@@ -619,4 +795,25 @@ extern "C" int ptb_mse_fwd_bwd(const float* pred, const float* target, const flo
   PTB_REQUIRE(pred && target && (loss_sum || grad), "NULL input");
   return launch_sum(loss_sum_kernel<MSELoss>, stream, "ptb_mse_fwd_bwd", MSELoss{pred, target, weight, inv_norm}, M * 2, loss_sum,
                     scale, grad);
+}
+
+extern "C" int ptb_smooth_l1_rows_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M,
+                                          const float* row_inv_norm, float beta, float* loss_sum, const float* scale, float* grad,
+                                          void* stream) {
+  PTB_REQUIRE(M >= 0 && beta > 0.f, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(pred && target && row_inv_norm && (loss_sum || grad), "NULL input");
+  using L = PerRowNorm<SmoothL1Loss>;
+  return launch_sum(loss_sum_kernel<L>, stream, "ptb_smooth_l1_rows_fwd_bwd", L{SmoothL1Loss{pred, target, weight, 0.f, beta}, row_inv_norm},
+                    M * 2, loss_sum, scale, grad);
+}
+
+extern "C" int ptb_mse_rows_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, const float* row_inv_norm,
+                                    float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(pred && target && row_inv_norm && (loss_sum || grad), "NULL input");
+  using L = PerRowNorm<MSELoss>;
+  return launch_sum(loss_sum_kernel<L>, stream, "ptb_mse_rows_fwd_bwd", L{MSELoss{pred, target, weight, 0.f}, row_inv_norm}, M * 2,
+                    loss_sum, scale, grad);
 }

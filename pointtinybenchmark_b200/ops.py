@@ -470,8 +470,75 @@ def p2p_decode_topk_softmax(cls_map, reg_map, num_classes, k, point_anchor, stri
     return idx, pts, sc
 
 
-def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img):
-    """ptb_multiclass_nms. pts (B,P,2), scores (B,P,C) -> count (B,), det (B,max,5), label (B,max), keep (B,max), cand_count (B,)"""
+def p2p_chunk_plan(featmap_sizes, k, nms_pre):
+    """Host plan of the multi-level decode (P2PHead._get_bboxes_single, p2p_head.py:355-373).  featmap_sizes [(H_l, W_l)], k anchors.
+    An image's T = sum_l H_l W_l k rows (level-major) are reshaped into L = len(featmap_sizes) equal chunks of T / L rows, so chunk
+    boundaries need not fall on level boundaries; each chunk keeps its top nms_pre rows, or all of them when nms_pre <= 0 or
+    nms_pre >= T / L.  Returns dict(T, L, chunk = T / L, P = rows kept per chunk, level_row0 = [first row of each level] + [T]).
+    Raises RuntimeError when L does not divide T: the reference's reshape raises there (training is unaffected)."""
+    L = len(featmap_sizes)
+    row0 = [0]
+    for h, w in featmap_sizes:
+        row0.append(row0[-1] + int(h) * int(w) * int(k))
+    T = row0[-1]
+    if L < 1 or T % L:
+        raise RuntimeError(f'P2PHead inference over {L} levels: {T} proposals per image (sum of H*W*{k} over the levels) do not '
+                           f'split into {L} equal chunks, which the reference\'s _get_bboxes_single reshapes them into (it raises '
+                           f'there too); pick feature map sizes whose proposal count is a multiple of {L}')
+    chunk = T // L
+    return dict(T=T, L=L, chunk=chunk, P=nms_pre if 0 < nms_pre < chunk else chunk, level_row0=row0)
+
+
+def p2p_decode_topk_levels(cls_maps, reg_maps, strides, num_classes, k, point_anchor, pts_gamma, img_hw, nms_pre, scale_xy=None,
+                           softmax=False):
+    """ptb_p2p_decode_topk_levels(_softmax): decode + per-chunk top-k over L FPN levels.  cls_maps[l] (B,H_l,W_l,k*C1) and
+    reg_maps[l] (B,H_l,W_l,2k) channels-last logits (C1 = C, or C+1 with softmax).  The T = sum_l H_l W_l k rows of an image are cut
+    into L equal chunks (p2p_chunk_plan); each keeps its top nms_pre rows (or all when nms_pre <= 0 or >= T / L).
+    returns topk_idx (B,L*P) int32 chunk-local row indices, pts (B,L*P,2), scores (B,L*P,C), chunk-major."""
+    lib = _lib.load()
+    L = len(cls_maps)
+    if len(reg_maps) != L or len(strides) != L:
+        raise ValueError(f'{L} cls maps, {len(reg_maps)} reg maps and {len(strides)} strides')
+    _chk(point_anchor, torch.float32, 'anchor'); _chk(img_hw, torch.int32, 'img_hw')
+    B = cls_maps[0].shape[0]
+    n_cls = k * (num_classes + 1 if softmax else num_classes)
+    if point_anchor.shape != (k, 2):
+        raise ValueError(f'point_anchor must have shape ({k}, 2), got {tuple(point_anchor.shape)}')
+    if img_hw.shape != (B, 2) or (scale_xy is not None and tuple(scale_xy.shape) != (B, 2)):
+        raise ValueError(f'img_hw (and scale_xy) must have shape ({B}, 2)')
+    if scale_xy is not None:
+        _chk(scale_xy, torch.float32, 'scale_xy')
+    for l, (c, r) in enumerate(zip(cls_maps, reg_maps)):
+        _chk(c, torch.float32, f'cls_maps[{l}]'); _chk(r, torch.float32, f'reg_maps[{l}]')
+        if c.dim() != 4 or tuple(c.shape) != (B, c.shape[1], c.shape[2], n_cls):
+            raise ValueError(f'cls_maps[{l}] must be (B={B}, H, W, {n_cls}) channels-last, got {tuple(c.shape)}')
+        if tuple(r.shape) != (B, c.shape[1], c.shape[2], 2 * k):
+            raise ValueError(f'reg_maps[{l}] must be {(B, c.shape[1], c.shape[2], 2 * k)} like cls_maps[{l}], got {tuple(r.shape)}')
+    hw = [(int(c.shape[1]), int(c.shape[2])) for c in cls_maps]
+    P = p2p_chunk_plan(hw, k, nms_pre)['P']
+    dev = cls_maps[0].device
+    idx = torch.empty((B, L * P), dtype=torch.int32, device=dev)
+    pts = torch.empty((B, L * P, 2), dtype=torch.float32, device=dev)
+    sc = torch.empty((B, L * P, num_classes), dtype=torch.float32, device=dev)
+    hw_arr = (ctypes.c_int32 * (2 * L))(*[v for p in hw for v in p])
+    st_arr = (ctypes.c_float * L)(*[float(s) for s in strides])
+    cls_arr = (ctypes.c_void_p * L)(*[c.data_ptr() for c in cls_maps])
+    reg_arr = (ctypes.c_void_p * L)(*[r.data_ptr() for r in reg_maps])
+    nbytes = lib.ptb_p2p_decode_topk_levels_workspace(B, L, hw_arr, k)
+    ws = torch.empty(max(int(nbytes), 8), dtype=torch.uint8, device=dev)
+    fn, name = ((lib.ptb_p2p_decode_topk_levels_softmax, 'ptb_p2p_decode_topk_levels_softmax') if softmax
+                else (lib.ptb_p2p_decode_topk_levels, 'ptb_p2p_decode_topk_levels'))
+    check(fn(cls_arr, reg_arr, L, hw_arr, st_arr, B, num_classes, k, _ptr(point_anchor), float(pts_gamma), _ptr(img_hw), _ptr(scale_xy),
+             int(nms_pre), _ptr(idx), _ptr(pts), _ptr(sc), _ptr(ws), nbytes, _stream()), name)
+    return idx, pts, sc
+
+
+NMS_WIDE_MAX_POINTS = 8192    # points per image of ptb_multiclass_nms_wide / ptb_multiclass_soft_nms_wide
+
+
+def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img, wide=False):
+    """ptb_multiclass_nms. pts (B,P,2), scores (B,P,C) -> count (B,), det (B,max,5), label (B,max), keep (B,max), cand_count (B,)
+    P <= 4096; wide=True: ptb_multiclass_nms_wide, P <= 8192 (the multi-level P2P head's candidates)."""
     lib = _lib.load()
     _chk(pts, torch.float32, 'pts'); _chk(scores, torch.float32, 'scores')
     B, P, C = scores.shape
@@ -483,9 +550,9 @@ def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img):
     cc = torch.empty((B,), dtype=torch.int32, device=dev)
     nbytes = lib.ptb_multiclass_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    check(lib.ptb_multiclass_nms(_ptr(pts), _ptr(scores), B, P, C, float(pseudo_wh[0]), float(pseudo_wh[1]), float(score_thr),
-                                 float(iou_thr), int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc),
-                                 _ptr(ws), nbytes, _stream()), 'ptb_multiclass_nms')
+    fn, name = (lib.ptb_multiclass_nms_wide, 'ptb_multiclass_nms_wide') if wide else (lib.ptb_multiclass_nms, 'ptb_multiclass_nms')
+    check(fn(_ptr(pts), _ptr(scores), B, P, C, float(pseudo_wh[0]), float(pseudo_wh[1]), float(score_thr), float(iou_thr),
+             int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes, _stream()), name)
     return cnt, det, lab, keep, cc
 
 
@@ -522,9 +589,11 @@ def multiclass_nms_boxes(boxes, scores, score_thr, iou_thr, max_per_img):
 SOFT_NMS_METHODS = {'naive': 0, 'linear': 1, 'gaussian': 2}
 
 
-def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max_per_img, sigma=0.5, min_score=1e-3, method='linear'):
+def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max_per_img, sigma=0.5, min_score=1e-3, method='linear',
+                        wide=False):
     """ptb_multiclass_soft_nms.  pts_or_boxes: (B,P,2) points (pseudo boxes of pseudo_wh) or (B,P,4) boxes; scores (B,P,C).
-    Class-specific boxes (B,P,C,4) go to ptb_multiclass_soft_nms_cls_boxes.
+    Class-specific boxes (B,P,C,4) go to ptb_multiclass_soft_nms_cls_boxes.  P <= 4096; wide=True (points or shared boxes):
+    ptb_multiclass_soft_nms_wide, P <= 8192.
     returns count (B,), det (B,max,5) with DECAYED scores, label, keep, cand_count."""
     lib = _lib.load()
     _chk(pts_or_boxes, torch.float32, 'pts_or_boxes'); _chk(scores, torch.float32, 'scores')
@@ -543,14 +612,16 @@ def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     outs = (SOFT_NMS_METHODS[method], int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes,
             _stream())
+    if cls_boxes and wide:
+        raise ValueError('multiclass_soft_nms: wide=True takes points or shared boxes, not class-specific boxes')
     if cls_boxes:
         name = 'ptb_multiclass_soft_nms_cls_boxes'
         check(lib.ptb_multiclass_soft_nms_cls_boxes(_ptr(pts_or_boxes), _ptr(scores), B, P, C, float(score_thr), float(iou_thr),
                                                     float(sigma), float(min_score), *outs), name)
     else:
-        name = 'ptb_multiclass_soft_nms'
+        name = 'ptb_multiclass_soft_nms_wide' if wide else 'ptb_multiclass_soft_nms'
         wh = pseudo_wh if pseudo_wh is not None else (0.0, 0.0)
-        check(lib.ptb_multiclass_soft_nms(None if is_boxes else _ptr(pts_or_boxes), _ptr(pts_or_boxes) if is_boxes else None,
+        check(getattr(lib, name)(None if is_boxes else _ptr(pts_or_boxes), _ptr(pts_or_boxes) if is_boxes else None,
                                           _ptr(scores), B, P, C, float(wh[0]), float(wh[1]), float(score_thr), float(iou_thr),
                                           float(sigma), float(min_score), *outs), name)
     if method == 'gaussian':              # refused images (count -1): one device read, gaussian only
@@ -765,6 +836,16 @@ def smooth_l1(pred, target, weight, inv_norm, beta, scale=None, want_grad=False)
                      scale, want_grad)
 
 
+def smooth_l1_rows(pred, target, weight, row_inv_norm, beta, scale=None, want_grad=False):
+    """smooth_l1 with one normalisation per row of pred (M, 2): row_inv_norm (M,) = 1 / (stride_m * reg_norm)."""
+    lib = _lib.load()
+    _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target'); _chk(row_inv_norm, torch.float32, 'row_inv_norm')
+    if row_inv_norm.shape != (pred.shape[0],):
+        raise ValueError(f'row_inv_norm must have shape ({pred.shape[0]},), got {tuple(row_inv_norm.shape)}')
+    return _loss_sum(lib.ptb_smooth_l1_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm), float(beta)),
+                     scale, want_grad)
+
+
 def sigmoid_bce(logits, labels, weight, pos_weight=None, scale=None, want_grad=False):
     """sum_m,c binary_cross_entropy_with_logits(logits, onehot(labels), pos_weight) * weight[m] (labels == C: background row);
     optional grad = scale * d/dlogits.  pos_weight (C,) = CrossEntropyLoss.class_weight in sigmoid mode."""
@@ -796,6 +877,15 @@ def mse(pred, target, weight, inv_norm, scale=None, want_grad=False):
     lib = _lib.load()
     _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target')
     return _loss_sum(lib.ptb_mse_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], float(inv_norm)), scale, want_grad)
+
+
+def mse_rows(pred, target, weight, row_inv_norm, scale=None, want_grad=False):
+    """mse with one normalisation per row of pred (M, 2): row_inv_norm (M,) = 1 / (stride_m * reg_norm)."""
+    lib = _lib.load()
+    _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target'); _chk(row_inv_norm, torch.float32, 'row_inv_norm')
+    if row_inv_norm.shape != (pred.shape[0],):
+        raise ValueError(f'row_inv_norm must have shape ({pred.shape[0]},), got {tuple(row_inv_norm.shape)}')
+    return _loss_sum(lib.ptb_mse_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm)), scale, want_grad)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

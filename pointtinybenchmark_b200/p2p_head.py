@@ -60,6 +60,7 @@ MAX_OUT_CHANNELS = 512     # widest output of one wgmma conv launch (ptb_conv_tc
 MAX_CLASSES = 1280         # CPRHead's limit (cpr_head.MAX_CLASSES): the second stage takes every dataset the first one refines
 WIDE_MIN_CLASSES = 257     # the many-class path (cls_out in column slices) starts above 256 classes, where CPRHead's sliced logit map does;
                            # up to 256 classes cls_out must fit one launch, as it always had to
+MAX_LEVELS = 8             # levels of one multi-level decode launch (ptb_p2p_decode_topk_levels)
 LOSS_CLS_TYPES = ('FocalLoss', 'CrossEntropyLoss')
 LOSS_REG_TYPES = ('SmoothL1Loss', 'MSELoss')
 
@@ -87,8 +88,8 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         self.loss_reg_cfg.update(loss_reg or {})
         self.train_cfg = CfgNode(train_cfg) if train_cfg is not None else None
         self.test_cfg = CfgNode(test_cfg) if test_cfg is not None else None
-        if len(self.strides) != 1:
-            raise NotImplementedError('P2PHead: one FPN level only (all configs2/*/p2p configs use strides=[s])')
+        if not 1 <= len(self.strides) <= MAX_LEVELS:
+            raise NotImplementedError(f'P2PHead: {len(self.strides)} FPN levels; the CUDA head takes 1 to {MAX_LEVELS} (strides)')
         # p2p_head.py:63-67: sigmoid scores C classes, softmax C + 1 with the background column last
         self.use_sigmoid_cls = bool(self.loss_cls_cfg.get('use_sigmoid', False))
         if not self.use_sigmoid_cls and self.loss_cls_cfg['type'] == 'FocalLoss':
@@ -185,8 +186,8 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         return self.get_bboxes(*outs, img_metas, rescale=rescale)
 
     # ------------------------------------------------------------------------------------------------
-    def _grid(self, H, W, device):
-        s = float(self.strides[0])
+    def _grid(self, H, W, device, s=None):
+        s = float(self.strides[0]) if s is None else s
         xx = (torch.arange(0., W, device=device) * s).repeat(H)
         yy = (torch.arange(0., H, device=device) * s).view(-1, 1).repeat(1, W).view(-1)
         return xx, yy
@@ -214,6 +215,46 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         valid = torch.stack(vflag).to(dev)[:, :, None].expand(B, H * W, k).reshape(B, -1)
         return anchor.reshape(B, -1, 2), pred.reshape(B, -1, 2), valid, cls
 
+    @torch.autocast('cuda', enabled=False)
+    def get_pred_points_levels(self, cls_outs, pts_outs, img_metas):
+        """p2p_head.py:125-170 over L >= 2 levels: each level as get_pred_points with its own stride, the rows concatenated
+        level-major (cell-major, anchor-minor inside a level), as the reference's torch.cat of the flattened maps orders them."""
+        B = cls_outs[0].shape[0]
+        k, C = self.num_points, self.num_cls_out
+        dev = cls_outs[0].device
+        if len(cls_outs) != len(self.strides) or len(pts_outs) != len(self.strides):
+            raise ValueError(f'P2PHead has {len(self.strides)} strides but got {len(cls_outs)} cls maps and {len(pts_outs)} pts maps')
+        anchors, preds, clss, vflag = [], [], [], [[] for _ in img_metas]
+        for cls_out, pts_out, s in zip(cls_outs, pts_outs, self.strides):
+            s = float(s)
+            _, _, H, W = cls_out.shape
+            clss.append(ops.to_nhwc(cls_out).reshape(B, H * W * k, C))
+            reg = ops.to_nhwc(pts_out).reshape(B, H * W, k, 2)
+            xx, yy = self._grid(H, W, dev, s)
+            anchor = torch.stack([xx, yy], -1)[None, :, None, :] + (self.point_anchor.to(dev) * s)[None, None]
+            anchor = anchor.expand(B, H * W, k, 2)
+            preds.append((anchor + reg * self.pts_gamma * s).reshape(B, -1, 2))
+            anchors.append(anchor.reshape(B, -1, 2))
+            for b, m in enumerate(img_metas):
+                ph, pw = m['pad_shape'][:2]
+                vh, vw = min(int(np.ceil(ph / s)), H), min(int(np.ceil(pw / s)), W)
+                v = torch.zeros(H, W, dtype=torch.bool)
+                v[:vh, :vw] = True
+                vflag[b].append(v.reshape(-1))
+        self._valid_host = [torch.cat(v) for v in vflag]
+        valid = torch.stack(self._valid_host).to(dev)[:, :, None].expand(B, -1, k).reshape(B, -1)
+        return torch.cat(anchors, 1), torch.cat(preds, 1), valid, torch.cat(clss, 1)
+
+    def row_inv_norm(self, featmap_sizes, device):
+        """(Q,) fp32 1 / (stride_q * reg_norm) of every proposal row of get_pred_points_levels (p2p_head.py:234-240 divides each row
+        by its own stride, column 2 of pred_pts).  Depends on the map sizes only: built once per size set and device."""
+        key = (tuple(tuple(int(v) for v in hw) for hw in featmap_sizes), str(device))
+        if getattr(self, '_row_inv_cache', (None,))[0] != key:
+            inv = torch.cat([torch.full((int(h) * int(w) * self.num_points,), 1.0 / (float(s) * self.reg_norm))
+                             for (h, w), s in zip(featmap_sizes, self.strides)])
+            self._row_inv_cache = (key, inv.to(device))
+        return self._row_inv_cache[1]
+
     def loss(self, cls_outs, pts_outs, gt_bboxes, gt_labels, img_metas, gt_bboxes_ignore=None):
         """p2p_head.py:172-248 -> dict(loss_cls=[B], loss_pts=[B])."""
         cls_out, pts_out = cls_outs[0], pts_outs[0]
@@ -222,13 +263,17 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         for gb in gt_bboxes:                       # p2p_head.py:183-184: the reference refuses images without a GT point
             assert len(gb) > 0, gt_bboxes
         dev = cls_out.device
-        anchor, pred, valid, cls = self.get_pred_points(cls_out, pts_out, img_metas)
+        multi = len(self.strides) > 1
+        if multi:
+            anchor, pred, valid, cls = self.get_pred_points_levels(cls_outs, pts_outs, img_metas)
+        else:
+            anchor, pred, valid, cls = self.get_pred_points(cls_out, pts_out, img_metas)
         B, Q, C = cls.shape
         s = float(self.strides[0])
         prop = (anchor if self.assign_before_pred else pred).detach().contiguous()
         a = self.assign
         # ---- cost matrices and the Hungarian matching on the GPU: no cost.cpu(), no scipy (hungarian_assigner.py:229-270)
-        key = (tuple(cls_out.shape[-2:]), tuple(tuple(m['pad_shape'][:2]) for m in img_metas), str(dev))
+        key = (tuple(tuple(c.shape[-2:]) for c in cls_outs), tuple(tuple(m['pad_shape'][:2]) for m in img_metas), str(dev))
         if getattr(self, '_ridx_cache', (None,))[0] != key:           # valid-row lists depend on the map size and pad shapes only
             valid_host = torch.stack(self._valid_host)[:, :, None].expand(B, valid.shape[1] // self.num_points, self.num_points).reshape(B, -1)
             ridx_l = [torch.nonzero(valid_host[b]).squeeze(1).int() for b in range(B)]
@@ -289,10 +334,13 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             cls_op, cls_args = ops.sigmoid_focal, (self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25))
         else:
             cls_op, cls_args = (ops.sigmoid_bce if self.use_sigmoid_cls else ops.softmax_ce), (cw,)
+        if multi:        # p2p_head.py:234-240: every row divided by its own level's stride
+            row_inv = self.row_inv_norm([c.shape[-2:] for c in cls_outs], dev)
         if reg_type == 'MSELoss':
-            reg_op, reg_args = ops.mse, (inv_norm,)
+            reg_op, reg_args = (ops.mse_rows, (row_inv,)) if multi else (ops.mse, (inv_norm,))
         else:
-            reg_op, reg_args = ops.smooth_l1, (inv_norm, self.loss_reg_cfg.get('beta', 1.0))
+            beta = self.loss_reg_cfg.get('beta', 1.0)
+            reg_op, reg_args = (ops.smooth_l1_rows, (row_inv, beta)) if multi else (ops.smooth_l1, (inv_norm, beta))
         loss_cls, loss_pts = [], []
         for b in range(B):
             lc = _LossSumFn.apply(cls_op, cls[b].contiguous(), labels_l[b], lw_l[b], *cls_args)
@@ -318,21 +366,36 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         scale_xy = None
         if rescale:
             scale_xy = torch.tensor(np.array([m['scale_factor'][:2] for m in img_metas], dtype=np.float32), device=dev)
-        cmap, rmap = ops.to_nhwc(cls_out).contiguous(), ops.to_nhwc(pts_out).contiguous()
-        # p2p_head.py:363-372: sigmoid scores, or the softmax over C+1 columns of which NMS sees the C foreground ones
-        decode = ops.p2p_decode_topk if self.use_sigmoid_cls else ops.p2p_decode_topk_softmax
-        idx, pts, scores = decode(cmap, rmap, self.num_classes, self.num_points, self.point_anchor.to(dev), self.strides[0],
-                                  self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
+        multi = len(self.strides) > 1
+        if multi:
+            plan = ops.p2p_chunk_plan([c.shape[-2:] for c in cls_outs], self.num_points, cfg.get('nms_pre', -1))
+            if plan['L'] * plan['P'] > ops.NMS_WIDE_MAX_POINTS:
+                raise RuntimeError(
+                    f"P2PHead over {plan['L']} levels: nms_pre={cfg.get('nms_pre', -1)} keeps {plan['P']} of the {plan['chunk']} rows of "
+                    f"each of the {plan['L']} chunks, {plan['L'] * plan['P']} NMS points per image; the NMS takes at most "
+                    f"{ops.NMS_WIDE_MAX_POINTS}: set test_cfg.nms_pre to at most {ops.NMS_WIDE_MAX_POINTS // plan['L']}")
+            # p2p_head.py:355-381: the level-major rows cut into len(strides) equal chunks, top nms_pre per chunk (ops.p2p_chunk_plan);
+            # up to 8192 candidates go to NMS
+            idx, pts, scores = ops.p2p_decode_topk_levels(
+                [ops.to_nhwc(c).contiguous() for c in cls_outs], [ops.to_nhwc(p).contiguous() for p in pts_outs], self.strides,
+                self.num_classes, self.num_points, self.point_anchor.to(dev), self.pts_gamma, img_hw, cfg.get('nms_pre', -1),
+                scale_xy, softmax=not self.use_sigmoid_cls)
+        else:
+            cmap, rmap = ops.to_nhwc(cls_out).contiguous(), ops.to_nhwc(pts_out).contiguous()
+            # p2p_head.py:363-372: sigmoid scores, or the softmax over C+1 columns of which NMS sees the C foreground ones
+            decode = ops.p2p_decode_topk if self.use_sigmoid_cls else ops.p2p_decode_topk_softmax
+            idx, pts, scores = decode(cmap, rmap, self.num_classes, self.num_points, self.point_anchor.to(dev), self.strides[0],
+                                      self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
         wh = cfg.get('pseudo_wh', (16, 16))
         nms = cfg.get('nms')
         check_split_thr(nms)
         if nms.get('type', 'nms') == 'soft_nms':       # batched_nms dispatches on nms_cfg['type'] (mmcv/ops/nms.py)
             cnt, det, lab, keep, cc = ops.multiclass_soft_nms(pts, scores, wh, cfg.get('score_thr'), nms.get('iou_threshold', 0.3),
                                                               cfg.get('max_per_img'), nms.get('sigma', 0.5),
-                                                              nms.get('min_score', 1e-3), nms.get('method', 'linear'))
+                                                              nms.get('min_score', 1e-3), nms.get('method', 'linear'), wide=multi)
         elif nms.get('type', 'nms') == 'nms':
             cnt, det, lab, keep, cc = ops.multiclass_nms(pts, scores, wh, cfg.get('score_thr'), _iou_of(nms),
-                                                         cfg.get('max_per_img'))
+                                                         cfg.get('max_per_img'), wide=multi)
         else:
             raise NotImplementedError(f"nms type {nms.get('type')}")
         cnt_h = cnt.cpu().tolist()
