@@ -499,6 +499,41 @@ int ptb_smooth_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target
                                void* stream);
 int ptb_mse_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
                          const float* row_inv_norm /*[M]*/, float* loss_sum, const float* scale, float* grad, void* stream);
+/* P2PHead's other point losses on the normalised points d = (pred - target) * row_inv_norm[m], same conventions:
+ *   ptb_l1_rows_fwd_bwd           L1Loss (smooth_l1_loss.py:33-45): sum |d| * weight; the gradient of |d| is 0 at d == 0
+ *   ptb_balanced_l1_rows_fwd_bwd  BalancedL1Loss (balanced_l1_loss.py:12-49) with its alpha, gamma, beta */
+int ptb_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
+                        const float* row_inv_norm /*[M]*/, float* loss_sum, const float* scale, float* grad, void* stream);
+int ptb_balanced_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
+                                 const float* row_inv_norm /*[M]*/, float alpha, float gamma, float beta, float* loss_sum,
+                                 const float* scale, float* grad, void* stream);
+/* GHM-C and GHM-R (ghm_loss.py:21-172) as P2PHead calls them, one image at a time, in two steps, all on the device:
+ *   ptb_ghm{c,r}_bin_weights  over a batch of B images: counts[b][i] (i < bins) = valid elements of image b whose gradient length g
+ *                             lies in [edges[i], edges[i+1]) (edges nondecreasing), counts[b][bins] = valid elements; then, image by
+ *                             image in order, tot[b] = max(counts[b][bins], 1) and the per-bin element weights bin_weight[b][i] =
+ *                             (tot / cnt_i) / n, or with momentum > 0 (tot / acc_sum[i]) / n after the in-place update
+ *                             acc_sum[i] = momentum * acc_sum[i] + (1 - momentum) * cnt_i of every non-empty bin; n = non-empty bins.
+ *                             GHMC: g = |sigmoid(x) - t| over B x Q x C logits, t = one-hot(labels) (label outside [0, C): zero row),
+ *                             valid = label_weight[b][q] > 0.  GHMR: g = |d / sqrt(d^2 + mu^2)|, valid = weight > 0.
+ *   ptb_ghm{c,r}_fwd_bwd      one image: loss_sum += sum of the element losses times their bin's weight (GHMC: binary cross-entropy
+ *                             with logits, GHMR: sqrt(d^2 + mu^2) - mu); with grad != NULL the gradient scale * d sum / d input instead.
+ * At most PTB_GHM_MAX_BINS bins. */
+#define PTB_GHM_MAX_BINS 256
+int ptb_ghmc_bin_weights(const float* logits /*[B][Q][C]*/, const int64_t* labels /*[B][Q], ==C: background*/,
+                         const float* label_weight /*[B][Q]*/, int B, int64_t Q, int num_classes, const float* edges /*[bins+1]*/,
+                         int bins, double momentum, float* acc_sum /*[bins], NULL without momentum*/, int32_t* counts /*[B][bins+1]*/,
+                         float* bin_weight /*[B][bins]*/, float* tot /*[B]*/, void* stream);
+int ptb_ghmc_fwd_bwd(const float* logits /*[Q][C]*/, const int64_t* labels /*[Q]*/, const float* label_weight /*[Q]*/, int64_t Q,
+                     int num_classes, const float* edges /*[bins+1]*/, int bins, const float* bin_weight /*[bins]*/, float* loss_sum,
+                     const float* scale, float* grad /*[Q][C] or NULL*/, void* stream);
+int ptb_ghmr_bin_weights(const float* pred /*[B][Q][2]*/, const float* target, const float* weight /*[B][Q][2]*/,
+                         const float* row_inv_norm /*[Q]*/, float mu, int B, int64_t Q, const float* edges /*[bins+1]*/, int bins,
+                         double momentum, float* acc_sum /*[bins] or NULL*/, int32_t* counts /*[B][bins+1]*/,
+                         float* bin_weight /*[B][bins]*/, float* tot /*[B]*/, void* stream);
+int ptb_ghmr_fwd_bwd(const float* pred /*[Q][2]*/, const float* target, const float* weight /*[Q][2]*/, int64_t Q,
+                     const float* row_inv_norm /*[Q]*/, float mu, const float* edges /*[bins+1]*/, int bins,
+                     const float* bin_weight /*[bins]*/, float* loss_sum, const float* scale, float* grad /*[Q][2] or NULL*/,
+                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Conv towers on the tensor cores — replace the cuDNN calls behind CPRHead.forward_single / P2PHead.forward_single

@@ -11,7 +11,8 @@ LIB_PATH = os.path.join(_HERE, 'libptb_b200.so')
 _lib = None
 MISSING = []
 
-c_int, c_float, c_void_p, c_u64, c_i64 = ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int64
+c_int, c_float, c_void_p, c_u64, c_i64, c_double = ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int64, \
+    ctypes.c_double
 
 
 class RefineCfg(ctypes.Structure):
@@ -97,6 +98,12 @@ SIGNATURES = {
     'ptb_mse_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, P, P, P, P]),
     'ptb_sigmoid_bce_cw_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
     'ptb_softmax_ce_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
+    'ptb_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, P, P, P, P]),
+    'ptb_balanced_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, c_float, c_float, P, P, P, P]),
+    'ptb_ghmc_bin_weights': (c_int, [P, P, P, c_int, c_i64, c_int, P, c_int, c_double, P, P, P, P, P]),
+    'ptb_ghmc_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, c_int, P, P, P, P, P]),
+    'ptb_ghmr_bin_weights': (c_int, [P, P, P, P, c_float, c_int, c_i64, P, c_int, c_double, P, P, P, P, P]),
+    'ptb_ghmr_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, P, c_int, P, P, P, P, P]),
     'ptb_split_tf32': (c_int, [P, c_i64, P, P, P]),
     'ptb_conv3x3_pack_weight': (c_int, [P, c_int, c_int, P, P, P]),
     'ptb_conv3x3_c256_tf32x3': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P, P]),

@@ -22,7 +22,10 @@ StreamScratch* stream_scratch(void* stream) {
   auto it = g_scratch.find(key);
   if (it != g_scratch.end()) return it->second;
   StreamScratch* p = nullptr;
-  if (cudaMalloc(&p, sizeof(StreamScratch)) != cudaSuccess || cudaMemset(p, 0, sizeof(StreamScratch)) != cudaSuccess) {
+  // zeroed on the stream that owns the block: a plain cudaMemset of device memory is queued on the legacy default stream, which a
+  // non-blocking stream's first kernel does not wait for
+  if (cudaMalloc(&p, sizeof(StreamScratch)) != cudaSuccess ||
+      cudaMemsetAsync(p, 0, sizeof(StreamScratch), (cudaStream_t)stream) != cudaSuccess) {
     cudaGetLastError();
     fail("%s", "stream_scratch: cudaMalloc / cudaMemset of the per-stream scratch block failed");
     return nullptr;

@@ -817,3 +817,270 @@ extern "C" int ptb_mse_rows_fwd_bwd(const float* pred, const float* target, cons
   return launch_sum(loss_sum_kernel<L>, stream, "ptb_mse_rows_fwd_bwd", L{MSELoss{pred, target, weight, 0.f}, row_inv_norm}, M * 2,
                     loss_sum, scale, grad);
 }
+
+// ------------------------------------------------------------------------------------------------
+// GHM-C / GHM-R (ghm_loss.py:21-172), L1Loss (smooth_l1_loss.py:33-45) and BalancedL1Loss (balanced_l1_loss.py:12-49)
+// ------------------------------------------------------------------------------------------------
+// GHM runs in three launches over a batch of B images and nothing returns to the host:
+//   1. ghm_hist_kernel: per (image, chunk) CTA, integer shared-memory counts of the valid elements per gradient-length bin, added to
+//      the image's global counts with integer atomics (the same counts in any order);
+//   2. ghm_weights_kernel: one thread walks the images in order and forms, with the reference's fp32 operation order, the image's
+//      tot, its number of non-empty bins n, its per-bin weights and the in-place momentum update of acc_sum;
+//   3. the loss pass per image (loss_sum_kernel with GHMCLoss / GHMRLoss): the element's bin again, its weight, the loss term into the
+//      fixed-order sum, and with grad the gradient in the same launch.  Its backward reuses the bin weights of step 2.
+// Bins are [edges[i], edges[i+1]) on fp32 g, as `(g >= edges[i]) & (g < edges[i+1])`; edges must be nondecreasing (the head checks a
+// loaded buffer), so an element lies in at most one bin: the last i with edges[i] <= g, if g < edges[i+1].
+namespace ptb {
+
+__device__ __forceinline__ int ghm_bin(float g, const float* edges, int bins) {
+  int lo = 0, hi = bins + 1;                // first index with edges[idx] > g, in [0, bins + 1]; a NaN g finds 0: no bin
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (edges[mid] <= g) lo = mid + 1; else hi = mid;
+  }
+  const int i = lo - 1;
+  return (i >= 0 && i < bins && g < edges[i + 1]) ? i : -1;
+}
+
+// g of GHM-C: |sigmoid(x) - t| with ATen's CPU sigmoid bits (sigmoidf_acc)
+struct GHMCGrad {
+  const float* x; const int64_t* labels; const float* label_weight; long long Q; int C;
+  __device__ __forceinline__ float operator()(int b, long long e, bool& valid) const {
+    const long long m = e / C;
+    const int c = (int)(e - m * C);
+    valid = label_weight[b * Q + m] > 0.f;
+    const float t = labels[b * Q + m] == c ? 1.f : 0.f;
+    return fabsf(__fsub_rn(sigmoidf_acc(x[b * Q * C + e]), t));
+  }
+};
+
+// GHM-R's normalised difference and g = |d / sqrt(mu^2 + d^2)| (mu2 = fp32(mu * mu), the reference's python-float square)
+__device__ __forceinline__ float ghmr_diff(float p, float t, float inv) { return (p - t) * inv; }
+__device__ __forceinline__ float ghmr_root(float d, float mu2) { return __fsqrt_rn(__fadd_rn(__fmul_rn(d, d), mu2)); }
+
+struct GHMRGrad {
+  const float* pred; const float* target; const float* weight; const float* row_inv_norm; long long Q; float mu2;
+  __device__ __forceinline__ float operator()(int b, long long e, bool& valid) const {
+    const long long o = b * Q * 2 + e;
+    valid = weight[o] > 0.f;
+    const float d = ghmr_diff(pred[o], target[o], row_inv_norm[e >> 1]);
+    return fabsf(__fdiv_rn(d, ghmr_root(d, mu2)));
+  }
+};
+
+constexpr int GHM_HIST_ITEMS = 8;        // elements per thread and CTA sweep before the grid strides
+
+// counts[b][i] (i < bins) = valid elements of image b in bin i; counts[b][bins] = valid elements of image b.  The warp aggregates
+// equal bins (__match_any_sync) before the shared atomics: most of GHM-C's elements share the lowest bin.
+template <class G>
+__global__ void __launch_bounds__(256)
+ghm_hist_kernel(G gf, long long n, const float* __restrict__ edges, int bins, int* __restrict__ counts) {
+  __shared__ float se[PTB_GHM_MAX_BINS + 1];
+  __shared__ int sc[PTB_GHM_MAX_BINS + 1];
+  const int b = blockIdx.y, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i <= bins; i += 256) { se[i] = edges[i]; sc[i] = 0; }
+  __syncthreads();
+  int nvalid = 0;
+  for (long long base = (long long)blockIdx.x * 256; base < n; base += (long long)gridDim.x * 256) {
+    const long long e = base + threadIdx.x;
+    int key = -2;                                   // -2: out of range or invalid, -1: valid but in no bin
+    if (e < n) {
+      bool valid;
+      const float g = gf(b, e, valid);
+      if (valid) { key = ghm_bin(g, se, bins); ++nvalid; }
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, key);
+    if (key >= 0 && lane == __ffs(peers) - 1) atomicAdd(&sc[key], __popc(peers));
+  }
+  nvalid = warp_sum_int(nvalid);
+  if (lane == 0 && nvalid) atomicAdd(&sc[bins], nvalid);
+  __syncthreads();
+  for (int i = threadIdx.x; i <= bins; i += 256)
+    if (sc[i]) atomicAdd(&counts[(long long)b * (bins + 1) + i], sc[i]);
+}
+
+// ghm_loss.py:76-90 / 154-168 per image, images in order.  tot = max(valid, 1) (GHM-R: the sum of its 0/1 point weights, the same
+// count); exact while a count stays below 2^24, as the reference's fp32 sum is.  Without momentum w_i = fp32(tot / cnt_i) in double
+// (python floats); with it acc_i = fp32(mmt) * acc_i + fp32((1 - mmt) * cnt_i), w_i = (1 / acc_i) * tot (python's float / tensor is
+// reciprocal() * other).  Then w_i / n in fp32.  Empty bins weigh 0.
+__global__ void ghm_weights_kernel(const int* __restrict__ counts, int B, int bins, double mmt, float* __restrict__ acc_sum,
+                                   float* __restrict__ bin_weight, float* __restrict__ tot) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  for (int b = 0; b < B; ++b) {
+    const int* cb = counts + (long long)b * (bins + 1);
+    const float t = fmaxf((float)cb[bins], 1.f);
+    int nb = 0;
+    for (int i = 0; i < bins; ++i) nb += cb[i] > 0;
+    for (int i = 0; i < bins; ++i) {
+      float w = 0.f;
+      if (cb[i] > 0) {
+        if (mmt > 0.0) {
+          acc_sum[i] = __fadd_rn(__fmul_rn((float)mmt, acc_sum[i]), (float)((1.0 - mmt) * (double)cb[i]));
+          w = __fmul_rn(__frcp_rn(acc_sum[i]), t);
+        } else {
+          w = (float)((double)t / (double)cb[i]);
+        }
+        w = __fdiv_rn(w, (float)nb);
+      }
+      bin_weight[(long long)b * bins + i] = w;
+    }
+    tot[b] = t;
+  }
+}
+
+template <class G>
+static int ghm_bin_weights(const char* name, G gf, int B, long long n, const float* edges, int bins, double momentum, float* acc_sum,
+                           int* counts, float* bin_weight, float* tot, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (cudaMemsetAsync(counts, 0, sizeof(int) * (size_t)B * (bins + 1), st) != cudaSuccess) return fail("%s: cudaMemsetAsync failed", name);
+  if (n > 0) {
+    const long long per_cta = 256LL * GHM_HIST_ITEMS;
+    const long long want = (n + per_cta - 1) / per_cta, cap = (4LL * sm_count() + B - 1) / B;
+    const dim3 grid((unsigned)(want < cap ? want : cap), (unsigned)B);
+    ghm_hist_kernel<G><<<grid, 256, 0, st>>>(gf, n, edges, bins, counts);
+    int rc = check_launch(name);
+    if (rc) return rc;
+  }
+  ghm_weights_kernel<<<1, 32, 0, st>>>(counts, B, bins, momentum, acc_sum, bin_weight, tot);
+  return check_launch(name);
+}
+
+// GHMC's loss pass over one image's Q x C logits: binary_cross_entropy_with_logits(x, t, weights, reduction='sum') in ATen's CPU form
+// ((1 - t) x - log_sigmoid(x), times the element weight); d/dx = (sigmoid(x) - t) * weight.
+struct GHMCLoss {
+  const float* x; const int64_t* labels; const float* label_weight; int C; const float* edges; int bins; const float* bin_weight;
+  __device__ __forceinline__ float operator()(long long e, bool want_loss, float* grad, float sc) const {
+    const long long m = e / C;
+    const int c = (int)(e - m * C);
+    const float t = labels[m] == c ? 1.f : 0.f;
+    const float v = x[e];
+    const float p = sigmoidf_acc(v);
+    float w = 0.f;
+    if (label_weight[m] > 0.f) {
+      const int i = ghm_bin(fabsf(__fsub_rn(p, t)), edges, bins);
+      if (i >= 0) w = bin_weight[i];
+    }
+    if (grad) grad[e] = sc * w * (p - t);
+    if (!want_loss) return 0.f;
+    const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
+    return __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
+  }
+};
+
+// GHMR's loss pass over one image's (Q, 2) points: (sqrt(d^2 + mu^2) - mu) * weight; d/dpred = d / sqrt(d^2 + mu^2) * inv * weight
+struct GHMRLoss {
+  const float* pred; const float* target; const float* weight; const float* row_inv_norm; float mu, mu2; const float* edges; int bins;
+  const float* bin_weight;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
+    const float inv = row_inv_norm[e >> 1];
+    const float d = ghmr_diff(pred[e], target[e], inv);
+    const float r = ghmr_root(d, mu2);
+    float w = 0.f;
+    if (weight[e] > 0.f) {
+      const int i = ghm_bin(fabsf(__fdiv_rn(d, r)), edges, bins);
+      if (i >= 0) w = bin_weight[i];
+    }
+    if (grad) grad[e] = sc * w * inv * (d / r);
+    return (r - mu) * w;
+  }
+};
+
+// L1Loss on the normalised points: |d| * weight; d/dpred = sign(d) * inv * weight, 0 at d == 0 as ATen's abs backward (a NaN d keeps
+// its NaN gradient)
+struct L1RowsLoss {
+  const float* pred; const float* target; const float* weight; const float* row_inv_norm;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
+    const float inv = row_inv_norm[e >> 1];
+    const float w = weight ? weight[e] : 1.f;
+    const float d = (pred[e] - target[e]) * inv;
+    if (grad) grad[e] = sc * w * inv * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f * d));
+    return fabsf(d) * w;
+  }
+};
+
+// BalancedL1Loss on the normalised points, a = |d|, b = e^(gamma / alpha) - 1 (kb = fp32(b), kab = fp32(alpha / b)):
+//   a < beta:  kab (kb a + 1) log(kb a / beta + 1) - alpha a;   else gamma a + gamma / b - alpha beta.
+// d/da = kab kb log(u) + kab (kb a + 1) kb / (beta u) - alpha with u = kb a / beta + 1, or gamma; times sign(d) (0 at 0) * inv * weight.
+struct BalancedL1RowsLoss {
+  const float* pred; const float* target; const float* weight; const float* row_inv_norm; float alpha, gamma, beta, kb, kab, kgb;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
+    const float inv = row_inv_norm[e >> 1];
+    const float w = weight ? weight[e] : 1.f;
+    const float d = (pred[e] - target[e]) * inv;
+    const float a = fabsf(d);
+    const bool in = a < beta;
+    const float u = kb * a / beta + 1.f;
+    if (grad) {
+      const float da = in ? kab * kb * logf(u) + kab * (kb * a + 1.f) * kb / (beta * u) - alpha : gamma;
+      grad[e] = sc * w * inv * da * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f * d));
+    }
+    return (in ? kab * (kb * a + 1.f) * logf(u) - alpha * a : gamma * a + kgb - alpha * beta) * w;
+  }
+};
+
+}  // namespace ptb
+
+extern "C" int ptb_ghmc_bin_weights(const float* logits, const int64_t* labels, const float* label_weight, int B, int64_t Q,
+                                    int num_classes, const float* edges, int bins, double momentum, float* acc_sum, int32_t* counts,
+                                    float* bin_weight, float* tot, void* stream) {
+  PTB_REQUIRE(B > 0 && Q >= 0 && num_classes > 0 && Q * num_classes < (1LL << 31), "shape (Q x num_classes must stay below 2^31)");
+  PTB_REQUIRE(bins >= 1 && bins <= PTB_GHM_MAX_BINS, "GHMC bins must lie in [1, PTB_GHM_MAX_BINS]");
+  PTB_REQUIRE(logits && labels && label_weight && edges && counts && bin_weight && tot && (momentum <= 0.0 || acc_sum), "NULL input");
+  return ghm_bin_weights("ptb_ghmc_bin_weights", GHMCGrad{logits, labels, label_weight, Q, num_classes}, B, Q * num_classes, edges,
+                         bins, momentum, acc_sum, counts, bin_weight, tot, stream);
+}
+
+extern "C" int ptb_ghmc_fwd_bwd(const float* logits, const int64_t* labels, const float* label_weight, int64_t Q, int num_classes,
+                                const float* edges, int bins, const float* bin_weight, float* loss_sum, const float* scale, float* grad,
+                                void* stream) {
+  PTB_REQUIRE(Q >= 0 && num_classes > 0 && bins >= 1 && bins <= PTB_GHM_MAX_BINS, "shape");
+  if (Q == 0) return 0;
+  PTB_REQUIRE(logits && labels && label_weight && edges && bin_weight && (loss_sum || grad), "NULL input");
+  return launch_sum(loss_sum_kernel<GHMCLoss>, stream, "ptb_ghmc_fwd_bwd",
+                    GHMCLoss{logits, labels, label_weight, num_classes, edges, bins, bin_weight}, Q * num_classes, loss_sum, scale, grad);
+}
+
+extern "C" int ptb_ghmr_bin_weights(const float* pred, const float* target, const float* weight, const float* row_inv_norm, float mu,
+                                    int B, int64_t Q, const float* edges, int bins, double momentum, float* acc_sum, int32_t* counts,
+                                    float* bin_weight, float* tot, void* stream) {
+  PTB_REQUIRE(B > 0 && Q >= 0 && Q < (1LL << 30), "shape");
+  PTB_REQUIRE(bins >= 1 && bins <= PTB_GHM_MAX_BINS, "GHMR bins must lie in [1, PTB_GHM_MAX_BINS]");
+  PTB_REQUIRE(pred && target && weight && row_inv_norm && edges && counts && bin_weight && tot && (momentum <= 0.0 || acc_sum),
+              "NULL input");
+  const float mu2 = (float)((double)mu * (double)mu);
+  return ghm_bin_weights("ptb_ghmr_bin_weights", GHMRGrad{pred, target, weight, row_inv_norm, Q, mu2}, B, Q * 2, edges, bins, momentum,
+                         acc_sum, counts, bin_weight, tot, stream);
+}
+
+extern "C" int ptb_ghmr_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t Q, const float* row_inv_norm,
+                                float mu, const float* edges, int bins, const float* bin_weight, float* loss_sum, const float* scale,
+                                float* grad, void* stream) {
+  PTB_REQUIRE(Q >= 0 && bins >= 1 && bins <= PTB_GHM_MAX_BINS, "shape");
+  if (Q == 0) return 0;
+  PTB_REQUIRE(pred && target && weight && row_inv_norm && edges && bin_weight && (loss_sum || grad), "NULL input");
+  const float mu2 = (float)((double)mu * (double)mu);
+  return launch_sum(loss_sum_kernel<GHMRLoss>, stream, "ptb_ghmr_fwd_bwd",
+                    GHMRLoss{pred, target, weight, row_inv_norm, mu, mu2, edges, bins, bin_weight}, Q * 2, loss_sum, scale, grad);
+}
+
+extern "C" int ptb_l1_rows_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M, const float* row_inv_norm,
+                                   float* loss_sum, const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0, "shape");
+  if (M == 0) return 0;
+  PTB_REQUIRE(pred && target && row_inv_norm && (loss_sum || grad), "NULL input");
+  return launch_sum(loss_sum_kernel<L1RowsLoss>, stream, "ptb_l1_rows_fwd_bwd", L1RowsLoss{pred, target, weight, row_inv_norm}, M * 2,
+                    loss_sum, scale, grad);
+}
+
+extern "C" int ptb_balanced_l1_rows_fwd_bwd(const float* pred, const float* target, const float* weight, int64_t M,
+                                            const float* row_inv_norm, float alpha, float gamma, float beta, float* loss_sum,
+                                            const float* scale, float* grad, void* stream) {
+  PTB_REQUIRE(M >= 0 && alpha > 0.f && beta > 0.f, "shape (alpha and beta must be positive)");
+  if (M == 0) return 0;
+  PTB_REQUIRE(pred && target && row_inv_norm && (loss_sum || grad), "NULL input");
+  const double b = exp((double)gamma / (double)alpha) - 1.0;
+  return launch_sum(loss_sum_kernel<BalancedL1RowsLoss>, stream, "ptb_balanced_l1_rows_fwd_bwd",
+                    BalancedL1RowsLoss{pred, target, weight, row_inv_norm, alpha, gamma, beta, (float)b, (float)((double)alpha / b),
+                                       (float)((double)gamma / b)},
+                    M * 2, loss_sum, scale, grad);
+}

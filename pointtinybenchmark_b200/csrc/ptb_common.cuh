@@ -42,7 +42,7 @@ inline int check_launch(const char* what) {
 // per-(device, stream) scratch: self-resetting scheduler tickets / "last block" counters and block partials of the fixed-order
 // reductions.  Launches on ONE stream are serialised, and the last block of every fixed-order sum resets `done` before its
 // kernel ends, so one SumScratch serves every sum kernel of the stream; a block per stream keeps concurrent launches on
-// different streams apart.  Allocated lazily (cudaMalloc + memset, once per stream) by capi.cu; ptb_reset_stream_state()
+// different streams apart.  Allocated lazily (cudaMalloc + cudaMemsetAsync on its stream, once per stream) by capi.cu; ptb_reset_stream_state()
 // zeroes it after an aborted launch.
 // ---------------------------------------------------------------------------------------------
 constexpr int SCRATCH_BLOCKS = 528;      // 4 x 132 (H100 SMs): grid of the fixed-order sum kernels

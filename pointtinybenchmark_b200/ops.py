@@ -888,6 +888,102 @@ def mse_rows(pred, target, weight, row_inv_norm, scale=None, want_grad=False):
     return _loss_sum(lib.ptb_mse_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm)), scale, want_grad)
 
 
+def _check_rows(pred, target, row_inv_norm):
+    _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target'); _chk(row_inv_norm, torch.float32, 'row_inv_norm')
+    if pred.shape[-1] != 2 or target.shape != pred.shape:
+        raise ValueError(f'pred and target must be (..., Q, 2) of one shape, got {tuple(pred.shape)} and {tuple(target.shape)}')
+    if row_inv_norm.shape != (pred.shape[-2],):
+        raise ValueError(f'row_inv_norm must have shape ({pred.shape[-2]},), got {tuple(row_inv_norm.shape)}')
+
+
+def l1_rows(pred, target, weight, row_inv_norm, scale=None, want_grad=False):
+    """sum |(pred - target) * row_inv_norm[m]| * weight over (M, 2) points (L1Loss); optional grad = scale * d/dpred."""
+    lib = _lib.load()
+    _check_rows(pred, target, row_inv_norm)
+    return _loss_sum(lib.ptb_l1_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm)), scale, want_grad)
+
+
+def balanced_l1_rows(pred, target, weight, row_inv_norm, alpha, gamma, beta, scale=None, want_grad=False):
+    """BalancedL1Loss(alpha, gamma, beta) summed over (M, 2) normalised points times weight; optional grad = scale * d/dpred."""
+    lib = _lib.load()
+    _check_rows(pred, target, row_inv_norm)
+    return _loss_sum(lib.ptb_balanced_l1_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm),
+                                                              float(alpha), float(gamma), float(beta)), scale, want_grad)
+
+
+def _check_edges(edges, acc_sum, momentum):
+    _chk(edges, torch.float32, 'edges')
+    bins = edges.numel() - 1
+    if not 1 <= bins <= GHM_MAX_BINS:
+        raise ValueError(f'GHM takes 1 to {GHM_MAX_BINS} bins (PTB_GHM_MAX_BINS), got {bins}')
+    if momentum > 0:
+        _chk(acc_sum, torch.float32, 'acc_sum')
+        if acc_sum.shape != (bins,):
+            raise ValueError(f'acc_sum must have shape ({bins},), got {tuple(acc_sum.shape)}')
+    return bins
+
+
+def _ghm_outputs(B, bins, dev):
+    return (torch.empty((B, bins + 1), dtype=torch.int32, device=dev), torch.empty((B, bins), dtype=torch.float32, device=dev),
+            torch.empty((B,), dtype=torch.float32, device=dev))
+
+
+GHM_MAX_BINS = 256        # PTB_GHM_MAX_BINS: the edges and counts of a bin histogram live in shared memory
+
+
+def ghmc_bin_weights(logits, labels, label_weight, edges, momentum=0.0, acc_sum=None):
+    """GHMC's histogram and weight step over a batch (B, Q, C) of logits, labels (B, Q) (== C: background) and label_weight (B, Q).
+    Returns counts (B, bins + 1) int32 (the last column: valid elements), bin_weight (B, bins) and tot (B,), all on the device; with
+    momentum > 0 acc_sum (bins,) is updated in place, image by image."""
+    lib = _lib.load()
+    _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels'); _chk(label_weight, torch.float32, 'label_weight')
+    B, Q, C = logits.shape
+    if labels.shape != (B, Q) or label_weight.shape != (B, Q):
+        raise ValueError(f'labels and label_weight must be ({B}, {Q})')
+    bins = _check_edges(edges, acc_sum, momentum)
+    counts, bw, tot = _ghm_outputs(B, bins, logits.device)
+    check(lib.ptb_ghmc_bin_weights(_ptr(logits), _ptr(labels), _ptr(label_weight), B, Q, C, _ptr(edges), bins, float(momentum),
+                                   _ptr(acc_sum if momentum > 0 else None), _ptr(counts), _ptr(bw), _ptr(tot), _stream()),
+          'ptb_ghmc_bin_weights')
+    return counts, bw, tot
+
+
+def ghmc(logits, labels, label_weight, edges, bin_weight, scale=None, want_grad=False):
+    """one image's GHMC sum: sum_q,c BCE-with-logits(logits, onehot(labels)) * bin_weight[bin(q, c)] over valid elements (not yet
+    divided by tot); optional grad = scale * d/dlogits.  bin_weight (bins,) is ghmc_bin_weights' row for this image."""
+    lib = _lib.load()
+    _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels'); _chk(bin_weight, torch.float32, 'bin_weight')
+    Q, C = logits.shape
+    bins = _check_edges(edges, None, 0)
+    return _loss_sum(lib.ptb_ghmc_fwd_bwd, logits, (_ptr(labels), _ptr(label_weight), Q, C, _ptr(edges), bins, _ptr(bin_weight)),
+                     scale, want_grad)
+
+
+def ghmr_bin_weights(pred, target, weight, row_inv_norm, mu, edges, momentum=0.0, acc_sum=None):
+    """GHMR's histogram and weight step over a batch of (B, Q, 2) points (d = (pred - target) * row_inv_norm[q]) and weights; returns
+    and updates as ghmc_bin_weights."""
+    lib = _lib.load()
+    _check_rows(pred, target, row_inv_norm); _chk(weight, torch.float32, 'weight')
+    B, Q, _ = pred.shape
+    if weight.shape != pred.shape:
+        raise ValueError(f'weight must have shape {tuple(pred.shape)}, got {tuple(weight.shape)}')
+    bins = _check_edges(edges, acc_sum, momentum)
+    counts, bw, tot = _ghm_outputs(B, bins, pred.device)
+    check(lib.ptb_ghmr_bin_weights(_ptr(pred), _ptr(target), _ptr(weight), _ptr(row_inv_norm), float(mu), B, Q, _ptr(edges), bins,
+                                   float(momentum), _ptr(acc_sum if momentum > 0 else None), _ptr(counts), _ptr(bw), _ptr(tot),
+                                   _stream()), 'ptb_ghmr_bin_weights')
+    return counts, bw, tot
+
+
+def ghmr(pred, target, weight, row_inv_norm, mu, edges, bin_weight, scale=None, want_grad=False):
+    """one image's GHMR sum: sum (sqrt(d^2 + mu^2) - mu) * bin_weight[bin] over valid (Q, 2) elements; optional grad = scale * d/dpred."""
+    lib = _lib.load()
+    _check_rows(pred, target, row_inv_norm); _chk(bin_weight, torch.float32, 'bin_weight')
+    bins = _check_edges(edges, None, 0)
+    return _loss_sum(lib.ptb_ghmr_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm), float(mu), _ptr(edges),
+                                                  bins, _ptr(bin_weight)), scale, want_grad)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # conv towers on the tensor cores (3xTF32 implicit GEMM + GroupNorm + ReLU)
 # ----------------------------------------------------------------------------------------------------------------------

@@ -38,8 +38,9 @@ def _iou_of(nms_cfg):
 
 
 class _LossSumFn(torch.autograd.Function):
-    """op(x, *args)[0] for a fused loss of ops (sigmoid_focal, sigmoid_bce, softmax_ce, smooth_l1, mse), differentiable in x: the
-    backward is op's gradient launch, op(x, *args, scale=g, want_grad=True)."""
+    """op(x, *args)[0] for a fused loss of ops (sigmoid_focal, sigmoid_bce, softmax_ce, ghmc, smooth_l1, mse, l1_rows, balanced_l1_rows,
+    ghmr), differentiable in x: the backward is op's gradient launch, op(x, *args, scale=g, want_grad=True), with the tensors the
+    forward saw (GHM: the bin weights of the forward step, not ones recomputed from an updated acc_sum)."""
 
     @staticmethod
     def forward(ctx, op, x, *args):
@@ -61,8 +62,50 @@ MAX_CLASSES = 1280         # CPRHead's limit (cpr_head.MAX_CLASSES): the second 
 WIDE_MIN_CLASSES = 257     # the many-class path (cls_out in column slices) starts above 256 classes, where CPRHead's sliced logit map does;
                            # up to 256 classes cls_out must fit one launch, as it always had to
 MAX_LEVELS = 8             # levels of one multi-level decode launch (ptb_p2p_decode_topk_levels)
-LOSS_CLS_TYPES = ('FocalLoss', 'CrossEntropyLoss')
-LOSS_REG_TYPES = ('SmoothL1Loss', 'MSELoss')
+LOSS_CLS_TYPES = ('FocalLoss', 'CrossEntropyLoss', 'GHMC')
+LOSS_REG_TYPES = ('SmoothL1Loss', 'MSELoss', 'GHMR', 'L1Loss', 'BalancedL1Loss')
+# the mmdet defaults of the losses added after the first four (ghm_loss.py, smooth_l1_loss.py, balanced_l1_loss.py); a config of one
+# of them takes these, not the defaults the head fills in for the others
+LOSS_DEFAULTS = {'GHMC': dict(bins=10, momentum=0, use_sigmoid=True, loss_weight=1.0),
+                 'GHMR': dict(mu=0.02, bins=10, momentum=0, loss_weight=1.0),
+                 'L1Loss': dict(reduction='mean', loss_weight=1.0),
+                 'BalancedL1Loss': dict(alpha=0.5, gamma=1.5, beta=1.0, reduction='mean', loss_weight=1.0)}
+# losses of the reference tree that cannot run on P2PHead's (labels, label_weights) / (points, point_weights) targets
+UNSUPPORTED_LOSSES = {
+    'VarifocalLoss': 'it takes soft IoU-aware score targets of the logits\' shape; P2PHead\'s targets are integer labels '
+                     '(the reference fails its pred.size() == target.size() assertion)',
+    'QualityFocalLoss': 'it takes a (labels, quality scores) target pair; P2PHead passes labels only (the reference fails its '
+                        'len(target) == 2 assertion)',
+    'SeesawLoss': 'it needs num_classes + 2 softmax columns (an objectness pair); P2PHead has num_classes or num_classes + 1',
+    **{t: 'it compares boxes; P2PHead regresses points' for t in ('IoULoss', 'BoundedIoULoss', 'GIoULoss', 'DIoULoss', 'CIoULoss')}}
+
+
+class GHMBuffers(nn.Module):
+    """The state of GHMC / GHMR (ghm_loss.py:35-48, 113-124): the bin `edges` buffer and, with momentum > 0, `acc_sum`, under the
+    reference's names (loss_cls.edges, loss_cls.acc_sum, loss_reg.*), so its checkpoints load with strict=True.  The loss reads
+    `edges` from the buffer; a loaded set must be nondecreasing (the kernels' bins are disjoint)."""
+
+    def __init__(self, bins, momentum, last_edge):
+        super().__init__()
+        if not 1 <= int(bins) <= ops.GHM_MAX_BINS:
+            raise NotImplementedError(f'P2PHead: GHM bins={bins}; the CUDA histogram takes 1 to {ops.GHM_MAX_BINS} bins')
+        self.bins, self.momentum = int(bins), float(momentum)
+        edges = torch.arange(self.bins + 1).float() / self.bins
+        if last_edge is None:
+            edges[-1] += 1e-6           # GHMC
+        else:
+            edges[-1] = last_edge       # GHMR: 1e3
+        self.register_buffer('edges', edges)
+        if self.momentum > 0:
+            self.register_buffer('acc_sum', torch.zeros(self.bins))
+        else:
+            self.acc_sum = None
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
+        e = state_dict.get(prefix + 'edges')
+        if e is not None and e.numel() > 1 and bool((e[1:] < e[:-1]).any()):
+            raise ValueError(f'{prefix}edges must be nondecreasing, got {e.tolist()}')
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
 
 @register_head
@@ -86,12 +129,27 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         self.loss_cls_cfg.update(loss_cls or {})
         self.loss_reg_cfg = dict(type='MSELoss', loss_weight=2e-4)
         self.loss_reg_cfg.update(loss_reg or {})
+        if self.loss_cls_cfg['type'] in LOSS_DEFAULTS:
+            self.loss_cls_cfg = dict(LOSS_DEFAULTS[self.loss_cls_cfg['type']], **loss_cls)
+        if self.loss_reg_cfg['type'] in LOSS_DEFAULTS:
+            self.loss_reg_cfg = dict(LOSS_DEFAULTS[self.loss_reg_cfg['type']], **loss_reg)
+        for c in (self.loss_cls_cfg, self.loss_reg_cfg):
+            if c['type'] in ('L1Loss', 'BalancedL1Loss') and c['reduction'] != 'mean':
+                raise NotImplementedError(f"P2PHead: {c['type']}(reduction={c['reduction']!r}); the head averages the point loss over "
+                                          f"the positives, which mmdet does for reduction='mean' only")
         self.train_cfg = CfgNode(train_cfg) if train_cfg is not None else None
         self.test_cfg = CfgNode(test_cfg) if test_cfg is not None else None
         if not 1 <= len(self.strides) <= MAX_LEVELS:
             raise NotImplementedError(f'P2PHead: {len(self.strides)} FPN levels; the CUDA head takes 1 to {MAX_LEVELS} (strides)')
         # p2p_head.py:63-67: sigmoid scores C classes, softmax C + 1 with the background column last
         self.use_sigmoid_cls = bool(self.loss_cls_cfg.get('use_sigmoid', False))
+        if self.loss_cls_cfg['type'] == 'GHMC':
+            if not self.loss_cls_cfg['use_sigmoid']:
+                raise NotImplementedError('P2PHead: GHMC supports use_sigmoid=True only (ghm_loss.py raises NotImplementedError '
+                                          'for the softmax form)')
+            # p2p_head.py:63 reads use_sigmoid from the config as written (default False): a GHMC config without it makes a
+            # softmax head of num_classes + 1 columns, whose background label then fills the last column of GHMC's one-hot
+            self.use_sigmoid_cls = bool(loss_cls.get('use_sigmoid', False))
         if not self.use_sigmoid_cls and self.loss_cls_cfg['type'] == 'FocalLoss':
             raise NotImplementedError('P2PHead: FocalLoss supports sigmoid classification only (use_sigmoid=True)')
         self.num_cls_out = num_classes if self.use_sigmoid_cls else num_classes + 1
@@ -129,6 +187,10 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             if a.get('type') != 'HungarianAssignerV2':
                 raise NotImplementedError(f"assigner {a.get('type')}")
             self.assign = dict(terms=match_cost_terms(a.get('cls_costs'), a.get('reg_costs')), topk_k=a.get('topk_k', 1))
+        if self.loss_cls_cfg['type'] == 'GHMC':
+            self.loss_cls = GHMBuffers(self.loss_cls_cfg['bins'], self.loss_cls_cfg['momentum'], None)
+        if self.loss_reg_cfg['type'] == 'GHMR':
+            self.loss_reg = GHMBuffers(self.loss_reg_cfg['bins'], self.loss_reg_cfg['momentum'], 1e3)
         self._init_packed_hooks()
         self.check_assign_status = True      # read the (B,) status of the matching kernel each step (scipy's ValueErrors)
 
@@ -257,6 +319,12 @@ class P2PHead(PackedWeightsMixin, nn.Module):
 
     def loss(self, cls_outs, pts_outs, gt_bboxes, gt_labels, img_metas, gt_bboxes_ignore=None):
         """p2p_head.py:172-248 -> dict(loss_cls=[B], loss_pts=[B])."""
+        cls_type, reg_type = self.loss_cls_cfg['type'], self.loss_reg_cfg['type']
+        for t in (cls_type, reg_type):
+            if t in UNSUPPORTED_LOSSES:
+                raise NotImplementedError(f'P2PHead cannot train with {t}: {UNSUPPORTED_LOSSES[t]}')
+        if cls_type not in LOSS_CLS_TYPES or reg_type not in LOSS_REG_TYPES:
+            raise NotImplementedError(f'P2PHead: loss_cls must be one of {LOSS_CLS_TYPES} and loss_reg one of {LOSS_REG_TYPES}')
         cls_out, pts_out = cls_outs[0], pts_outs[0]
         if not cls_out.is_cuda:
             raise RuntimeError('P2PHead runs on CUDA tensors only; there is no CPU fallback')
@@ -323,9 +391,6 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             pw = pos.float()[:, None].expand(Q, 2).contiguous()
             labels_l.append(labels); lw_l.append(lw.contiguous()); gp_l.append(gp.contiguous()); pw_l.append(pw)
         num_total_pos = sum([(p[:, 0] > 0).sum() for p in pw_l]).float()
-        cls_type, reg_type = self.loss_cls_cfg['type'], self.loss_reg_cfg['type']
-        if cls_type not in LOSS_CLS_TYPES or reg_type not in LOSS_REG_TYPES:
-            raise NotImplementedError(f'P2PHead: loss_cls must be one of {LOSS_CLS_TYPES} and loss_reg one of {LOSS_REG_TYPES}')
         # loss_single (p2p_head.py:220-231): CrossEntropyLoss averages over every proposal of the batch, FocalLoss over the positives
         cls_avg = float(B * Q) if cls_type == 'CrossEntropyLoss' else num_total_pos
         inv_norm = 1.0 / (s * self.reg_norm)
@@ -334,19 +399,48 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             cls_op, cls_args = ops.sigmoid_focal, (self.loss_cls_cfg.get('gamma', 2.0), self.loss_cls_cfg.get('alpha', 0.25))
         else:
             cls_op, cls_args = (ops.sigmoid_bce if self.use_sigmoid_cls else ops.softmax_ce), (cw,)
-        if multi:        # p2p_head.py:234-240: every row divided by its own level's stride
+        # p2p_head.py:234-240: every row divided by its own level's stride (the losses added with GHM take the per-row form at
+        # any level count)
+        if multi or reg_type in ('GHMR', 'L1Loss', 'BalancedL1Loss'):
             row_inv = self.row_inv_norm([c.shape[-2:] for c in cls_outs], dev)
+        rc = self.loss_reg_cfg
         if reg_type == 'MSELoss':
             reg_op, reg_args = (ops.mse_rows, (row_inv,)) if multi else (ops.mse, (inv_norm,))
+        elif reg_type == 'L1Loss':
+            reg_op, reg_args = ops.l1_rows, (row_inv,)
+        elif reg_type == 'BalancedL1Loss':
+            reg_op, reg_args = ops.balanced_l1_rows, (row_inv, rc['alpha'], rc['gamma'], rc['beta'])
         else:
-            beta = self.loss_reg_cfg.get('beta', 1.0)
+            beta = rc.get('beta', 1.0)
             reg_op, reg_args = (ops.smooth_l1_rows, (row_inv, beta)) if multi else (ops.smooth_l1, (inv_norm, beta))
+        self._last_ghm = {}
+        # GHMC / GHMR (ghm_loss.py:50-94, 127-172), called per image by loss_single: the batch's histograms and bin weights in one
+        # step (momentum: acc_sum updated image by image, in the forward pass), then each image's sum over its tot with the bin
+        # weights that step made, which _LossSumFn keeps for the backward.  avg_factor is not used.
+        if cls_type == 'GHMC':
+            x_all, m = cls.contiguous(), self.loss_cls
+            counts, cls_bw, cls_tot = ops.ghmc_bin_weights(x_all.detach(), torch.stack(labels_l), torch.stack(lw_l), m.edges,
+                                                           m.momentum, m.acc_sum)
+            self._last_ghm['cls_counts'] = counts
+        if reg_type == 'GHMR':
+            p_all, m = pred.contiguous(), self.loss_reg
+            counts, reg_bw, reg_tot = ops.ghmr_bin_weights(p_all.detach(), torch.stack(gp_l), torch.stack(pw_l), row_inv, rc['mu'],
+                                                           m.edges, m.momentum, m.acc_sum)
+            self._last_ghm['reg_counts'] = counts
         loss_cls, loss_pts = [], []
         for b in range(B):
-            lc = _LossSumFn.apply(cls_op, cls[b].contiguous(), labels_l[b], lw_l[b], *cls_args)
-            loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / cls_avg)
-            lp = _LossSumFn.apply(reg_op, pred[b].contiguous(), gp_l[b], pw_l[b], *reg_args)
-            loss_pts.append(self.loss_reg_cfg.get('loss_weight', 1.0) * lp / num_total_pos)
+            if cls_type == 'GHMC':
+                lc = _LossSumFn.apply(ops.ghmc, x_all[b], labels_l[b], lw_l[b], self.loss_cls.edges, cls_bw[b])
+                loss_cls.append(lc / cls_tot[b] * self.loss_cls_cfg['loss_weight'])
+            else:
+                lc = _LossSumFn.apply(cls_op, cls[b].contiguous(), labels_l[b], lw_l[b], *cls_args)
+                loss_cls.append(self.loss_cls_cfg.get('loss_weight', 1.0) * lc / cls_avg)
+            if reg_type == 'GHMR':
+                lp = _LossSumFn.apply(ops.ghmr, p_all[b], gp_l[b], pw_l[b], row_inv, rc['mu'], self.loss_reg.edges, reg_bw[b])
+                loss_pts.append(lp / reg_tot[b] * rc['loss_weight'])
+            else:
+                lp = _LossSumFn.apply(reg_op, pred[b].contiguous(), gp_l[b], pw_l[b], *reg_args)
+                loss_pts.append(rc.get('loss_weight', 1.0) * lp / num_total_pos)
         self._last_targets = dict(labels=labels_l, label_weights=lw_l, gt_pts=gp_l, pts_weights=pw_l)
         return dict(loss_cls=loss_cls, loss_pts=loss_pts)
 
