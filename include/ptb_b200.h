@@ -500,8 +500,10 @@ int ptb_smooth_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target
 int ptb_mse_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
                          const float* row_inv_norm /*[M]*/, float* loss_sum, const float* scale, float* grad, void* stream);
 /* P2PHead's other point losses on the normalised points d = (pred - target) * row_inv_norm[m], same conventions:
- *   ptb_l1_rows_fwd_bwd           L1Loss (smooth_l1_loss.py:33-45): sum |d| * weight; the gradient of |d| is 0 at d == 0
- *   ptb_balanced_l1_rows_fwd_bwd  BalancedL1Loss (balanced_l1_loss.py:12-49) with its alpha, gamma, beta */
+ *   ptb_l1_rows_fwd_bwd           L1Loss (smooth_l1_loss.py:33-45): sum |d| * weight; the gradient of |d| is sgn(d), 0 at d == 0
+ *                                 and at a NaN d, as torch's
+ *   ptb_balanced_l1_rows_fwd_bwd  BalancedL1Loss (balanced_l1_loss.py:12-49) with its alpha, gamma, beta; alpha > 0, beta > 0 and
+ *                                 gamma != 0 (b = e^(gamma / alpha) - 1 divides the loss), else it returns an error */
 int ptb_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
                         const float* row_inv_norm /*[M]*/, float* loss_sum, const float* scale, float* grad, void* stream);
 int ptb_balanced_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* target, const float* weight /*[M][2] or NULL*/, int64_t M,
@@ -515,6 +517,9 @@ int ptb_balanced_l1_rows_fwd_bwd(const float* pred /*[M][2]*/, const float* targ
  *                             acc_sum[i] = momentum * acc_sum[i] + (1 - momentum) * cnt_i of every non-empty bin; n = non-empty bins.
  *                             GHMC: g = |sigmoid(x) - t| over B x Q x C logits, t = one-hot(labels) (label outside [0, C): zero row),
  *                             valid = label_weight[b][q] > 0.  GHMR: g = |d / sqrt(d^2 + mu^2)|, valid = weight > 0.
+ *                             tot counts the valid elements.  For GHMR the reference sums the weights instead: the two agree for
+ *                             P2PHead's 0/1 point weights, not for fractional ones.  Above 2^24 valid elements tot is the count
+ *                             rounded to fp32, which can differ by one ulp from the reference's fp32 sum.
  *   ptb_ghm{c,r}_fwd_bwd      one image: loss_sum += sum of the element losses times their bin's weight (GHMC: binary cross-entropy
  *                             with logits, GHMR: sqrt(d^2 + mu^2) - mu); with grad != NULL the gradient scale * d sum / d input instead.
  * At most PTB_GHM_MAX_BINS bins. */

@@ -899,8 +899,9 @@ ghm_hist_kernel(G gf, long long n, const float* __restrict__ edges, int bins, in
     if (sc[i]) atomicAdd(&counts[(long long)b * (bins + 1) + i], sc[i]);
 }
 
-// ghm_loss.py:76-90 / 154-168 per image, images in order.  tot = max(valid, 1) (GHM-R: the sum of its 0/1 point weights, the same
-// count); exact while a count stays below 2^24, as the reference's fp32 sum is.  Without momentum w_i = fp32(tot / cnt_i) in double
+// ghm_loss.py:76-90 / 154-168 per image, images in order.  tot = max(valid, 1) (GHM-R: the number of points with weight > 0, which is
+// the reference's sum of its weights for the head's 0/1 point weights) is the exact count rounded once to fp32.  The reference sums
+// the valid mask in fp32: the same value while the count stays below 2^24, within one ulp above it.  Without momentum w_i = fp32(tot / cnt_i) in double
 // (python floats); with it acc_i = fp32(mmt) * acc_i + fp32((1 - mmt) * cnt_i), w_i = (1 / acc_i) * tot (python's float / tensor is
 // reciprocal() * other).  Then w_i / n in fp32.  Empty bins weigh 0.
 __global__ void ghm_weights_kernel(const int* __restrict__ counts, int B, int bins, double mmt, float* __restrict__ acc_sum,
@@ -985,15 +986,15 @@ struct GHMRLoss {
   }
 };
 
-// L1Loss on the normalised points: |d| * weight; d/dpred = sign(d) * inv * weight, 0 at d == 0 as ATen's abs backward (a NaN d keeps
-// its NaN gradient)
+// L1Loss on the normalised points: |d| * weight; d/dpred = sgn(d) * inv * weight.  ATen's abs backward multiplies by sgn(d), which is
+// 0 at d == 0 and at a NaN d, so a NaN difference has gradient 0 (its loss term is NaN)
 struct L1RowsLoss {
   const float* pred; const float* target; const float* weight; const float* row_inv_norm;
   __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
     const float inv = row_inv_norm[e >> 1];
     const float w = weight ? weight[e] : 1.f;
     const float d = (pred[e] - target[e]) * inv;
-    if (grad) grad[e] = sc * w * inv * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f * d));
+    if (grad) grad[e] = sc * w * inv * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
     return fabsf(d) * w;
   }
 };
@@ -1076,6 +1077,8 @@ extern "C" int ptb_balanced_l1_rows_fwd_bwd(const float* pred, const float* targ
                                             const float* row_inv_norm, float alpha, float gamma, float beta, float* loss_sum,
                                             const float* scale, float* grad, void* stream) {
   PTB_REQUIRE(M >= 0 && alpha > 0.f && beta > 0.f, "shape (alpha and beta must be positive)");
+  // b = e^(gamma / alpha) - 1 divides the loss: mmdet raises at gamma == 0, and a NaN gamma makes every term NaN
+  PTB_REQUIRE(gamma != 0.f && gamma == gamma, "gamma must be non-zero and not NaN (b = e^(gamma / alpha) - 1 must not be 0)");
   if (M == 0) return 0;
   PTB_REQUIRE(pred && target && row_inv_norm && (loss_sum || grad), "NULL input");
   const double b = exp((double)gamma / (double)alpha) - 1.0;

@@ -888,25 +888,40 @@ def mse_rows(pred, target, weight, row_inv_norm, scale=None, want_grad=False):
     return _loss_sum(lib.ptb_mse_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm)), scale, want_grad)
 
 
-def _check_rows(pred, target, row_inv_norm):
+def _chk_shape(t, dtype, name, shape):
+    """_chk and an exact shape: the kernels index these tensors by the sizes of the others"""
+    _chk(t, dtype, name)
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f'{name} must have shape {tuple(shape)}, got {tuple(t.shape)}')
+    return t
+
+
+def _check_rows(pred, target, row_inv_norm, ndim=None):
     _chk(pred, torch.float32, 'pred'); _chk(target, torch.float32, 'target'); _chk(row_inv_norm, torch.float32, 'row_inv_norm')
+    if ndim is not None and pred.dim() != ndim:
+        raise ValueError(f'pred must have {ndim} dimensions, got shape {tuple(pred.shape)}')
     if pred.shape[-1] != 2 or target.shape != pred.shape:
         raise ValueError(f'pred and target must be (..., Q, 2) of one shape, got {tuple(pred.shape)} and {tuple(target.shape)}')
     if row_inv_norm.shape != (pred.shape[-2],):
         raise ValueError(f'row_inv_norm must have shape ({pred.shape[-2]},), got {tuple(row_inv_norm.shape)}')
 
 
+def _check_point_weight(weight, pred):
+    if weight is not None:
+        _chk_shape(weight, torch.float32, 'weight', pred.shape)
+
+
 def l1_rows(pred, target, weight, row_inv_norm, scale=None, want_grad=False):
     """sum |(pred - target) * row_inv_norm[m]| * weight over (M, 2) points (L1Loss); optional grad = scale * d/dpred."""
     lib = _lib.load()
-    _check_rows(pred, target, row_inv_norm)
+    _check_rows(pred, target, row_inv_norm, 2); _check_point_weight(weight, pred)
     return _loss_sum(lib.ptb_l1_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm)), scale, want_grad)
 
 
 def balanced_l1_rows(pred, target, weight, row_inv_norm, alpha, gamma, beta, scale=None, want_grad=False):
     """BalancedL1Loss(alpha, gamma, beta) summed over (M, 2) normalised points times weight; optional grad = scale * d/dpred."""
     lib = _lib.load()
-    _check_rows(pred, target, row_inv_norm)
+    _check_rows(pred, target, row_inv_norm, 2); _check_point_weight(weight, pred)
     return _loss_sum(lib.ptb_balanced_l1_rows_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm),
                                                               float(alpha), float(gamma), float(beta)), scale, want_grad)
 
@@ -937,6 +952,8 @@ def ghmc_bin_weights(logits, labels, label_weight, edges, momentum=0.0, acc_sum=
     momentum > 0 acc_sum (bins,) is updated in place, image by image."""
     lib = _lib.load()
     _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels'); _chk(label_weight, torch.float32, 'label_weight')
+    if logits.dim() != 3:
+        raise ValueError(f'logits must be (B, Q, C), got shape {tuple(logits.shape)}')
     B, Q, C = logits.shape
     if labels.shape != (B, Q) or label_weight.shape != (B, Q):
         raise ValueError(f'labels and label_weight must be ({B}, {Q})')
@@ -952,9 +969,13 @@ def ghmc(logits, labels, label_weight, edges, bin_weight, scale=None, want_grad=
     """one image's GHMC sum: sum_q,c BCE-with-logits(logits, onehot(labels)) * bin_weight[bin(q, c)] over valid elements (not yet
     divided by tot); optional grad = scale * d/dlogits.  bin_weight (bins,) is ghmc_bin_weights' row for this image."""
     lib = _lib.load()
-    _chk(logits, torch.float32, 'logits'); _chk(labels, torch.int64, 'labels'); _chk(bin_weight, torch.float32, 'bin_weight')
+    _chk(logits, torch.float32, 'logits')
+    if logits.dim() != 2:
+        raise ValueError(f'logits must be (Q, C), got shape {tuple(logits.shape)}')
     Q, C = logits.shape
     bins = _check_edges(edges, None, 0)
+    _chk_shape(labels, torch.int64, 'labels', (Q,)); _chk_shape(label_weight, torch.float32, 'label_weight', (Q,))
+    _chk_shape(bin_weight, torch.float32, 'bin_weight', (bins,))
     return _loss_sum(lib.ptb_ghmc_fwd_bwd, logits, (_ptr(labels), _ptr(label_weight), Q, C, _ptr(edges), bins, _ptr(bin_weight)),
                      scale, want_grad)
 
@@ -963,7 +984,7 @@ def ghmr_bin_weights(pred, target, weight, row_inv_norm, mu, edges, momentum=0.0
     """GHMR's histogram and weight step over a batch of (B, Q, 2) points (d = (pred - target) * row_inv_norm[q]) and weights; returns
     and updates as ghmc_bin_weights."""
     lib = _lib.load()
-    _check_rows(pred, target, row_inv_norm); _chk(weight, torch.float32, 'weight')
+    _check_rows(pred, target, row_inv_norm, 3); _chk(weight, torch.float32, 'weight')
     B, Q, _ = pred.shape
     if weight.shape != pred.shape:
         raise ValueError(f'weight must have shape {tuple(pred.shape)}, got {tuple(weight.shape)}')
@@ -978,8 +999,9 @@ def ghmr_bin_weights(pred, target, weight, row_inv_norm, mu, edges, momentum=0.0
 def ghmr(pred, target, weight, row_inv_norm, mu, edges, bin_weight, scale=None, want_grad=False):
     """one image's GHMR sum: sum (sqrt(d^2 + mu^2) - mu) * bin_weight[bin] over valid (Q, 2) elements; optional grad = scale * d/dpred."""
     lib = _lib.load()
-    _check_rows(pred, target, row_inv_norm); _chk(bin_weight, torch.float32, 'bin_weight')
+    _check_rows(pred, target, row_inv_norm, 2); _chk_shape(weight, torch.float32, 'weight', pred.shape)
     bins = _check_edges(edges, None, 0)
+    _chk_shape(bin_weight, torch.float32, 'bin_weight', (bins,))
     return _loss_sum(lib.ptb_ghmr_fwd_bwd, pred, (_ptr(target), _ptr(weight), pred.shape[0], _ptr(row_inv_norm), float(mu), _ptr(edges),
                                                   bins, _ptr(bin_weight)), scale, want_grad)
 

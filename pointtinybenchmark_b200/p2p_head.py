@@ -137,6 +137,13 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             if c['type'] in ('L1Loss', 'BalancedL1Loss') and c['reduction'] != 'mean':
                 raise NotImplementedError(f"P2PHead: {c['type']}(reduction={c['reduction']!r}); the head averages the point loss over "
                                           f"the positives, which mmdet does for reduction='mean' only")
+        rc = self.loss_reg_cfg
+        if rc['type'] == 'BalancedL1Loss':
+            # balanced_l1_loss.py divides by b = e^(gamma / alpha) - 1 and by beta
+            a, g, be = float(rc['alpha']), float(rc['gamma']), float(rc['beta'])
+            if not (a > 0 and be > 0 and g == g and g != 0):
+                raise ValueError(f'P2PHead: BalancedL1Loss(alpha={a}, gamma={g}, beta={be}); alpha and beta must be positive and gamma '
+                                 f'non-zero (b = e^(gamma / alpha) - 1 divides the loss; mmdet raises ZeroDivisionError at gamma=0)')
         self.train_cfg = CfgNode(train_cfg) if train_cfg is not None else None
         self.test_cfg = CfgNode(test_cfg) if test_cfg is not None else None
         if not 1 <= len(self.strides) <= MAX_LEVELS:
