@@ -674,6 +674,44 @@ int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, int ld_dy, co
 uint64_t ptb_col_sum_workspace(int64_t M, int N);
 int ptb_col_sum(const float* y /*[M][ld]*/, int64_t M, int N, int ld, float* workspace, float* out /*[N]*/, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * RPN training (SURVEY.md §8f rank 4, BASELINE.json configs[3]): AnchorHead.get_targets / loss (anchor_head.py:171-267, 269-365,
+ * 422-482) with RandomSampler (random_sampler.py:31-80) for B images of L levels, A anchors per cell, N = sum_l H_l W_l A anchors
+ * per image in the reference's flat (level, y, x, anchor) order.  featmap_hw [L][2] = (H, W), strides [L][2] = (sx, sy), host arrays.
+ *   ptb_rpn_inside_anchors   inside_box [B][L][A] int32 (x0, x1, y0, y1): anchor (l, y, x, a) of image b is inside iff
+ *                            x0 <= x < x1 and y0 <= y < y1 (the host restates valid_flags and anchor_inside_flags as these boxes).
+ *                            Writes the inside anchors compacted in flat order (inside_anchors [B][N][4], the first n_inside[b] rows
+ *                            of each image), inside_idx [B][N] (the anchor's row there, -1 outside) and n_inside [B].
+ *   ptb_rpn_candidate_ranks  gt_inds [B][N] (MaxIoUAssigner's result on image b's first n_inside[b] rows): rank [B][N] = the row's
+ *                            rank among the image's positives (gt_inds > 0) or negatives (== 0), -1 for ignored rows, and
+ *                            counts [B][2] = (positives, negatives).
+ *   plan                     int32: [B][2] x (offset, count) for the positives and the negatives of each image, then the sampled ranks
+ *                            of each (image, kind) ascending at plan[offset ...]; count -1: every candidate is sampled.
+ *   ptb_rpn_anchor_targets   the reference's unmapped targets in the layout of the output maps: labels (int64; 0 foreground, 1
+ *                            background) and label_weights like cls_score [B][A][H][W], bbox_targets and bbox_weights like
+ *                            bbox_pred [B][4A][H][W], one level after the other.  gt_bboxes: the images' GTs concatenated, image b's
+ *                            at rows [gt_off[b], gt_off[b+1]).  A sampled positive gets pos_weight (> 0) or 1 as label weight.
+ *   ptb_rpn_sampled_indices  one image (plan of B = 1): pos_inds / neg_inds = the sampled rows, ascending (SamplingResult).
+ *   ptb_rpn_level_loss       one level's sums of CrossEntropyLoss(use_sigmoid=True) over M = B*A*H*W logits (loss_sum[0]) and of
+ *                            L1Loss / SmoothL1Loss(beta) over the 4M box deltas (loss_sum[1]), weighted, un-normalised, fixed-order;
+ *                            or (loss_sum NULL) the gradients scale[0] * d/dcls_score and scale[1] * d/dbbox_pred in the maps' layout. */
+#define PTB_RPN_MAX_LEVELS 8
+#define PTB_RPN_LOSS_L1 0
+#define PTB_RPN_LOSS_SMOOTH_L1 1
+int ptb_rpn_inside_anchors(const float* base_anchors /*[L][A][4]*/, const int32_t* featmap_hw, const int32_t* strides, int L, int A, int B,
+                           const int32_t* inside_box, float* inside_anchors, int32_t* inside_idx, int32_t* n_inside, void* stream);
+int ptb_rpn_candidate_ranks(const int64_t* gt_inds, const int32_t* n_inside, int B, int N, int32_t* rank, int32_t* counts, void* stream);
+int ptb_rpn_anchor_targets(const int32_t* featmap_hw, const int32_t* strides, int L, int A, int B, const int32_t* inside_idx,
+                           const float* inside_anchors, const int64_t* gt_inds, const int32_t* rank, const int32_t* plan,
+                           const float* gt_bboxes, const int32_t* gt_off, const float* means /*[4]*/, const float* stds /*[4]*/,
+                           float pos_weight, int64_t* labels, float* label_weights, float* bbox_targets, float* bbox_weights,
+                           void* stream);
+int ptb_rpn_sampled_indices(const int64_t* gt_inds, const int32_t* rank, int n, const int32_t* plan, int64_t* pos_inds,
+                            int64_t* neg_inds, void* stream);
+int ptb_rpn_level_loss(const float* cls_score, const float* bbox_pred, const int64_t* labels, const float* label_weights,
+                       const float* bbox_targets, const float* bbox_weights, int64_t M, int bbox_loss, float beta, float* loss_sum /*[2]*/,
+                       const float* scale /*[2] or NULL*/, float* grad_cls, float* grad_bbox, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -132,6 +132,11 @@ SIGNATURES = {
     'ptb_conv_tc_wgrad_f16x2_ld': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, P, c_int, P]),
     'ptb_col_sum_workspace': (c_u64, [c_i64, c_int]),
     'ptb_col_sum': (c_int, [P, c_i64, c_int, c_int, P, P, P]),
+    'ptb_rpn_inside_anchors': (c_int, [P, P, P, c_int, c_int, c_int, P, P, P, P, P]),
+    'ptb_rpn_candidate_ranks': (c_int, [P, P, c_int, c_int, P, P, P]),
+    'ptb_rpn_anchor_targets': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_float, P, P, P, P, P]),
+    'ptb_rpn_sampled_indices': (c_int, [P, P, c_int, P, P, P, P]),
+    'ptb_rpn_level_loss': (c_int, [P, P, P, P, P, P, c_i64, c_int, c_float, P, P, P, P, P]),
 }
 
 

@@ -2,8 +2,8 @@
 (SURVEY.md §8f rank 4: the dense-anchor assignment of BASELINE.json configs[3]).  Same ctor kwargs, `assign` signature and result
 fields (`num_gts`, `gt_inds`, `max_overlaps`, `labels`) as the reference's AssignResult (assign_result.py:42-46).
 
-Also here: PointAssigner, HungarianAssignerV2 (the P2P point assigner named by BASELINE.json north_star) and PseudoSampler /
-SamplingResult mirrors.  `registry.register_core()` registers them into mmdet's BBOX_ASSIGNERS / BBOX_SAMPLERS when mmdet is importable."""
+Also here: PointAssigner, HungarianAssignerV2 (the P2P point assigner named by BASELINE.json north_star), PseudoSampler /
+SamplingResult mirrors and RandomSampler with its host draw plan.  `registry.register_core()` registers them into mmdet's BBOX_ASSIGNERS / BBOX_SAMPLERS when mmdet is importable."""
 import torch
 
 from . import ops
@@ -16,6 +16,15 @@ class AssignResult:
     @property
     def num_preds(self):
         return len(self.gt_inds)
+
+    def add_gt_(self, gt_labels):
+        """assign_result.py:190-204: the GT boxes prepended as proposals assigned to themselves."""
+        self_inds = torch.arange(1, len(gt_labels) + 1, dtype=torch.long, device=gt_labels.device)
+        self.gt_inds = torch.cat([self_inds, self.gt_inds])
+        if self.max_overlaps is not None:
+            self.max_overlaps = torch.cat([self.max_overlaps.new_ones(len(gt_labels)), self.max_overlaps])
+        if self.labels is not None:
+            self.labels = torch.cat([gt_labels, self.labels])
 
 
 class MaxIoUAssigner:
@@ -212,4 +221,80 @@ class PseudoSampler:
         pos_inds = torch.nonzero(assign_result.gt_inds > 0, as_tuple=False).squeeze(-1).unique()
         neg_inds = torch.nonzero(assign_result.gt_inds == 0, as_tuple=False).squeeze(-1).unique()
         gt_flags = bboxes.new_zeros(bboxes.shape[0], dtype=torch.uint8)
+        return SamplingResult(pos_inds, neg_inds, bboxes, gt_bboxes, assign_result, gt_flags)
+
+
+def random_sample_plan(counts, num, pos_fraction, neg_pos_ub=-1):
+    """The draws of BaseSampler.sample + RandomSampler (base_sampler.py:82-97, random_sampler.py:31-81) for images whose assignment has
+    counts = [(positives, negatives), ...], image by image.  Makes exactly the reference's torch.randperm calls on the CPU default
+    generator, in its order, so the sampled sets and the generator state after the call are the reference's.  Per image returns
+    (pos, neg): None when every candidate of that kind is sampled (no draw), else the sorted ranks (int64) of the sampled candidates
+    among the image's positives / negatives — the reference's `gallery[randperm(n)[:k]].unique()` with an ascending gallery."""
+    plan = []
+    num_expected_pos = int(num * pos_fraction)
+    for n_pos, n_neg in counts:
+        pos = torch.randperm(n_pos)[:num_expected_pos].unique() if n_pos > num_expected_pos else None
+        n_sampled_pos = n_pos if pos is None else pos.numel()
+        num_expected_neg = num - n_sampled_pos
+        if neg_pos_ub >= 0:
+            neg_upper_bound = int(neg_pos_ub * max(1, n_sampled_pos))
+            if num_expected_neg > neg_upper_bound:
+                num_expected_neg = neg_upper_bound
+        neg = torch.randperm(n_neg)[:num_expected_neg].unique() if n_neg > num_expected_neg else None
+        plan.append((pos, neg))
+    return plan
+
+
+def sampled_counts(plan, counts):
+    """per image (sampled positives, sampled negatives) of a random_sample_plan"""
+    return [tuple(c if sel is None else sel.numel() for sel, c in zip(p, cnt)) for p, cnt in zip(plan, counts)]
+
+
+def upload_sample_plan(plan, device):
+    """the plan in the layout of ptb_rpn_anchor_targets / ptb_rpn_sampled_indices (include/ptb_b200.h), one copy from pinned memory"""
+    head, body, off = [], [], 4 * len(plan)
+    for p in plan:
+        for sel in p:
+            if sel is None:
+                head += [0, -1]
+            else:
+                head += [off, sel.numel()]
+                body.append(sel)
+                off += sel.numel()
+    buf = torch.empty((off,), dtype=torch.int32, pin_memory=True)
+    buf[:len(head)] = torch.tensor(head, dtype=torch.int32)
+    if body:
+        buf[len(head):] = torch.cat(body)
+    return buf.to(device, non_blocking=True)
+
+
+class RandomSampler:
+    """mmdet/core/bbox/samplers/random_sampler.py:7-81 with base_sampler.py:8-101: same ctor kwargs and `sample` signature and result.
+    The candidate ranks and counts come from ptb_rpn_candidate_ranks, the draws from random_sample_plan (the reference's randperm
+    calls on the CPU generator), the sampled index lists from ptb_rpn_sampled_indices: one device-to-host copy (the two counts)."""
+
+    def __init__(self, num, pos_fraction, neg_pos_ub=-1, add_gt_as_proposals=True, **kwargs):
+        # kwargs may carry the reference's `rng`, which its random_choice never reads (it draws with torch.randperm)
+        self.num, self.pos_fraction, self.neg_pos_ub, self.add_gt_as_proposals = num, pos_fraction, neg_pos_ub, add_gt_as_proposals
+
+    def sample(self, assign_result, bboxes, gt_bboxes, gt_labels=None, **kwargs):
+        if not assign_result.gt_inds.is_cuda:
+            raise RuntimeError('RandomSampler runs on CUDA tensors only; there is no CPU fallback')
+        if len(bboxes.shape) < 2:
+            bboxes = bboxes[None, :]
+        bboxes = bboxes[:, :4]
+        gt_flags = bboxes.new_zeros((bboxes.shape[0],), dtype=torch.uint8)
+        if self.add_gt_as_proposals and len(gt_bboxes) > 0:
+            if gt_labels is None:
+                raise ValueError('gt_labels must be given when add_gt_as_proposals is True')
+            bboxes = torch.cat([gt_bboxes, bboxes], dim=0)
+            assign_result.add_gt_(gt_labels)
+            gt_flags = torch.cat([bboxes.new_ones(gt_bboxes.shape[0], dtype=torch.uint8), gt_flags])
+        gt_inds = assign_result.gt_inds.contiguous()
+        n = gt_inds.numel()
+        rank, counts = ops.rpn_candidate_ranks(gt_inds.view(1, n), torch.full((1,), n, dtype=torch.int32, device=gt_inds.device))
+        counts = [tuple(c) for c in counts.cpu().tolist()]
+        plan = random_sample_plan(counts, self.num, self.pos_fraction, self.neg_pos_ub)
+        (n_pos, n_neg), = sampled_counts(plan, counts)
+        pos_inds, neg_inds = ops.rpn_sampled_indices(gt_inds, rank.view(-1), upload_sample_plan(plan, gt_inds.device), n_pos, n_neg)
         return SamplingResult(pos_inds, neg_inds, bboxes, gt_bboxes, assign_result, gt_flags)

@@ -4,6 +4,7 @@
 // mse_loss.py:9-48).  All HBM-bound scan / select work: coalesced channels-last
 // reads, warp-shuffle reductions, radix select + bitonic sort in shared memory (no library sort).
 #include "ptb_common.cuh"
+#include "loss_terms.cuh"
 #include "topk_select.cuh"
 #include <math_constants.h>
 
@@ -372,19 +373,6 @@ __global__ void pa_finish_kernel(const unsigned long long* __restrict__ best, in
 // ------------------------------------------------------------------------------------------------
 // losses with fused forward / backward and a fixed-order sum
 // ------------------------------------------------------------------------------------------------
-// An elementwise loss is a functor over element e:  op(e, want_loss, grad, sc) returns e's term of the loss sum (read only when
-// want_loss) and, when grad is set, stores grad[e] = sc * d term / dx[e].  The kernel owns the loop and the sum.
-template <class Loss>
-__global__ void __launch_bounds__(256)
-loss_sum_kernel(Loss op, long long n, float* loss_sum, const float* __restrict__ scale, float* __restrict__ grad,
-                SumScratch* __restrict__ scr) {
-  const float sc = (grad && scale) ? scale[0] : 1.f;
-  float acc = 0.f;
-  for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < n; e += (long long)gridDim.x * 256)
-    acc += op(e, loss_sum != nullptr, grad, sc);
-  if (loss_sum) block_partial_finish(acc, *scr, loss_sum);
-}
-
 // FocalLoss (focal_loss.py:11-56) over M x C logits, the per-proposal weight broadcast over the classes
 struct FocalLoss {
   const float* x; const int64_t* labels; const float* weight; int C; float gamma, alpha;
@@ -410,19 +398,6 @@ struct FocalLoss {
   }
 };
 
-// SmoothL1Loss (smooth_l1_loss.py:25-31) on the normalised points
-struct SmoothL1Loss {
-  const float* pred; const float* target; const float* weight; float inv_norm, beta;
-  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
-    const float w = weight ? weight[e] : 1.f;
-    const float diff = (pred[e] - target[e]) * inv_norm;
-    const float d = fabsf(diff);
-    // a NaN diff keeps its NaN gradient (0 * |diff|), as torch's does through the unselected branch of torch.where
-    if (grad) grad[e] = sc * w * inv_norm * (d < beta ? diff / beta : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f * d)));
-    return (d < beta ? 0.5f * d * d / beta : d - 0.5f * beta) * w;
-  }
-};
-
 // The regression losses over several FPN levels: each proposal row m brings its own 1 / (stride_m * reg_norm) (p2p_head.py:234-240
 // divides by the row's own stride), the rest is the single-level functor.
 template <class Loss>
@@ -432,47 +407,6 @@ struct PerRowNorm {
     Loss l = base;
     l.inv_norm = row_inv_norm[e >> 1];
     return l(e, want_loss, grad, sc);
-  }
-};
-
-// CrossEntropyLoss(use_sigmoid=True) = binary_cross_entropy (cross_entropy_loss.py:42-89): labels expanded to one-hot rows
-// (_expand_onehot_labels; a label outside [0, C), e.g. the background label C, is an all-zero row), the per-proposal weight
-// broadcast over the classes, F.binary_cross_entropy_with_logits(reduction='none') in ATen's CPU form
-//   (1 - t) * x - log_sigmoid(x),   log_sigmoid(x) = min(x, 0) - log1p(exp(-|x|)),
-// then the weighted sum of weight_reduce_loss (the caller divides by avg_factor).  d/dx = sigmoid(x) - t.
-// POS_WEIGHT: CrossEntropyLoss.class_weight, which binary_cross_entropy passes as pos_weight (cross_entropy_loss.py:85-86), in
-// ATen's CPU order: log_weight = (pw_c - 1) * t + 1, loss = (1 - t) * x - log_sigmoid(x) * log_weight; d/dx = (pw_c t + 1 - t)
-// sigmoid(x) - pw_c t (binary_cross_entropy_with_logits_backward).  Without it this is the class_weight=None form above.
-// The log is computed only when the sum is wanted: the backward launch skips it.
-template <bool POS_WEIGHT>
-struct SigmoidBCELoss {
-  const float* x; const int64_t* labels; const float* weight; const float* pos_weight; int C;
-  __device__ __forceinline__ float operator()(long long e, bool want_loss, float* grad, float sc) const {
-    const long long m = e / C;
-    const int c = (int)(e - m * C);
-    const float w = weight ? weight[m] : 1.f;
-    const float t = (labels[m] == c) ? 1.f : 0.f;
-    const float v = x[e];
-    float term = 0.f;
-    if constexpr (POS_WEIGHT) {
-      const float pw = pos_weight[c];
-      if (want_loss) {
-        const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
-        const float log_w = __fadd_rn(__fmul_rn(__fsub_rn(pw, 1.f), t), 1.f);
-        term = __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), __fmul_rn(log_sig, log_w)), w);
-      }
-      if (grad) {
-        const float pt = __fmul_rn(pw, t);
-        grad[e] = sc * w * __fsub_rn(__fmul_rn(__fsub_rn(__fadd_rn(pt, 1.f), t), sigmoidf_acc(v)), pt);
-      }
-    } else {
-      if (want_loss) {
-        const float log_sig = __fsub_rn(fminf(v, 0.f), log1pf(expf(-fabsf(v))));
-        term = __fmul_rn(__fsub_rn(__fmul_rn(1.f - t, v), log_sig), w);
-      }
-      if (grad) grad[e] = sc * w * (sigmoidf_acc(v) - t);
-    }
-    return term;
   }
 };
 
@@ -983,19 +917,6 @@ struct GHMRLoss {
     }
     if (grad) grad[e] = sc * w * inv * (d / r);
     return (r - mu) * w;
-  }
-};
-
-// L1Loss on the normalised points: |d| * weight; d/dpred = sgn(d) * inv * weight.  ATen's abs backward multiplies by sgn(d), which is
-// 0 at d == 0 and at a NaN d, so a NaN difference has gradient 0 (its loss term is NaN)
-struct L1RowsLoss {
-  const float* pred; const float* target; const float* weight; const float* row_inv_norm;
-  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
-    const float inv = row_inv_norm[e >> 1];
-    const float w = weight ? weight[e] : 1.f;
-    const float d = (pred[e] - target[e]) * inv;
-    if (grad) grad[e] = sc * w * inv * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
-    return fabsf(d) * w;
   }
 };
 

@@ -776,15 +776,22 @@ def bbox_overlaps(boxes1, boxes2, mode='iou'):
 
 
 def max_iou_assign(bboxes, gt_bboxes, gt_labels=None, gt_bboxes_ignore=None, pos_iou_thr=0.5, neg_iou_thr=0.5, min_pos_iou=0.0,
-                   gt_max_assign_all=True, ignore_iof_thr=-1, ignore_wrt_candidates=True, match_low_quality=True):
-    """ptb_max_iou_assign.  returns gt_inds (N,) int64, max_overlaps (N,), labels (N,) int64 | None."""
+                   gt_max_assign_all=True, ignore_iof_thr=-1, ignore_wrt_candidates=True, match_low_quality=True, out=None):
+    """ptb_max_iou_assign.  returns gt_inds (N,) int64, max_overlaps (N,), labels (N,) int64 | None.  out: optional contiguous
+    (gt_inds, max_overlaps) tensors of N elements to write into, e.g. one image's rows of a batch buffer."""
     lib = _lib.load()
     _chk(bboxes, torch.float32, 'bboxes'); _chk(gt_bboxes, torch.float32, 'gt_bboxes')
     N, n = bboxes.shape[0], gt_bboxes.shape[0]
     dev = bboxes.device
     lo, hi = (0.0, float(neg_iou_thr)) if isinstance(neg_iou_thr, float) else (float(neg_iou_thr[0]), float(neg_iou_thr[1]))
-    gt_inds = torch.empty((N,), dtype=torch.int64, device=dev)
-    max_ov = torch.empty((N,), dtype=torch.float32, device=dev)
+    if out is not None:
+        gt_inds, max_ov = out
+        _chk(gt_inds, torch.int64, 'out gt_inds'); _chk(max_ov, torch.float32, 'out max_overlaps')
+        if gt_inds.numel() != N or max_ov.numel() != N:
+            raise ValueError(f'out tensors must have {N} elements')
+    else:
+        gt_inds = torch.empty((N,), dtype=torch.int64, device=dev)
+        max_ov = torch.empty((N,), dtype=torch.float32, device=dev)
     labels = torch.empty((N,), dtype=torch.int64, device=dev) if gt_labels is not None else None
     gl = gt_labels.to(torch.int32).contiguous() if gt_labels is not None else None
     ign = gt_bboxes_ignore if (gt_bboxes_ignore is not None and gt_bboxes_ignore.numel() > 0) else None
@@ -1319,3 +1326,117 @@ def conv_tc_f16(x_h, x_l, packed, taps, n_out, bias=None, dev_out_scale=None, ld
                                              _ptr(dev_out_scale), _ptr(bias), _ptr(y), HALF_DTYPES[out_dtype], ldy, _stream()),
               'ptb_conv_tc_f16x2_half_out')
     return y
+
+
+# ---- RPN training (ptb_rpn_*): targets, sampling plan and losses of AnchorHead.loss with RandomSampler
+RPN_MAX_LEVELS = 8                     # PTB_RPN_MAX_LEVELS
+RPN_LOSS_L1, RPN_LOSS_SMOOTH_L1 = 0, 1
+
+
+def _level_arrays(featmap_sizes, strides_wh):
+    L = len(featmap_sizes)
+    if not 1 <= L <= RPN_MAX_LEVELS:
+        raise ValueError(f'1 to {RPN_MAX_LEVELS} levels, got {L}')
+    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for s in featmap_sizes for v in s])
+    st = (ctypes.c_int32 * (2 * L))(*[int(v) for s in strides_wh for v in s])
+    return L, hw, st
+
+
+def rpn_inside_anchors(base_anchors, featmap_sizes, strides_wh, inside_box):
+    """ptb_rpn_inside_anchors.  base_anchors (L, A, 4) fp32, inside_box (B, L, A, 4) int32 (x0, x1, y0, y1).
+    returns inside_anchors (B, N, 4) (image b's first n_inside[b] rows), inside_idx (B, N) int32, n_inside (B,) int32."""
+    lib = _lib.load()
+    _chk(base_anchors, torch.float32, 'base_anchors'); _chk(inside_box, torch.int32, 'inside_box')
+    L, hw, st = _level_arrays(featmap_sizes, strides_wh)
+    A = base_anchors.shape[1]
+    B = inside_box.shape[0]
+    if tuple(base_anchors.shape) != (L, A, 4) or tuple(inside_box.shape) != (B, L, A, 4):
+        raise ValueError('base_anchors must be (L, A, 4) and inside_box (B, L, A, 4)')
+    N = sum(int(h) * int(w) * A for h, w in featmap_sizes)
+    dev = base_anchors.device
+    anchors = torch.empty((B, N, 4), dtype=torch.float32, device=dev)
+    idx = torch.empty((B, N), dtype=torch.int32, device=dev)
+    n_inside = torch.empty((B,), dtype=torch.int32, device=dev)
+    check(lib.ptb_rpn_inside_anchors(_ptr(base_anchors), hw, st, L, A, B, _ptr(inside_box), _ptr(anchors), _ptr(idx), _ptr(n_inside),
+                                     _stream()), 'ptb_rpn_inside_anchors')
+    return anchors, idx, n_inside
+
+
+def rpn_candidate_ranks(gt_inds, n_inside):
+    """ptb_rpn_candidate_ranks.  gt_inds (B, N) int64, n_inside (B,) int32 -> rank (B, N) int32, counts (B, 2) int32 (pos, neg)."""
+    lib = _lib.load()
+    _chk(gt_inds, torch.int64, 'gt_inds'); _chk(n_inside, torch.int32, 'n_inside')
+    B, N = gt_inds.shape
+    if tuple(n_inside.shape) != (B,):
+        raise ValueError(f'n_inside must have shape ({B},)')
+    rank = torch.empty((B, N), dtype=torch.int32, device=gt_inds.device)
+    counts = torch.empty((B, 2), dtype=torch.int32, device=gt_inds.device)
+    check(lib.ptb_rpn_candidate_ranks(_ptr(gt_inds), _ptr(n_inside), B, N, _ptr(rank), _ptr(counts), _stream()), 'ptb_rpn_candidate_ranks')
+    return rank, counts
+
+
+def rpn_anchor_targets(featmap_sizes, strides_wh, A, inside_idx, inside_anchors, gt_inds, rank, plan, gt_bboxes, gt_off, means, stds,
+                       pos_weight):
+    """ptb_rpn_anchor_targets.  returns labels (int64), label_weights like the concatenated cls_score maps (B*A*H*W per level, level
+    after level) and bbox_targets, bbox_weights like the concatenated bbox_pred maps (B*4A*H*W per level)."""
+    lib = _lib.load()
+    L, hw, st = _level_arrays(featmap_sizes, strides_wh)
+    B, N = inside_idx.shape
+    for t, dt, name in ((inside_idx, torch.int32, 'inside_idx'), (inside_anchors, torch.float32, 'inside_anchors'),
+                        (gt_inds, torch.int64, 'gt_inds'), (rank, torch.int32, 'rank'), (plan, torch.int32, 'plan'),
+                        (gt_bboxes, torch.float32, 'gt_bboxes'), (gt_off, torch.int32, 'gt_off')):
+        _chk(t, dt, name)
+    if N != sum(int(h) * int(w) * A for h, w in featmap_sizes) or tuple(inside_anchors.shape) != (B, N, 4) or \
+            tuple(gt_inds.shape) != (B, N) or tuple(rank.shape) != (B, N) or tuple(gt_off.shape) != (B + 1,) or \
+            gt_bboxes.dim() != 2 or gt_bboxes.shape[1] != 4 or plan.numel() < 4 * B:
+        raise ValueError('rpn_anchor_targets: inconsistent shapes')
+    dev = inside_idx.device
+    labels = torch.empty((B * N,), dtype=torch.int64, device=dev)
+    lw = torch.empty((B * N,), dtype=torch.float32, device=dev)
+    bt = torch.empty((B * N * 4,), dtype=torch.float32, device=dev)
+    bw = torch.empty((B * N * 4,), dtype=torch.float32, device=dev)
+    mean = (ctypes.c_float * 4)(*[float(v) for v in means])
+    std = (ctypes.c_float * 4)(*[float(v) for v in stds])
+    check(lib.ptb_rpn_anchor_targets(hw, st, L, A, B, _ptr(inside_idx), _ptr(inside_anchors), _ptr(gt_inds), _ptr(rank), _ptr(plan),
+                                     _ptr(gt_bboxes), _ptr(gt_off), mean, std, float(pos_weight), _ptr(labels), _ptr(lw), _ptr(bt),
+                                     _ptr(bw), _stream()), 'ptb_rpn_anchor_targets')
+    return labels, lw, bt, bw
+
+
+def rpn_sampled_indices(gt_inds, rank, plan, n_pos, n_neg):
+    """ptb_rpn_sampled_indices for one image: the sampled positive and negative rows (int64, ascending)."""
+    lib = _lib.load()
+    _chk(gt_inds, torch.int64, 'gt_inds'); _chk(rank, torch.int32, 'rank'); _chk(plan, torch.int32, 'plan')
+    n = gt_inds.numel()
+    if rank.numel() != n or plan.numel() < 4:
+        raise ValueError('rpn_sampled_indices: inconsistent shapes')
+    pos = torch.empty((n_pos,), dtype=torch.int64, device=gt_inds.device)
+    neg = torch.empty((n_neg,), dtype=torch.int64, device=gt_inds.device)
+    check(lib.ptb_rpn_sampled_indices(_ptr(gt_inds), _ptr(rank), n, _ptr(plan), _ptr(pos), _ptr(neg), _stream()),
+          'ptb_rpn_sampled_indices')
+    return pos, neg
+
+
+def rpn_level_loss(cls_score, bbox_pred, labels, label_weights, bbox_targets, bbox_weights, bbox_loss, beta, scale=None, want_grad=False):
+    """ptb_rpn_level_loss on one level's maps cls_score (B, A, H, W) / bbox_pred (B, 4A, H, W) and its target slices.  Returns the
+    (2,) un-normalised sums (cls, bbox) or, with want_grad, (scale[0] d/dcls_score, scale[1] d/dbbox_pred)."""
+    lib = _lib.load()
+    _chk(cls_score, torch.float32, 'cls_score'); _chk(bbox_pred, torch.float32, 'bbox_pred')
+    M = cls_score.numel()
+    if bbox_pred.numel() != 4 * M or labels.numel() != M or label_weights.numel() != M or bbox_targets.numel() != 4 * M or \
+            bbox_weights.numel() != 4 * M:
+        raise ValueError('rpn_level_loss: inconsistent sizes')
+    _chk(labels, torch.int64, 'labels'); _chk(label_weights, torch.float32, 'label_weights')
+    _chk(bbox_targets, torch.float32, 'bbox_targets'); _chk(bbox_weights, torch.float32, 'bbox_weights')
+    if want_grad:
+        _chk(scale, torch.float32, 'scale')
+        gc, gb = torch.empty_like(cls_score), torch.empty_like(bbox_pred)
+        check(lib.ptb_rpn_level_loss(_ptr(cls_score), _ptr(bbox_pred), _ptr(labels), _ptr(label_weights), _ptr(bbox_targets),
+                                     _ptr(bbox_weights), M, int(bbox_loss), float(beta), None, _ptr(scale), _ptr(gc), _ptr(gb), _stream()),
+              'ptb_rpn_level_loss')
+        return gc, gb
+    loss = torch.zeros(2, dtype=torch.float32, device=cls_score.device)
+    check(lib.ptb_rpn_level_loss(_ptr(cls_score), _ptr(bbox_pred), _ptr(labels), _ptr(label_weights), _ptr(bbox_targets),
+                                 _ptr(bbox_weights), M, int(bbox_loss), float(beta), _ptr(loss), None, None, None, _stream()),
+          'ptb_rpn_level_loss')
+    return loss

@@ -76,6 +76,15 @@ def register_core():
     ANCHOR_GENERATORS.register_module(name='AnchorGenerator', force=True, module=AnchorGenerator)
 
 
+def register_rpn():
+    """register RPNHead (HEADS) and RandomSampler (BBOX_SAMPLERS) with force=True over the reference classes.  Not done on import nor by
+    register_core(): a detector whose RoI head samples with the reference's RandomSampler keeps it until this is called."""
+    from .assigners import RandomSampler
+    from .rpn import RPNHead
+    HEADS.register_module(name='RPNHead', force=True, module=RPNHead)
+    BBOX_SAMPLERS.register_module(name='RandomSampler', force=True, module=RandomSampler)
+
+
 def build_assigner(cfg, **default_args):
     return BBOX_ASSIGNERS.build(cfg, default_args)
 
