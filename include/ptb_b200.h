@@ -642,7 +642,8 @@ int ptb_bbox_overlaps(const float* boxes1, int m, const float* boxes2, int n, in
  *                            max|dy| as float bits (device) for the operand scale.  Deterministic (no fp atomics).
  *   ptb_split_f16_amax       dy -> fp16 (h, l) pair with the power-of-two scale derived from that device max; 1/scale -> dev_inv_scale
  *   ptb_conv_tc_f16x2        dgrad: the forward kernel on (dy pair, weights transposed + flipped and packed by the host layer)
- *   ptb_conv3x3_wgrad_f16x2  dW[co][ci][3][3] (+)= scale * s_dy * s_x * sum_pixels dy (x) x_shifted  on wgmma with MN-major operands
+ *   ptb_conv_tc_wgrad_f16x2_ld  taps 9, ld_dy = Cout: dW[co][ci][3][3] (+)= scale * s_dy * s_x * sum_pixels dy (x) x_shifted
+ *                            on wgmma with MN-major operands
  * All tensors channels-last; C = 256 for the tensor-core kernels.
  */
 uint64_t ptb_gn_relu_bwd_workspace(int B, int HW, int C, int groups);
@@ -651,21 +652,16 @@ int ptb_gn_relu_bwd(const float* da, const float* y, const double* gn_stats, con
                     float* dbeta /*[C] or NULL*/, unsigned int* amax_bits /*device, or NULL*/, void* stream);
 int ptb_split_f16_amax(const float* x, int64_t n, const unsigned int* dev_amax_bits, void* hi, void* lo, float* dev_inv_scale,
                        void* stream);
-uint64_t ptb_conv3x3_wgrad_workspace(int B, int H, int W);
-int ptb_conv3x3_wgrad_f16x2(const void* dy_h, const void* dy_l, const void* x_h, const void* x_l, int B, int H, int W, int Cout, int Cin,
-                            float scale, const float* dev_scale_dy /*or NULL*/, const float* dev_scale_x /*or NULL*/, void* workspace,
-                            float* dw /*[Cout][Cin][3][3]*/, int accumulate, void* stream);
 
-/* The same kernel for any channels-last GEMM with K = pixels:  dW[co][ci][tap] = scale * s_dy * s_x * sum_pixels dy[p][co] * x[p + tap][ci]
- * with taps = 9 (conv3x3, pad 1) or taps = 1 (conv1x1 / per-cell Linear: the weight gradient of CPRHead's cls_out / ins_out logit map,
- * cpr_head.py:1045-1078 under autograd), Cin = 256, Cout a multiple of 8 up to 256 (rows beyond Cout are never written).
- * dw is [Cout][256][taps] fp32.  Deterministic (fixed-order reduction of the pixel splits). */
+/* The weight gradient of any channels-last GEMM with K = pixels:
+ *   dW[co][ci][tap] (+)= scale * s_dy * s_x * sum_pixels dy[p][co] * x[p + tap][ci]
+ * with taps = 9 (conv3x3, pad 1: the towers) or taps = 1 (conv1x1 / per-cell Linear: the weight gradient of CPRHead's cls_out / ins_out
+ * logit map, cpr_head.py:1045-1078 under autograd), Cin = 256, Cout a multiple of 8 up to 256 (rows beyond Cout are never written).
+ * dy (fp16 pair [B][H][W][.], 16-byte aligned) has rows ld_dy fp16 apart (ld_dy >= Cout, a multiple of 8): ld_dy = Cout for a dense
+ * map, or one column slice [c0, c0 + Cout) of a wider pair (dy + c0), e.g. the logit map's gradient of more than 256 columns, without
+ * a copy.  x is [B][H][W][256] fp16.  dw is [Cout][256][taps] fp32; dev_scale_dy / dev_scale_x may be NULL.  Deterministic
+ * (fixed-order reduction of the pixel splits). */
 uint64_t ptb_conv_tc_wgrad_workspace(int B, int H, int W, int taps);
-int ptb_conv_tc_wgrad_f16x2(const void* dy_h, const void* dy_l /*[B][H][W][Cout] fp16*/, const void* x_h, const void* x_l /*[B][H][W][256] fp16*/,
-                            int B, int H, int W, int Cout, int Cin, int taps, float scale, const float* dev_scale_dy,
-                            const float* dev_scale_x, void* workspace, float* dw, int accumulate, void* stream);
-/* the same with dy rows ld_dy fp16 apart (ld_dy >= Cout, a multiple of 8; dy 16-byte aligned): one column slice [c0, c0 + Cout) of a wider
- * fp16 pair (dy + c0), e.g. the logit map's gradient of more than 256 columns, without a copy.  dw [Cout][256] as above. */
 int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H, int W,
                                int Cout, int Cin, int taps, float scale, const float* dev_scale_dy, const float* dev_scale_x,
                                void* workspace, float* dw, int accumulate, void* stream);

@@ -125,10 +125,7 @@ SIGNATURES = {
     'ptb_gn_relu_bwd_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
     'ptb_gn_relu_bwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_float, c_int, P, P, P, P, P, P]),
     'ptb_split_f16_amax': (c_int, [P, c_i64, P, P, P, P, P]),
-    'ptb_conv3x3_wgrad_workspace': (c_u64, [c_int, c_int, c_int]),
-    'ptb_conv3x3_wgrad_f16x2': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, P, c_int, P]),
     'ptb_conv_tc_wgrad_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
-    'ptb_conv_tc_wgrad_f16x2': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, P, c_int, P]),
     'ptb_conv_tc_wgrad_f16x2_ld': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, P, c_int, P]),
     'ptb_col_sum_workspace': (c_u64, [c_i64, c_int]),
     'ptb_col_sum': (c_int, [P, c_i64, c_int, c_int, P, P, P]),

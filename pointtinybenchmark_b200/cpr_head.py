@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc, _packed_tc_cols
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
 from .registry import register_head
 
 _SUPPORTED_POS = ('CirclePtFeatGenerator', 'GridCirclesPtFeatGenerator')
@@ -103,19 +103,13 @@ class _GridCircleBags:
         return ops.grid_bag_bwd(grad, map_shape, gt.centers, gt.bag_img, cell, self.stride)
 
 
-def _loss_gemm_on_tc(C, LD):
-    """the two GEMMs of the loss that are plain 1x1 convolutions (logit map forward, its input gradient) run on the wgmma kernel
-    when the channel counts fit it (Cin % 32 == 0, LD <= 256); PTB_LOSS_GEMM=ffma keeps the fp32 FFMA kernels."""
-    import os
-    return os.environ.get('PTB_LOSS_GEMM', 'tc') == 'tc' and C % 32 == 0 and LD % 32 == 0 and C <= 256 and LD <= 256
-
-
-def _loss_map_sliced_on_tc(N, C):
-    """above 256 classes the training logit map runs as column slices of the wgmma kernel (ops.conv_tc_f16_cols); with 256 input
-    channels its two backward GEMMs run on the tensor cores too (dW in column slices, dX as one conv with Cin = LD).  Up to 256 classes
-    the choice is _loss_gemm_on_tc's."""
-    import os
-    return os.environ.get('PTB_LOSS_GEMM', 'tc') == 'tc' and N > 256 and C % 32 == 0
+def _loss_map_on_tc(N, C, LD):
+    """the logit map of the loss (a 1x1 convolution of the C-channel feature map to LD = 2 * NP columns) runs on the wgmma kernel, in
+    column slices of <= 512, when its input channels fit it (C % 32 == 0) and either the map fits one launch with LD % 32 == 0 and
+    C, LD <= 256, or there are more than 256 classes (loss_bwd_plan then pads LD to a multiple of 32).  Every other shape runs on the
+    fp32 FFMA kernels.  With 256 input channels its two backward GEMMs run on the tensor cores too (dW in column slices of <= 256,
+    dX as one conv with Cin = LD)."""
+    return C % 32 == 0 and ((LD % 32 == 0 and C <= 256 and LD <= 256) or N > 256)
 
 
 MAX_CLASSES = 1280     # the loss kernels' class limit (ptb_cpr_loss_bwd_scatter: 4 classes x 320 lanes, ptb_mil_loss_fwd / _bwd)
@@ -200,20 +194,14 @@ class _CPRLossFn(torch.autograd.Function):
         bcat = torch.zeros((LD,), device=dev)
         wcat[:N], wcat[NP:NP + N], bcat[:N], bcat[NP:NP + N] = w_cls, w_ins, b_cls, b_ins
         x2d = fmap.reshape(M, C)
-        use_tc = _loss_gemm_on_tc(C, LD)
-        sliced = not use_tc and _loss_map_sliced_on_tc(N, C)
-        if use_tc:       # logit map on the tensor cores: 1-tap conv of the fp16 operand pair (fp32-accurate two-term split)
+        on_tc = _loss_map_on_tc(N, C, LD)
+        if on_tc:       # logit map on the tensor cores: 1-tap conv of the fp16 operand pair (fp32-accurate two-term split)
             fh, fl, finv = ops.split_f16(fmap, auto_scale=True)
             lmap = ops.conv_tc_f16(fh, fl, ops.conv_tc_pack_weight_f16(wcat, 1), 1, LD, bias=bcat, dev_out_scale=finv, ldy=LD).view(M, LD)
-        elif sliced:
-            fh, fl, finv = ops.split_f16(fmap, auto_scale=True)
-            lmap = ops.conv_tc_f16_cols(fh, fl, ops.conv_tc_pack_weight_f16_cols(wcat, 1), 1, LD, bias=bcat, dev_out_scale=finv,
-                                        ldy=LD).view(M, LD)
         else:
             lmap = ops.linear_rows(x2d, wcat, bcat)                              # (M, LD) fp32 FFMA GEMM
         allpos, kind = hp['allpos'], hp['loss_kind']
-        fused_fwd = isinstance(bags, _CircleBags) and hp['with_mil_loss'] and not allpos and N <= 128 and \
-            os.environ.get('PTB_LOSS_FWD', 'fused') == 'fused'
+        fused_fwd = isinstance(bags, _CircleBags) and hp['with_mil_loss'] and not allpos and N <= 128
         if fused_fwd:   # ring-bag gather + MIL forward in ONE kernel (online softmax): the (G,K,LD) tensor is written once, never re-read
             bl, weight, bag_prob, mil_sum, mil_stats, mil_mt, mil_lw = ops.bag_mil_fwd(
                 lmap.view(B, H, W, LD), N, NP, gt.centers, gt.bag_img, bags.offsets, bags.stride, gt.pad_hw, gt.labels, hp['eps'],
@@ -265,7 +253,7 @@ class _CPRLossFn(torch.autograd.Function):
             saved['neg_mask'] = nm
         ctx.hp, ctx.gt, ctx.bags, ctx.aux, ctx.saved = hp, gt, bags, aux, saved
         ctx.num_pos = num_pos
-        ctx.fpair = (fh, fl, finv) if (use_tc or sliced) else None    # fp16 operand pair of the feature map: the wgrad's second operand
+        ctx.fpair = (fh, fl, finv) if on_tc else None    # fp16 operand pair of the feature map: the wgrad's second operand
         ctx.save_for_backward(fmap, wcat, lmap, bl, weight)
         return gt_loss, pos_loss, neg_loss, bag_acc
 
@@ -348,18 +336,11 @@ class _CPRLossFn(torch.autograd.Function):
             dlmap = _CPRLossFn._bwd_map_staged(ctx, g_gt, g_pos, g_neg, bl, weight, lmap, B, H, W, N, NP, LD, M, G, K)
         d2 = dlmap.view(M, LD)
         x2d = fmap.reshape(M, C)
-        if ctx.fpair is not None and C == 256 and LD > 256 and LD % 32 == 0:
-            # above 256 classes: dW in column slices of <= 256 of the gradient's fp16 pair (the wgrad's widest output), read in place;
-            # dX as one conv with Cin = LD (loss_bwd_plan pads LD to a multiple of 32 here)
-            dh, dl_, dinv = ops.split_f16(dlmap.view(B, H, W, LD), auto_scale=True)
-            fh, fl, finv = ctx.fpair
-            dw = ops.conv_tc_wgrad_f16_cols(dh, dl_, fh, fl, 1.0, dinv, finv)
-            db = ops.col_sum(d2)
-            dx = ops.conv_tc_f16(dh, dl_, ops.conv_tc_pack_weight_f16(wcat.t().contiguous(), 1), 1, C, dev_out_scale=dinv, ldy=C)
-        elif _loss_gemm_on_tc(C, LD) and ctx.fpair is not None and C == 256 and LD % 8 == 0:
+        if ctx.fpair is not None and C == 256:
             # both GEMMs of the Linear's backward on the tensor cores (fp16 two-term split, fp32-accurate, deterministic):
-            #   dW = dL^T @ X  : K = pixels, MN-major operands (the tower's wgrad kernel with one tap)
-            #   dX = dL @ W    : 1-tap conv with W^T (Cin = LD)
+            #   dW = dL^T @ X  : K = pixels, MN-major operands (the tower's wgrad kernel with one tap), in column slices of <= 256 of
+            #                    the gradient's fp16 pair, read in place
+            #   dX = dL @ W    : 1-tap conv with W^T (Cin = LD, a multiple of 32 whenever the forward ran on the tensor cores)
             dh, dl_, dinv = ops.split_f16(dlmap.view(B, H, W, LD), auto_scale=True)
             fh, fl, finv = ctx.fpair
             dw = ops.conv_tc_wgrad_f16(dh, dl_, fh, fl, 1, 1.0, dinv, finv)
@@ -638,11 +619,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 if self.debug and self.last_overflow_flag is not None and int(self.last_overflow_flag) != 0:    # host sync: debug only
                     raise FloatingPointError('CPRHead: a GroupNorm output exceeded the fp16 operand range (|x| > 6e4) and was clamped')
                 h, l = pair
-                bias = self.cls_out.bias.detach()
-                if self.num_classes <= ops.CONV_TC_N_MAX:
-                    lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1, 'lin'), 1, self.num_classes, bias=bias)
-                else:            # wider than one wgmma launch: column slices of the same kernel into one map
-                    lmap = ops.conv_tc_f16_cols(h, l, _packed_tc_cols(self.cls_out, 1), 1, self.num_classes, bias=bias)
+                lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1), 1, self.num_classes, bias=self.cls_out.bias.detach())
                 return self._get_bboxes_from_logit_map(lmap, img_metas, rescale=rescale, **kwargs)
         outs = self.forward(feats)
         return self.get_bboxes(*outs, img_metas, rescale=rescale, **kwargs)

@@ -260,12 +260,12 @@ static uint64_t wgrad_ws_bytes(int B, int H, int W, int taps) {
   return (uint64_t)splits * wgrad_max_runs(n_blocks, splits) * taps * WG_C * WG_C * sizeof(float);
 }
 
-extern "C" uint64_t ptb_conv3x3_wgrad_workspace(int B, int H, int W) { return wgrad_ws_bytes(B, H, W, 9); }
 extern "C" uint64_t ptb_conv_tc_wgrad_workspace(int B, int H, int W, int taps) { return wgrad_ws_bytes(B, H, W, taps); }
 
 static int wgrad_run(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H, int W, int Cout, int Cin,
                      int taps, float scale, const float* dev_scale_dy, const float* dev_scale_x, void* workspace, float* dw, int accumulate,
-                     void* stream, const char* what) {
+                     void* stream) {
+  const char* what = "ptb_conv_tc_wgrad_f16x2_ld";
   CUtensorMap tm_dyh, tm_dyl, tm_xh, tm_xl;
   int rc;
   if ((rc = make_px_map(&tm_dyh, dy_h, B, H, W, Cout, ld_dy))) return rc;
@@ -293,30 +293,6 @@ static int wgrad_run(const void* dy_h, const void* dy_l, int ld_dy, const void* 
   return check_launch(what);
 }
 
-extern "C" int ptb_conv3x3_wgrad_f16x2(const void* dy_h, const void* dy_l, const void* x_h, const void* x_l, int B, int H, int W,
-                                       int Cout, int Cin, float scale, const float* dev_scale_dy, const float* dev_scale_x,
-                                       void* workspace, float* dw, int accumulate, void* stream) {
-  PTB_REQUIRE(B > 0 && H > 0 && W > 0, "shape");
-  PTB_REQUIRE(Cout == WG_C && Cin == WG_C, "the tensor-core weight gradient covers the head's 256 -> 256 convolutions");
-  PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
-  PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
-                  ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
-  return wgrad_run(dy_h, dy_l, Cout, x_h, x_l, B, H, W, Cout, Cin, 9, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
-                   "ptb_conv3x3_wgrad_f16x2");
-}
-
-extern "C" int ptb_conv_tc_wgrad_f16x2(const void* dy_h, const void* dy_l, const void* x_h, const void* x_l, int B, int H, int W,
-                                       int Cout, int Cin, int taps, float scale, const float* dev_scale_dy, const float* dev_scale_x,
-                                       void* workspace, float* dw, int accumulate, void* stream) {
-  PTB_REQUIRE(B > 0 && H > 0 && W > 0 && (taps == 1 || taps == 9), "shape");
-  PTB_REQUIRE(Cin == WG_C && Cout > 0 && Cout <= WG_C && Cout % 8 == 0, "Cin must be 256, Cout a multiple of 8 up to 256");
-  PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
-  PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
-                  ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
-  return wgrad_run(dy_h, dy_l, Cout, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
-                   "ptb_conv_tc_wgrad_f16x2");
-}
-
 extern "C" int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, int ld_dy, const void* x_h, const void* x_l, int B, int H,
                                           int W, int Cout, int Cin, int taps, float scale, const float* dev_scale_dy,
                                           const float* dev_scale_x, void* workspace, float* dw, int accumulate, void* stream) {
@@ -326,8 +302,8 @@ extern "C" int ptb_conv_tc_wgrad_f16x2_ld(const void* dy_h, const void* dy_l, in
   PTB_REQUIRE(dy_h && dy_l && x_h && x_l && workspace && dw, "NULL input");
   PTB_REQUIRE(((uintptr_t)dy_h % 16 == 0) && ((uintptr_t)dy_l % 16 == 0) && ((uintptr_t)x_h % 16 == 0) && ((uintptr_t)x_l % 16 == 0) &&
                   ((uintptr_t)workspace % 16 == 0), "16-byte alignment");
-  return wgrad_run(dy_h, dy_l, ld_dy, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate, stream,
-                   "ptb_conv_tc_wgrad_f16x2_ld");
+  return wgrad_run(dy_h, dy_l, ld_dy, x_h, x_l, B, H, W, Cout, Cin, taps, scale, dev_scale_dy, dev_scale_x, workspace, dw, accumulate,
+                   stream);
 }
 
 extern "C" uint64_t ptb_col_sum_workspace(int64_t M, int N) {

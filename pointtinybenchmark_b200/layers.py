@@ -56,7 +56,7 @@ def bias_init_with_prob(p):
     return float(-math.log((1 - p) / p))
 
 
-_PACK_ATTRS = ('_ptb_packed_f16', '_ptb_packed_f16_t', '_ptb_packed', '_ptb_packed_tc', '_ptb_packed_tc_cols')
+_PACK_ATTRS = ('_ptb_packed_f16', '_ptb_packed_f16_t', '_ptb_packed', '_ptb_packed_tc')
 
 
 def invalidate_packed(module):
@@ -166,29 +166,17 @@ def _packed_weight(m):
     return m._ptb_packed[1]
 
 
-def _packed_tc(module, taps, tag):
-    """fp16 (h, l) packing of a Linear / Conv2d weight for ptb_conv_tc_f16x2, cached per parameter version."""
+def _packed_tc(module, taps):
+    """fp16 (h, l) column-slice packing (ops.conv_tc_pack_weight_f16) of a Linear (taps 1) / Conv2d (taps 9) weight for
+    ops.conv_tc_f16, cached per parameter version."""
     from . import ops
     w = module.weight
-    key = (w.data_ptr(), w._version, str(w.device), tag)
+    key = (w.data_ptr(), w._version, str(w.device), taps)
     cache = getattr(module, '_ptb_packed_tc', None)
     if cache is None or cache[0] != key:
         w2 = w.detach().reshape(w.shape[0], w.shape[1], -1) if w.dim() == 4 else w.detach()
         module._ptb_packed_tc = (key, ops.conv_tc_pack_weight_f16(w2.contiguous(), taps))
     return module._ptb_packed_tc[1]
-
-
-def _packed_tc_cols(module, taps):
-    """column-slice packing (ops.conv_tc_pack_weight_f16_cols) of a Linear (taps 1) / conv3x3 (taps 9) weight wider than one wgmma
-    launch, cached per version."""
-    from . import ops
-    w = module.weight
-    key = (w.data_ptr(), w._version, str(w.device), taps)
-    cache = getattr(module, '_ptb_packed_tc_cols', None)
-    if cache is None or cache[0] != key:
-        w2 = w.detach().reshape(w.shape[0], w.shape[1], -1) if w.dim() == 4 else w.detach()
-        module._ptb_packed_tc_cols = (key, ops.conv_tc_pack_weight_f16_cols(w2.contiguous(), taps))
-    return module._ptb_packed_tc_cols[1]
 
 
 INT32_MAX = 2 ** 31 - 1
@@ -220,7 +208,7 @@ def wide_out_conv_plan(B, H, W, n_out, k=1, backward=False):
 class _WideOutConvFn(torch.autograd.Function):
     """conv3x3 (pad 1, bias) from 256 channels to n_out > 512 on the tensor cores, with a deterministic hand-written backward:
     forward  ptb_split_f16 of the input, then one ptb_conv_tc_f16x2 launch per column slice of <= 512 into one (B,H,W,ldy) map
-             (ops.conv_tc_f16_cols; the columns from n_out to ldy are not written)
+             (ops.conv_tc_f16; the columns from n_out to ldy are not written)
     backward the (B,H,W,ldy) gradient split once (columns past n_out are zero: the caller takes the [..., :n_out] view), then
              dW: one ptb_conv_tc_wgrad_f16x2_ld per 256-column slice, read in place; db: ptb_col_sum; dX: ONE 9-tap conv with
              Cin = ldy on the transposed, flipped weights, zero-padded to ldy rows (ldy % 32 == 0, wide_out_conv_plan).
@@ -231,8 +219,8 @@ class _WideOutConvFn(torch.autograd.Function):
         from . import ops
         n_out = weight.shape[0]
         h, l, inv = ops.split_f16(xm, auto_scale=True)
-        packs = ops.conv_tc_pack_weight_f16_cols(weight.detach().reshape(n_out, weight.shape[1], 9).contiguous(), 9)
-        y = ops.conv_tc_f16_cols(h, l, packs, 9, n_out, bias=bias.detach(), dev_out_scale=inv, ldy=ldy)
+        packs = ops.conv_tc_pack_weight_f16(weight.detach().reshape(n_out, weight.shape[1], 9).contiguous(), 9)
+        y = ops.conv_tc_f16(h, l, packs, 9, n_out, bias=bias.detach(), dev_out_scale=inv, ldy=ldy)
         ctx.save_for_backward(h, l, inv, weight.detach())
         return y
 
@@ -246,7 +234,7 @@ class _WideOutConvFn(torch.autograd.Function):
         gh, gl, ginv = ops.split_f16(g, auto_scale=True)
         dw = db = dx = None
         if ctx.needs_input_grad[1]:
-            dw = ops.conv_tc_wgrad_f16_cols(gh, gl, h, l, 1.0, ginv, inv, taps=9)[:n_out]
+            dw = ops.conv_tc_wgrad_f16(gh, gl, h, l, 9, 1.0, ginv, inv)[:n_out]
         if ctx.needs_input_grad[2]:
             db = ops.col_sum(g.view(-1, ldy))[:n_out]
         if ctx.needs_input_grad[0]:
@@ -300,7 +288,7 @@ class _TowerTCFn(torch.autograd.Function):
     """[conv3x3 -> GroupNorm -> ReLU] x n on the tensor cores with a hand-written backward:
     forward  ptb_conv3x3_c256_f16_gn: the conv with GroupNorm statistics and the GroupNorm + ReLU apply in one launch
              (the next layer's fp16 pair, fp32 after the last layer)                         (csrc/conv_tc.cu)
-    backward ptb_gn_relu_bwd -> ptb_split_f16_amax -> ptb_conv3x3_wgrad_f16x2 (dW) and ptb_conv_tc_f16x2 with the transposed,
+    backward ptb_gn_relu_bwd -> ptb_split_f16_amax -> ptb_conv_tc_wgrad_f16x2_ld (dW) and ptb_conv_tc_f16x2 with the transposed,
              flipped weights (dX)                                                          (csrc/tower_bwd.cu, wgrad_tc.cu)
     Saved per layer: the fp16 operand pair of its input (re-used as the wgrad operand), the conv output y and the statistics.
     A half-precision input is saved itself instead of a pair (backward derives the pair again as forward did), and its gradient is
@@ -352,7 +340,7 @@ class _TowerTCFn(torch.autograd.Function):
             dyh, dyl, inv_dy = ops.split_f16_amax(dy, amax)
             grads[3 * i + 1], grads[3 * i + 2] = dg, db
             if ctx.needs_input_grad[2 + 3 * i]:
-                grads[3 * i] = ops.conv3x3_wgrad_f16(dyh, dyl, h, l, 1.0, inv_dy, inv_x)
+                grads[3 * i] = ops.conv_tc_wgrad_f16(dyh, dyl, h, l, 9, 1.0, inv_dy, inv_x)
             if i > 0 or ctx.needs_input_grad[0]:
                 # dgrad = the forward kernel with W^T and reversed taps
                 da = ops.conv_tc_f16(dyh, dyl, _packed_weight_f16_t(ctx.convs[i]), 9, w.shape[1], dev_out_scale=inv_dy,

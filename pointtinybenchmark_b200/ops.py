@@ -1191,49 +1191,22 @@ def split_f16_amax(x, amax_bits):
     return h, l, inv
 
 
-def conv3x3_wgrad_f16(dy_h, dy_l, x_h, x_l, scale=1.0, dev_scale_dy=None, dev_scale_x=None, out=None, accumulate=False):
-    """ptb_conv3x3_wgrad_f16x2: dW (Cout,Cin,3,3) = scale * s_dy * s_x * sum_pixels dy (x) x_shifted; operands are fp16 pairs
-    (B,H,W,256) channels-last."""
-    lib = _lib.load()
-    _chk(dy_h, torch.float16, 'dy_h'); _chk(dy_l, torch.float16, 'dy_l'); _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
-    B, H, W, Cout = dy_h.shape
-    Cin = x_h.shape[3]
-    ws = torch.empty(int(lib.ptb_conv3x3_wgrad_workspace(B, H, W)), dtype=torch.uint8, device=dy_h.device)
-    dw = out if out is not None else torch.empty((Cout, Cin, 3, 3), dtype=torch.float32, device=dy_h.device)
-    check(lib.ptb_conv3x3_wgrad_f16x2(_ptr(dy_h), _ptr(dy_l), _ptr(x_h), _ptr(x_l), B, H, W, Cout, Cin, float(scale), _ptr(dev_scale_dy),
-                                      _ptr(dev_scale_x), _ptr(ws), _ptr(dw), 1 if accumulate else 0, _stream()),
-          'ptb_conv3x3_wgrad_f16x2')
-    return dw
-
-
-def conv_tc_wgrad_f16(dy_h, dy_l, x_h, x_l, taps, scale=1.0, dev_scale_dy=None, dev_scale_x=None):
-    """ptb_conv_tc_wgrad_f16x2: dW (Cout, 256[, 3, 3]) of a conv3x3 (taps 9) / per-cell Linear (taps 1) from fp16 operand pairs
-    (B,H,W,Cout) and (B,H,W,256); tensor cores with K = pixels, deterministic."""
+def conv_tc_wgrad_f16(dy_h, dy_l, x_h, x_l, taps, scale=1.0, dev_scale_dy=None, dev_scale_x=None, out=None, accumulate=False):
+    """dW (Cout, 256, 3, 3) of a conv3x3 (taps 9) or (Cout, 256) of a per-cell Linear (taps 1) (+)= scale * s_dy * s_x *
+    sum_pixels dy (x) x_shifted from fp16 operand pairs dy (B,H,W,Cout) and x (B,H,W,256); tensor cores with K = pixels, deterministic.
+    One ptb_conv_tc_wgrad_f16x2_ld launch per column slice of <= 256 (the wgrad's widest output) of dy, read in place (row stride
+    Cout), writing rows [c0, c0 + n) of dW.  Cout a multiple of 8.  accumulate: add into out."""
     lib = _lib.load()
     _chk(dy_h, torch.float16, 'dy_h'); _chk(dy_l, torch.float16, 'dy_l'); _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
     B, H, W, Cout = dy_h.shape
     Cin = x_h.shape[3]
     ws = torch.empty(int(lib.ptb_conv_tc_wgrad_workspace(B, H, W, taps)), dtype=torch.uint8, device=dy_h.device)
-    dw = torch.empty((Cout, Cin, 3, 3) if taps == 9 else (Cout, Cin), dtype=torch.float32, device=dy_h.device)
-    check(lib.ptb_conv_tc_wgrad_f16x2(_ptr(dy_h), _ptr(dy_l), _ptr(x_h), _ptr(x_l), B, H, W, Cout, Cin, taps, float(scale), _ptr(dev_scale_dy),
-                                      _ptr(dev_scale_x), _ptr(ws), _ptr(dw), 0, _stream()), 'ptb_conv_tc_wgrad_f16x2')
-    return dw
-
-
-def conv_tc_wgrad_f16_cols(dy_h, dy_l, x_h, x_l, scale=1.0, dev_scale_dy=None, dev_scale_x=None, width=256, taps=1):
-    """dW (Cout, 256) of a per-cell Linear (taps 1), or (Cout, 256, 3, 3) of a conv3x3 (taps 9), whose output gradient dy (B,H,W,Cout)
-    is wider than one tensor-core wgrad (Cout <= 256): one ptb_conv_tc_wgrad_f16x2_ld launch per column slice [c0, c0 + width) of the
-    fp16 pair, read in place (row stride Cout), writing rows [c0, c0 + n) of dW.  Cout a multiple of 8."""
-    lib = _lib.load()
-    _chk(dy_h, torch.float16, 'dy_h'); _chk(dy_l, torch.float16, 'dy_l'); _chk(x_h, torch.float16, 'x_h'); _chk(x_l, torch.float16, 'x_l')
-    B, H, W, Cout = dy_h.shape
-    Cin = x_h.shape[3]
-    ws = torch.empty(int(lib.ptb_conv_tc_wgrad_workspace(B, H, W, taps)), dtype=torch.uint8, device=dy_h.device)
-    dw = torch.empty((Cout, Cin, 3, 3) if taps == 9 else (Cout, Cin), dtype=torch.float32, device=dy_h.device)
-    for c0 in range(0, Cout, width):
-        n = min(width, Cout - c0)
+    dw = out if out is not None else torch.empty((Cout, Cin, 3, 3) if taps == 9 else (Cout, Cin), dtype=torch.float32, device=dy_h.device)
+    for c0 in range(0, Cout, CONV_TC_WGRAD_N_MAX):
+        n = min(CONV_TC_WGRAD_N_MAX, Cout - c0)
         check(lib.ptb_conv_tc_wgrad_f16x2_ld(_ptr(dy_h[..., c0:]), _ptr(dy_l[..., c0:]), Cout, _ptr(x_h), _ptr(x_l), B, H, W, n, Cin, taps,
-                                             float(scale), _ptr(dev_scale_dy), _ptr(dev_scale_x), _ptr(ws), _ptr(dw[c0:]), 0, _stream()),
+                                             float(scale), _ptr(dev_scale_dy), _ptr(dev_scale_x), _ptr(ws), _ptr(dw[c0:]),
+                                             1 if accumulate else 0, _stream()),
               'ptb_conv_tc_wgrad_f16x2_ld')
     return dw
 
@@ -1249,8 +1222,11 @@ def col_sum(y2d):
     return out
 
 
-def conv_tc_pack_weight_f16(w, taps):
-    """weights of a conv3x3 (n_out,Cin,3,3) or Linear / conv1x1 (n_out,Cin) -> packed fp16 (h, l), 1/scale, n_mma."""
+CONV_TC_N_MAX = 512         # widest output of one ptb_conv_tc_f16x2 launch
+CONV_TC_WGRAD_N_MAX = 256   # widest output of one ptb_conv_tc_wgrad_f16x2_ld launch
+
+
+def _pack_slice_f16(w, taps):
     lib = _lib.load()
     w = _chk(w.detach().contiguous(), torch.float32, 'w')
     n_out, Cin = w.shape[0], w.shape[1]
@@ -1264,67 +1240,47 @@ def conv_tc_pack_weight_f16(w, taps):
     return h, l, 1.0 / scale, n_mma
 
 
-CONV_TC_N_MAX = 512       # widest output of one ptb_conv_tc_f16x2 launch
-
-
-def conv_tc_pack_weight_f16_cols(w, taps, width=CONV_TC_N_MAX):
-    """column slices [c0, c0 + width) of a weight wider than one wgmma launch, each packed by conv_tc_pack_weight_f16 (its own scale):
-    [(c0, n, packed), ...] for conv_tc_f16_cols."""
-    return [(c0, min(width, w.shape[0] - c0), conv_tc_pack_weight_f16(w[c0:c0 + width], taps)) for c0 in range(0, w.shape[0], width)]
-
-
-def conv_tc_f16_cols(x_h, x_l, packs, taps, n_out, bias=None, dev_out_scale=None, ldy=None):
-    """conv_tc_f16 at any n_out: one wgmma launch per column slice of conv_tc_pack_weight_f16_cols, each writing columns
-    [c0, c0 + n) of one (B,H,W,ldy) fp32 map (+bias).  x_l None: x_h is used as is (ptb_conv_tc_f16x1a)."""
-    lib = _lib.load()
-    _chk(x_h, torch.float16, 'x_h')
-    if x_l is not None:
-        _chk(x_l, torch.float16, 'x_l')
-    B, H, W, Cin = x_h.shape
-    ldy = ldy or (n_out + 3) // 4 * 4
-    y = torch.empty((B, H, W, ldy), dtype=torch.float32, device=x_h.device)
-    if packs[-1][0] + packs[-1][1] != n_out:
-        raise ValueError(f'conv_tc_f16_cols: the packed slices cover {packs[-1][0] + packs[-1][1]} columns, not n_out = {n_out}')
-    for c0, n, (w_h, w_l, inv_w, n_mma) in packs:
-        yc, bc = y[..., c0:], (bias[c0:c0 + n] if bias is not None else None)
-        if x_l is None:
-            check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w), _ptr(dev_out_scale),
-                                         _ptr(bc), _ptr(yc), ldy, None, _stream()), 'ptb_conv_tc_f16x1a')
-        else:
-            check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w),
-                                        _ptr(dev_out_scale), _ptr(bc), _ptr(yc), ldy, _stream()), 'ptb_conv_tc_f16x2')
-    return y
+def conv_tc_pack_weight_f16(w, taps):
+    """weights of a conv3x3 (n_out,Cin,3,3) or Linear / conv1x1 (n_out,Cin) -> column slices of <= CONV_TC_N_MAX output rows for
+    conv_tc_f16, each packed as fp16 (h, l) with its own power-of-two scale: [(c0, n, (h, l, 1/scale, n_mma)), ...]."""
+    return [(c0, min(CONV_TC_N_MAX, w.shape[0] - c0), _pack_slice_f16(w[c0:c0 + CONV_TC_N_MAX], taps))
+            for c0 in range(0, w.shape[0], CONV_TC_N_MAX)]
 
 
 HALF_DTYPES = {torch.float16: 1, torch.bfloat16: 2}      # PTB_DTYPE_F16, PTB_DTYPE_BF16
 
 
-def conv_tc_f16(x_h, x_l, packed, taps, n_out, bias=None, dev_out_scale=None, ldy=None, out_dtype=torch.float32):
-    """general wgmma conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias).  x_l None: x_h is an fp16 tensor used as is
+def conv_tc_f16(x_h, x_l, packs, taps, n_out, bias=None, dev_out_scale=None, ldy=None, out_dtype=torch.float32):
+    """general wgmma conv (taps 1|9) on fp16 operand pairs -> (B,H,W,ldy) fp32 (+bias), at any n_out: one launch per column slice
+    of conv_tc_pack_weight_f16, each writing columns [c0, c0 + n) of the one map.  x_l None: x_h is an fp16 tensor used as is
     (lo == 0: ptb_conv_tc_f16x1a).  out_dtype fp16 / bf16: the fp32 result rounded to nearest even in the epilogue
     (ptb_conv_tc_f16x2_half_out), the input gradient of a half-precision feature map."""
     lib = _lib.load()
     _chk(x_h, torch.float16, 'x_h')
-    w_h, w_l, inv_w, n_mma = packed
-    B, H, W, Cin = x_h.shape
-    ldy = ldy or (n_out + 3) // 4 * 4
-    y = torch.empty((B, H, W, ldy), dtype=out_dtype, device=x_h.device)
     if x_l is None:
         if out_dtype != torch.float32:
             raise NotImplementedError('conv_tc_f16: a half-precision output of the lo == 0 variant')
-        check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w), _ptr(dev_out_scale),
-                                     _ptr(bias), _ptr(y), ldy, None, _stream()), 'ptb_conv_tc_f16x1a')
-        return y
-    _chk(x_l, torch.float16, 'x_l')
-    if out_dtype == torch.float32:
-        check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w),
-                                    _ptr(dev_out_scale), _ptr(bias), _ptr(y), ldy, _stream()), 'ptb_conv_tc_f16x2')
     else:
-        if out_dtype not in HALF_DTYPES:
-            raise TypeError(f'conv_tc_f16: out_dtype must be float32, float16 or bfloat16, got {out_dtype}')
-        check(lib.ptb_conv_tc_f16x2_half_out(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n_out, n_mma, float(inv_w),
-                                             _ptr(dev_out_scale), _ptr(bias), _ptr(y), HALF_DTYPES[out_dtype], ldy, _stream()),
-              'ptb_conv_tc_f16x2_half_out')
+        _chk(x_l, torch.float16, 'x_l')
+    if out_dtype != torch.float32 and out_dtype not in HALF_DTYPES:
+        raise TypeError(f'conv_tc_f16: out_dtype must be float32, float16 or bfloat16, got {out_dtype}')
+    if packs[-1][0] + packs[-1][1] != n_out:
+        raise ValueError(f'conv_tc_f16: the packed slices cover {packs[-1][0] + packs[-1][1]} columns, not n_out = {n_out}')
+    B, H, W, Cin = x_h.shape
+    ldy = ldy or (n_out + 3) // 4 * 4
+    y = torch.empty((B, H, W, ldy), dtype=out_dtype, device=x_h.device)
+    for c0, n, (w_h, w_l, inv_w, n_mma) in packs:
+        yc, bc = y[..., c0:], (bias[c0:c0 + n] if bias is not None else None)
+        if x_l is None:
+            check(lib.ptb_conv_tc_f16x1a(_ptr(x_h), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w), _ptr(dev_out_scale),
+                                         _ptr(bc), _ptr(yc), ldy, None, _stream()), 'ptb_conv_tc_f16x1a')
+        elif out_dtype == torch.float32:
+            check(lib.ptb_conv_tc_f16x2(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w),
+                                        _ptr(dev_out_scale), _ptr(bc), _ptr(yc), ldy, _stream()), 'ptb_conv_tc_f16x2')
+        else:
+            check(lib.ptb_conv_tc_f16x2_half_out(_ptr(x_h), _ptr(x_l), _ptr(w_h), _ptr(w_l), B, H, W, Cin, taps, n, n_mma, float(inv_w),
+                                                 _ptr(dev_out_scale), _ptr(bc), _ptr(yc), HALF_DTYPES[out_dtype], ldy, _stream()),
+                  'ptb_conv_tc_f16x2_half_out')
     return y
 
 

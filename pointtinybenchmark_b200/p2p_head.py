@@ -24,7 +24,7 @@ from . import ops
 from .assigners import cost_matrix, match_cost_terms
 from .post_processing import check_split_thr
 from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, wide_out_conv, \
-    wide_out_conv_plan, _packed_tc, _packed_tc_cols
+    wide_out_conv_plan, _packed_tc
 from .registry import CfgNode, register_head
 
 
@@ -220,13 +220,12 @@ class P2PHead(PackedWeightsMixin, nn.Module):
                 if pc is not None and pr is not None:
                     self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
                     nc, nr = self.cls_out.out_channels, self.reg_out.out_channels
-                    if nc > MAX_OUT_CHANNELS:      # one launch per 512-column slice; ldy = ceil4(nc): [..., :nc] is the whole map if 4 | nc
+                    ldy = None
+                    if nc > MAX_OUT_CHANNELS:      # ldy = ceil4(nc): [..., :nc] is the whole map if 4 | nc
                         B_, H_, W_ = pc[0].shape[:3]
-                        yc = ops.conv_tc_f16_cols(pc[0], pc[1], _packed_tc_cols(self.cls_out, 9), 9, nc, bias=self.cls_out.bias.detach(),
-                                                  ldy=wide_out_conv_plan(B_, H_, W_, nc, self.num_points))
-                    else:
-                        yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9, 'conv'), 9, nc, bias=self.cls_out.bias.detach())
-                    yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9, 'conv'), 9, nr, bias=self.reg_out.bias.detach())
+                        ldy = wide_out_conv_plan(B_, H_, W_, nc, self.num_points)
+                    yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9), 9, nc, bias=self.cls_out.bias.detach(), ldy=ldy)
+                    yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9), 9, nr, bias=self.reg_out.bias.detach())
                     cls_outs.append(yc[..., :nc].permute(0, 3, 1, 2))
                     pts_outs.append(yr[..., :nr].permute(0, 3, 1, 2))
                     continue

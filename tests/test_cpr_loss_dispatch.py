@@ -1,11 +1,11 @@
-"""CPU checks of the CPR loss plumbing: the backward-path choice of the fused loss (cpr_head.loss_bwd_plan), the reach of a bag offset
-table, and the float64 loss reference of tests/cpr_loss_ref.py against the oracle's fp32 autograd."""
+"""CPU checks of the CPR loss plumbing: the backward-path choice of the fused loss (cpr_head.loss_bwd_plan), the logit map's GEMM
+path, the reach of a bag offset table, and the float64 loss reference of tests/cpr_loss_ref.py against the oracle's fp32 autograd."""
 import pytest
 import torch
 
 from oracle import cpr as ocpr
 from pointtinybenchmark_b200 import ops
-from pointtinybenchmark_b200.cpr_head import _CircleBags, loss_bwd_plan
+from pointtinybenchmark_b200.cpr_head import _CircleBags, _loss_map_on_tc, loss_bwd_plan
 from tests.cpr_loss_ref import cpr_loss_ref, oracle_bag_logits, taps
 from tests.helpers import scale_rel_err
 
@@ -49,6 +49,22 @@ def test_explicit_atomic_path_under_deterministic_mode_is_flagged(env_mode):
 def test_n80_layout_is_the_same_in_every_mode():
     """N = 80 (COCO): NP = 80 whether or not the gradients must be bit-reproducible, so the training bits do not depend on the mode."""
     assert loss_bwd_plan(80, 289, True, True)[0] == loss_bwd_plan(80, 289, True, True, None, True)[0] == 80
+
+
+@pytest.mark.parametrize('deterministic', [False, True])
+@pytest.mark.parametrize('C', [32, 48, 128, 256])
+@pytest.mark.parametrize('N', [1, 20, 80, 128, 129, 200, 256, 257, 365, 1203, 1280])
+def test_logit_map_path_choice(N, C, deterministic):
+    """the logit map runs on the tensor cores for exactly the shapes of the two tensor-core branches it replaces (one launch: C, LD <= 256
+    with C and LD multiples of 32; column slices: more than 256 classes with C % 32 == 0), FFMA for every other shape; and at C = 256
+    every shape whose map ran on the tensor cores took one of those branches' tensor-core backwards, which is now the one taken."""
+    NP = loss_bwd_plan(N, 121, True, True, None, deterministic)[0]
+    LD = 2 * NP
+    one_launch = C % 32 == 0 and LD % 32 == 0 and C <= 256 and LD <= 256
+    sliced = not one_launch and N > 256 and C % 32 == 0
+    assert _loss_map_on_tc(N, C, LD) == (one_launch or sliced), (N, C, LD)
+    if C == 256 and (one_launch or sliced):
+        assert (LD > 256 and LD % 32 == 0) or (one_launch and LD % 8 == 0), (N, LD)
 
 
 def test_offsets_reach_is_cached_on_the_tensor():

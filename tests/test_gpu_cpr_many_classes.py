@@ -4,8 +4,8 @@
     sides of every chunk boundary up to the 1280-class limit, both loss kinds, bags of 1, 33 and 289 samples and a zero-weight bag;
     bag_acc with a planted tie across a chunk boundary;
   * ptb_cpr_neg_mask in class chunks (above 736 classes) bit-exact against the oracle (torch.cdist on the host);
-  * the logit-map GEMMs at LD = 256 .. 2416 on the tensor cores against fp64: the column-sliced forward (ops.conv_tc_f16_cols), dW in
-    column slices (ops.conv_tc_wgrad_f16_cols) and dX; the head's tensor-core backward against the FFMA kernels;
+  * the logit-map GEMMs at LD = 256 .. 2416 on the tensor cores against fp64: the column-sliced forward (ops.conv_tc_f16), dW in
+    column slices (ops.conv_tc_wgrad_f16) and dX; the head's tensor-core backward against the FFMA kernels;
   * the head at 365 and 1203 classes against the golden vectors of the reference (oracle/make_golden_cpr_many_classes.py), refine through
     the margin harness, simple_test's sliced inference map, and the refusal above 1280 classes.
 Tolerances as in tests/test_gpu_cpr_loss_types.py (kernels) and tests/test_gpu_cpr_loss_types.py::test_head_against_oracle_and_golden
@@ -139,7 +139,7 @@ def test_neg_mask_class_chunks_bit_exact(ops, N, class_wise):
 
 
 @pytest.mark.parametrize('LD', [256, 264, 520, 2416])
-def test_logit_map_gemms_on_tensor_cores(ops, LD):
+def test_logit_map_gemms_in_column_slices(ops, LD):
     """the logit map's three GEMMs on the tensor cores against fp64: the forward as column slices of the wgmma conv (1e-4), dW as column
     slices of <= 256 of the gradient's fp16 pair read in place (2e-4), and dX as one conv with Cin = LD (2e-4) at the width the head
     gives it (loss_bwd_plan pads LD to a multiple of 32 above 256 classes: 264 -> 288, 520 -> 544, 2416 -> 2432)."""
@@ -150,12 +150,12 @@ def test_logit_map_gemms_on_tensor_cores(ops, LD):
     bias = torch.randn(LD, generator=g) * 0.1
     dx, dw_, db_ = x.cuda(), w.cuda(), bias.cuda()
     fh, fl, finv = ops.split_f16(dx, auto_scale=True)
-    y = ops.conv_tc_f16_cols(fh, fl, ops.conv_tc_pack_weight_f16_cols(dw_, 1), 1, LD, bias=db_, dev_out_scale=finv, ldy=LD)
+    y = ops.conv_tc_f16(fh, fl, ops.conv_tc_pack_weight_f16(dw_, 1), 1, LD, bias=db_, dev_out_scale=finv, ldy=LD)
     ref = x.reshape(-1, C).double() @ w.double().t() + bias.double()
     assert_close(y.reshape(-1, LD), ref, 1e-4, f'LD={LD} sliced map')
     dy = torch.randn(B, H, W, LD, generator=g)
     dh, dl, dinv = ops.split_f16(dy.cuda(), auto_scale=True)
-    gw = ops.conv_tc_wgrad_f16_cols(dh, dl, fh, fl, 1.0, dinv, finv)
+    gw = ops.conv_tc_wgrad_f16(dh, dl, fh, fl, 1, 1.0, dinv, finv)
     assert_close(gw, dy.reshape(-1, LD).double().t() @ x.reshape(-1, C).double(), 2e-4, f'LD={LD} dW')
     LDx = (LD + 31) // 32 * 32
     dyx = torch.zeros(B, H, W, LDx)
@@ -168,10 +168,11 @@ def test_logit_map_gemms_on_tensor_cores(ops, LD):
 
 
 @pytest.mark.parametrize('N', [365, 1203])
-def test_head_backward_gemms_on_tensor_cores(ops, N):
+def test_head_backward_gemms_on_tensor_cores(ops, monkeypatch, N):
     """CPRHead.loss + backward at 256 feature channels: the tensor-core logit-map GEMMs (forward slices, sliced dW, dX conv) against the
-    fp32 FFMA kernels (PTB_LOSS_GEMM=ffma) on the same inputs: losses 1e-4, gradients 2e-4."""
+    fp32 FFMA kernels (the shape predicate forced off) on the same inputs: losses 1e-4, gradients 2e-4."""
     from oracle import synth
+    from pointtinybenchmark_b200 import cpr_head
     dev = torch.device('cuda:0')
     inp = synth.cpr_inputs('lite', 7000 + N, num_classes=N, n=16)
     head = _head(N, 256, dev, inp['weights'])
@@ -179,16 +180,14 @@ def test_head_backward_gemms_on_tensor_cores(ops, N):
     gtl = [l.to(dev) for l in inp['gt_labels']]
     runs = {}
     for mode in ('tc', 'ffma'):
-        os.environ['PTB_LOSS_GEMM'] = mode
-        try:
-            head.zero_grad(set_to_none=True)
-            feat = inp['cls_feat'].to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
-            losses = head.loss([feat], [feat], gtb, gtl, inp['img_metas'])
-            sum(v for k, v in losses.items() if 'loss' in k).backward()
-            runs[mode] = (losses, [feat.grad.clone(), head.cls_out.weight.grad.clone(), head.cls_out.bias.grad.clone(),
-                                   head.ins_out.weight.grad.clone()])
-        finally:
-            os.environ.pop('PTB_LOSS_GEMM', None)
+        if mode == 'ffma':
+            monkeypatch.setattr(cpr_head, '_loss_map_on_tc', lambda *a: False)
+        head.zero_grad(set_to_none=True)
+        feat = inp['cls_feat'].to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+        losses = head.loss([feat], [feat], gtb, gtl, inp['img_metas'])
+        sum(v for k, v in losses.items() if 'loss' in k).backward()
+        runs[mode] = (losses, [feat.grad.clone(), head.cls_out.weight.grad.clone(), head.cls_out.bias.grad.clone(),
+                               head.ins_out.weight.grad.clone()])
     (lt, gt_), (lf, gf) = runs['tc'], runs['ffma']
     for k in ('gt_loss', 'pos_loss', 'neg_loss'):
         assert_close(lt[k].reshape(-1), lf[k].reshape(-1), 1e-4, f'N={N} {k}')
@@ -265,7 +264,7 @@ def test_head_against_reference_golden(ops, golden_dir, N, mode):
 
 
 @pytest.mark.parametrize('N', [600, 1203])
-def test_simple_test_sliced_logit_map(ops, monkeypatch, N):
+def test_simple_test_logit_map_in_column_slices(ops, monkeypatch, N):
     """simple_test above 512 classes: the class-logit map from column slices of the wgmma kernel on the towers' fp16 pair, refined; its
     probabilities against the oracle on the head's own fp32 tower output through the margin harness (bound 1e-4: fp16-split map)."""
     from oracle import synth
@@ -278,8 +277,8 @@ def test_simple_test_sliced_logit_map(ops, monkeypatch, N):
     gtl = [l.to(dev) for l in inp['gt_labels']]
     x = torch.randn(1, 256, 32, 32, generator=torch.Generator().manual_seed(N)).to(dev)
     calls = []
-    sliced = ops.conv_tc_f16_cols
-    monkeypatch.setattr(ops, 'conv_tc_f16_cols', lambda *a, **k: calls.append(a[4]) or sliced(*a, **k))
+    conv = ops.conv_tc_f16
+    monkeypatch.setattr(ops, 'conv_tc_f16', lambda *a, **k: calls.append((a[4], len(a[2]))) or conv(*a, **k))
     with torch.no_grad():
         res = head.simple_test((x,), inp['img_metas'], gt_bboxes=gtb, gt_labels=gtl)
         feat = head.forward((x,))[0][0]
@@ -289,7 +288,7 @@ def test_simple_test_sliced_logit_map(ops, monkeypatch, N):
                                       oracle_cfg(d), return_all=True)
         gt = _BatchGT(gtb, gtl, inp['img_metas'], dev)
         got = head.refine_points(feat, gt, want_chosen=True)
-    assert calls == [N], f'simple_test did not take the sliced tensor-core map: {calls}'
+    assert calls == [(N, (N + 511) // 512)], f'simple_test did not take the sliced tensor-core map: {calls}'
     check_refine_against_oracle(got, _cat_refine(allo), allo['bag_prob'][:, 0], torch.cat(inp['gt_labels']), oracle_cfg(d), 1e-4,
                                 f'N={N} get_bboxes')
     det, det_ref = res[0][0].cpu(), ref_res[0][0].cpu()

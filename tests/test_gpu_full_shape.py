@@ -55,7 +55,7 @@ def config2():
 
 
 @pytest.mark.parametrize('variant', ['bench_weights', 'spread'])
-def test_config2_full_shape_product_step_vs_oracle(config2, variant):
+def test_config2_full_shape_product_step_and_pieces_vs_oracle(config2, variant):
     from pointtinybenchmark_b200 import ops
     from pointtinybenchmark_b200.cpr_head import _BatchGT
     from pointtinybenchmark_b200.layers import tower, _packed_tc
@@ -81,7 +81,7 @@ def test_config2_full_shape_product_step_vs_oracle(config2, variant):
         # the same step in pieces, to look inside: fp16 pair of the tower output -> logit map -> fused refine with the chosen mask
         info = {}
         h, l = tower(head.cls_convs, x, info, want='f16pair')
-        lmap = ops.conv_tc_f16(h, l, _packed_tc(head.cls_out, 1, 'lin'), 1, head.num_classes, bias=head.cls_out.bias.detach())
+        lmap = ops.conv_tc_f16(h, l, _packed_tc(head.cls_out, 1), 1, head.num_classes, bias=head.cls_out.bias.detach())
         gt = _BatchGT(gtb, gtl, metas, dev)
         got = head._refine_from_logit_map(lmap, gt, want_chosen=True)
         feat_g = head((x,))[0][0]

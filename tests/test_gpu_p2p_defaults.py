@@ -55,7 +55,7 @@ def build(inp, **over):
 
 @pytest.mark.parametrize('n_out', [264, 320, 512])
 @pytest.mark.parametrize('taps', [1, 9])
-def test_wide_conv_matches_fp32(ops, n_out, taps):
+def test_wide_conv_one_slice_matches_fp32(ops, n_out, taps):
     """ptb_conv_tc_f16x2 beyond 256 output channels (3 / 3 / 4 channel slices of 128 in one launch), with bias, on a map with partial
     edge tiles, against torch's fp32 conv (float64 reference)."""
     dev = torch.device('cuda:0')
@@ -67,7 +67,8 @@ def test_wide_conv_matches_fp32(ops, n_out, taps):
     ref = F.conv2d(x.double(), w.double(), b.double(), 1, 1 if taps == 9 else 0).float()
     h, l, dinv = ops.split_f16(ops.to_nhwc(x.to(dev)).contiguous(), auto_scale=True)
     packed = ops.conv_tc_pack_weight_f16(w.reshape(n_out, C, taps).to(dev), taps)
-    assert packed[3] == (n_out + 15) // 16 * 16
+    [(c0, n, (_, _, _, n_mma))] = packed                 # one slice, one launch, up to 512 channels
+    assert (c0, n, n_mma) == (0, n_out, (n_out + 15) // 16 * 16)
     y = ops.conv_tc_f16(h, l, packed, taps, n_out, bias=b.to(dev), dev_out_scale=dinv)
     assert y.shape[-1] == (n_out + 3) // 4 * 4
     assert_close(y[..., :n_out].permute(0, 3, 1, 2), ref, 1e-4, f'wide tc conv taps={taps} N={n_out}')

@@ -89,7 +89,7 @@ def test_wide_conv_forward_and_backward_match_float64(ops, n_out, H, W):
     assert torch.equal(y, y2) and torch.equal(dx, dx2) and torch.equal(dw, dw2) and torch.equal(db, db2), 'bit-identical reruns'
 
 
-def test_512_channels_keep_the_single_launch_and_cudnn_training(ops):
+def test_512_channels_keep_one_slice_and_cudnn_training(ops):
     """at 512 channels (128 classes x 4 anchors) inference is the one ptb_conv_tc_f16x2 launch, bit for bit, and training runs cuDNN;
     at 257 classes (1028 channels) training runs the wide conv."""
     from pointtinybenchmark_b200.layers import _packed_tc, tower
@@ -101,7 +101,7 @@ def test_512_channels_keep_the_single_launch_and_cudnn_training(ops):
     with torch.no_grad():
         cls_outs, _ = head.forward((x,))
         h, l = tower(head.cls_convs, x, {}, want='f16pair')
-        ref = ops.conv_tc_f16(h, l, _packed_tc(head.cls_out, 9, 'conv'), 9, 512, bias=head.cls_out.bias.detach())
+        ref = ops.conv_tc_f16(h, l, _packed_tc(head.cls_out, 9), 9, 512, bias=head.cls_out.bias.detach())
     assert torch.equal(cls_outs[0], ref.permute(0, 3, 1, 2))
     head.train()
     cls_outs, _ = head.forward((x,))

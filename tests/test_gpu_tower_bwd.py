@@ -51,7 +51,7 @@ def test_gn_relu_bwd_matches_fp64_autograd(ops, B, H, W):
 
 
 @pytest.mark.parametrize('B,H,W', [(2, 19, 37), (1, 8, 16), (8, 100, 168)])
-def test_wgrad_and_dgrad_match_fp64(ops, B, H, W):
+def test_tc_wgrad_and_dgrad_match_fp64(ops, B, H, W):
     dev = torch.device('cuda:0')
     g = torch.Generator(device='cpu').manual_seed(H)
     C = 256
@@ -61,7 +61,7 @@ def test_wgrad_and_dgrad_match_fp64(ops, B, H, W):
     xh, xl, inv_x = ops.split_f16(x, auto_scale=True)
     amax = dy.abs().max().reshape(1).view(torch.int32)
     dh, dl, inv_dy = ops.split_f16_amax(dy, amax)
-    dw = ops.conv3x3_wgrad_f16(dh, dl, xh, xl, 1.0, inv_dy, inv_x)
+    dw = ops.conv_tc_wgrad_f16(dh, dl, xh, xl, 9, 1.0, inv_dy, inv_x)
     wt = w.flip(2, 3).transpose(0, 1).reshape(C, C, 9).contiguous()
     dx = ops.conv_tc_f16(dh, dl, ops.conv_tc_pack_weight_f16(wt, 9), 9, C, dev_out_scale=inv_dy)
     xd = x.double().permute(0, 3, 1, 2).requires_grad_(True)
@@ -77,9 +77,9 @@ def test_wgrad_and_dgrad_match_fp64(ops, B, H, W):
         print(f'    cuDNN fp32: wgrad err {scale_rel_err(wf.grad, ref_dw):.2e}, dgrad err {scale_rel_err(xf.grad.permute(0, 2, 3, 1), ref_dx):.2e}')
     e1 = assert_close(dw, ref_dw, 5e-5, 'dW (wgmma wgrad, MN-major operands)')
     e2 = assert_close(dx, ref_dx, 2e-5, 'dX (forward kernel on W^T flipped)')
-    dw2 = ops.conv3x3_wgrad_f16(dh, dl, xh, xl, 1.0, inv_dy, inv_x, out=dw.clone(), accumulate=True)
+    dw2 = ops.conv_tc_wgrad_f16(dh, dl, xh, xl, 9, 1.0, inv_dy, inv_x, out=dw.clone(), accumulate=True)
     assert_close(dw2, 2 * ref_dw, 5e-5, 'accumulate')
-    assert torch.equal(ops.conv3x3_wgrad_f16(dh, dl, xh, xl, 1.0, inv_dy, inv_x), dw), 'deterministic'
+    assert torch.equal(ops.conv_tc_wgrad_f16(dh, dl, xh, xl, 9, 1.0, inv_dy, inv_x), dw), 'deterministic'
 
 
 def _tower_modules(weights, dev, dtype):
@@ -175,7 +175,7 @@ def test_tower_training_path_vs_fp64_and_oracle(ops):
 @pytest.mark.parametrize('B,H,W,Cout', [(2, 13, 21, 160), (1, 100, 168, 160), (1, 9, 16, 80)])
 def test_one_tap_wgrad_and_col_sum_match_fp64(ops, B, H, W, Cout):
     """dW / db of the logit-map Linear (cls_out | ins_out stacked, cpr_head.py:1045-1078 under autograd) on the tensor cores:
-    ptb_conv_tc_wgrad_f16x2 with taps = 1 (K = pixels) and ptb_col_sum against float64, plus run-to-run bit equality."""
+    ptb_conv_tc_wgrad_f16x2_ld with taps = 1 (K = pixels) and ptb_col_sum against float64, plus run-to-run bit equality."""
     dev = torch.device('cuda:0')
     g = torch.Generator().manual_seed(B * 100 + Cout)
     x = torch.relu(torch.randn(B, H, W, 256, generator=g)).to(dev)

@@ -46,7 +46,7 @@ res['gn_relu_bwd'] = dict(ms=t(lambda: ops.gn_relu_bwd(da, y16, st16, gn.weight.
 dy, _, _, amax = ops.gn_relu_bwd(da, y16, st16, gn.weight.detach(), gn.bias.detach())
 res['split_f16_amax'] = dict(ms=t(lambda: ops.split_f16_amax(dy, amax)))
 dyh, dyl, inv_dy = ops.split_f16_amax(dy, amax)
-ms = t(lambda: ops.conv3x3_wgrad_f16(dyh, dyl, h16, l16, 1.0, inv_dy, dinv))
+ms = t(lambda: ops.conv_tc_wgrad_f16(dyh, dyl, h16, l16, 9, 1.0, inv_dy, dinv))
 res['tc_wgrad_f16x2'] = dict(ms=ms, eff_tflops=flops / ms / 1e9, f16_mma_tflops=3 * flops / ms / 1e9)
 wt = conv.weight.detach().flip(2, 3).transpose(0, 1).reshape(C, C, 9).contiguous()
 pk = ops.conv_tc_pack_weight_f16(wt, 9)

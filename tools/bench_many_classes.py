@@ -104,9 +104,7 @@ def run(N, B, iters, warmup, dev):
 
     def tc_dw():
         dh, dl, dinv = ops.split_f16(dyv, auto_scale=True)
-        if LD <= 256:
-            return ops.conv_tc_wgrad_f16(dh, dl, xh, xl, 1, 1.0, dinv, xinv)
-        return ops.conv_tc_wgrad_f16_cols(dh, dl, xh, xl, 1.0, dinv, xinv)
+        return ops.conv_tc_wgrad_f16(dh, dl, xh, xl, 1, 1.0, dinv, xinv)
 
     def tc_dx():
         dh, dl, dinv = ops.split_f16(dyv, auto_scale=True)

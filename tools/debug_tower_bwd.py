@@ -60,5 +60,5 @@ for i in reversed(range(4)):
     da = ops.conv_tc_f16(dyh, dyl, ops.conv_tc_pack_weight_f16(wt, 9), 9, C, dev_out_scale=inv_dy)
     check(f'dgrad[{i}]')
     print('   da err', err(da, nhwc(acts[i].grad)))
-    dw = ops.conv3x3_wgrad_f16(dyh, dyl, h, l, 1.0, inv_dy, dinv if i == 0 else None)
+    dw = ops.conv_tc_wgrad_f16(dyh, dyl, h, l, 9, 1.0, inv_dy, dinv if i == 0 else None)
     check(f'wgrad[{i}]')

@@ -37,6 +37,6 @@ for _ in range(int(sys.argv[1]) if len(sys.argv) > 1 else 3):
     # training tower backward of one layer
     dy, dg, db, amax = ops.gn_relu_bwd(da, y16, st16, gamma, beta)
     dyh, dyl, inv_dy = ops.split_f16_amax(dy, amax)
-    ops.conv3x3_wgrad_f16(dyh, dyl, h16, l16, 1.0, inv_dy, dinv)
+    ops.conv_tc_wgrad_f16(dyh, dyl, h16, l16, 9, 1.0, inv_dy, dinv)
     ops.conv_tc_f16(dyh, dyl, packed_t, 9, 256, dev_out_scale=inv_dy)
 torch.cuda.synchronize()
