@@ -708,6 +708,45 @@ int ptb_rpn_level_loss(const float* cls_score, const float* bbox_pred, const int
                        const float* bbox_targets, const float* bbox_weights, int64_t M, int bbox_loss, float beta, float* loss_sum /*[2]*/,
                        const float* scale /*[2] or NULL*/, float* grad_cls, float* grad_bbox, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * The bbox branch of StandardRoIHead (roi_heads/standard_roi_head.py, bbox_heads/bbox_head.py) with SingleRoIExtractor and mmcv's
+ * RoIAlign(aligned=True, pool_mode='avg').  featmap_hw [L][2] and strides [L] (spatial_scale = 1 / stride) are host arrays.
+ *   ptb_roi_align_fwd   maps[l]: channels-last [B][H_l][W_l][C] (C a multiple of 4, 16-byte aligned); rois [R][5] (batch index, x1, y1,
+ *                       x2, y2).  levels[R] = floor(log2(sqrt(w h) / finest_scale + 1e-6)) clamped to [0, L-1] (-1 for a NaN scale,
+ *                       whose features stay 0; L == 1: level 0); y [R][C][out][out] = the RoI's bins on its level, ceil(roi / out)
+ *                       samples per bin side when sampling_ratio <= 0.
+ *   ptb_roi_align_bwd   grad_maps[l] (channels-last like the maps, zeroed by the caller) += the scatter of grad_y through the forward's
+ *                       taps (float atomics); levels from ptb_roi_align_fwd.
+ *   ptb_roi_targets     candidates cand [B][N][4] = each image's [GTs; proposals] padded to N, gt_inds [B][N] (MaxIoUAssigner with the
+ *                       GTs assigned to themselves, -1 on padding), rank from ptb_rpn_candidate_ranks, the sample plan of
+ *                       ptb_rpn_anchor_targets, row_off [B][2] = first output row of image b's positives / negatives.  Writes the
+ *                       sampled rows: rois [R][5], labels [R] (gt label or num_classes), label_weights [R] (pos_weight > 0 or 1 for
+ *                       positives, 1 for negatives), bbox_targets [R][4] (bbox2delta, then (delta - mean) / std) and bbox_weights [R][4].
+ *   ptb_roi_bbox_loss   sum over the positive rows of L1Loss / SmoothL1Loss(beta) * bbox_weights between bbox_pred's class columns
+ *                       (4 label .. 4 label + 3 of [R][ld], ld = 4 num_classes; columns 0..3 when class_agnostic, ld = 4) and the
+ *                       targets; or (loss_sum NULL) the gradient scale[0] * d/dbbox_pred at those columns (the caller zeroes grad).
+ *   ptb_roi_accuracy    out[0] = (number of rows whose first maximum is the label) * scale.
+ *   ptb_roi_decode      over B x N padded RoI rows: rows whose four coordinates are 0 take cls_score = 0 and bbox_pred = 0; softmax of
+ *                       cls_score [B*N][C+1]; delta2bbox of bbox_pred [B*N][4C] (or [B*N][4]) with dw, dh clamped to +-max_ratio,
+ *                       clipped to img_hw [B][2] (h, w, fp32), divided by scale_factor [B][4] when it is given.  boxes [B][N][C][4],
+ *                       scores [B][N][C] (the background column dropped). */
+#define PTB_ROI_MAX_LEVELS 4
+int ptb_roi_align_fwd(const float* const* maps, const int32_t* featmap_hw, const float* strides, int L, int B, int C, const float* rois,
+                      int R, int out, int sampling_ratio, float finest_scale, float* y, int32_t* levels, void* stream);
+int ptb_roi_align_bwd(float* const* grad_maps, const int32_t* featmap_hw, const float* strides, int L, int B, int C, const float* rois,
+                      const int32_t* levels, int R, int out, int sampling_ratio, const float* grad_y, void* stream);
+int ptb_roi_targets(int B, int N, const float* cand, const int64_t* gt_inds, const int32_t* rank, const int32_t* plan,
+                    const int32_t* row_off, const float* gt_bboxes, const int32_t* gt_off, const int64_t* gt_labels, int num_classes,
+                    const float* means /*[4]*/, const float* stds /*[4]*/, float pos_weight, float* rois, int64_t* labels,
+                    float* label_weights, float* bbox_targets, float* bbox_weights, void* stream);
+int ptb_roi_bbox_loss(const float* bbox_pred, int ld, const int64_t* labels, const float* bbox_targets, const float* bbox_weights, int64_t R,
+                      int num_classes, int class_agnostic, int bbox_loss, float beta, float* loss_sum, const float* scale, float* grad,
+                      void* stream);
+int ptb_roi_accuracy(const float* cls_score, const int64_t* labels, int64_t R, int num_cols, float scale, float* out, void* stream);
+int ptb_roi_decode(const float* rois, const float* cls_score, const float* bbox_pred, int B, int N, int num_classes, int class_agnostic,
+                   const float* means /*[4]*/, const float* stds /*[4]*/, float max_ratio, const float* img_hw, const float* scale_factor,
+                   float* boxes, float* scores, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -134,6 +134,12 @@ SIGNATURES = {
     'ptb_rpn_anchor_targets': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_float, P, P, P, P, P]),
     'ptb_rpn_sampled_indices': (c_int, [P, P, c_int, P, P, P, P]),
     'ptb_rpn_level_loss': (c_int, [P, P, P, P, P, P, c_i64, c_int, c_float, P, P, P, P, P]),
+    'ptb_roi_align_fwd': (c_int, [P, P, P, c_int, c_int, c_int, P, c_int, c_int, c_int, c_float, P, P, P]),
+    'ptb_roi_align_bwd': (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_int, c_int, c_int, P, P]),
+    'ptb_roi_targets': (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, c_int, P, P, c_float, P, P, P, P, P, P]),
+    'ptb_roi_bbox_loss': (c_int, [P, c_int, P, P, P, c_i64, c_int, c_int, c_int, c_float, P, P, P, P]),
+    'ptb_roi_accuracy': (c_int, [P, P, c_i64, c_int, c_float, P, P]),
+    'ptb_roi_decode': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, P, P, P, P]),
 }
 
 

@@ -250,8 +250,9 @@ def sampled_counts(plan, counts):
     return [tuple(c if sel is None else sel.numel() for sel, c in zip(p, cnt)) for p, cnt in zip(plan, counts)]
 
 
-def upload_sample_plan(plan, device):
-    """the plan in the layout of ptb_rpn_anchor_targets / ptb_rpn_sampled_indices (include/ptb_b200.h), one copy from pinned memory"""
+def upload_sample_plan(plan, device, tail=()):
+    """the plan in the layout of ptb_rpn_anchor_targets / ptb_rpn_sampled_indices (include/ptb_b200.h), one copy from pinned memory;
+    `tail` (ints) is appended after the drawn ranks, in the same copy"""
     head, body, off = [], [], 4 * len(plan)
     for p in plan:
         for sel in p:
@@ -261,10 +262,12 @@ def upload_sample_plan(plan, device):
                 head += [off, sel.numel()]
                 body.append(sel)
                 off += sel.numel()
-    buf = torch.empty((off,), dtype=torch.int32, pin_memory=True)
+    buf = torch.empty((off + len(tail),), dtype=torch.int32, pin_memory=True)
     buf[:len(head)] = torch.tensor(head, dtype=torch.int32)
     if body:
-        buf[len(head):] = torch.cat(body)
+        buf[len(head):off] = torch.cat(body)
+    if len(tail):
+        buf[off:] = torch.tensor(list(tail), dtype=torch.int32)
     return buf.to(device, non_blocking=True)
 
 

@@ -84,4 +84,30 @@ struct L1RowsLoss {
   }
 };
 
+// The RoI head's box loss (bbox_head.py:282-306): element e = 4 m + k of the (R, 4) targets.  Only positive rows (label in
+// [0, num_classes)) count; their prediction is column 4 * label + k of bbox_pred (R, ld), or column k when class-agnostic.  L1Loss
+// |d| * w or SmoothL1Loss (beta) on d = pred - target; the gradient is written at that column only (the caller zeroes the rest).
+template <bool SMOOTH>
+struct RoIBoxLoss {
+  const float* pred; const int64_t* labels; const float* target; const float* weight; int ld, num_classes, agnostic; float beta;
+  __device__ __forceinline__ float operator()(long long e, bool, float* grad, float sc) const {
+    const long long m = e >> 2;
+    const int k = (int)(e & 3);
+    const long long lab = labels[m];
+    if (lab < 0 || lab >= num_classes) return 0.f;
+    const long long col = m * ld + (agnostic ? k : 4 * lab + k);
+    const float w = weight[e];
+    const float diff = pred[col] - target[e];
+    const float d = fabsf(diff);
+    const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
+    if constexpr (SMOOTH) {
+      if (grad) grad[col] = sc * w * (d < beta ? diff / beta : sgn);
+      return (d < beta ? 0.5f * d * d / beta : d - 0.5f * beta) * w;
+    } else {
+      if (grad) grad[col] = sc * w * sgn;
+      return d * w;
+    }
+  }
+};
+
 }  // namespace ptb

@@ -19,6 +19,8 @@
 // Integer results (ranks, counts, labels, weights, sampled sets) are exact; every sum has a fixed order.
 #include "ptb_common.cuh"
 #include "loss_terms.cuh"
+#include "box_coder.cuh"
+#include "sample_plan.cuh"
 
 namespace ptb {
 namespace {
@@ -114,19 +116,6 @@ rpn_candidate_kernel(const int64_t* __restrict__ gt_inds /*[B][N]*/, const int32
   if (threadIdx.x == 0) { counts[2 * b] = npos; counts[2 * b + 1] = nneg; }
 }
 
-// output slot of candidate rank r of (image b, kind 0 pos / 1 neg) in the sampled list, -1 when it is not sampled.
-// plan: header [B][2] x (offset, count) — count -1: every candidate is sampled (no draw) — then the sorted drawn ranks.
-__device__ __forceinline__ int sampled_slot(const int32_t* __restrict__ plan, int b, int kind, int r) {
-  const int off = plan[(b * 2 + kind) * 2], cnt = plan[(b * 2 + kind) * 2 + 1];
-  if (cnt < 0) return r;
-  int lo = 0, hi = cnt;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (plan[off + mid] < r) lo = mid + 1; else hi = mid;
-  }
-  return (lo < cnt && plan[off + lo] == r) ? lo : -1;
-}
-
 struct EncodeCfg {
   float mean[4], stdv[4];
   float pos_weight;
@@ -163,17 +152,7 @@ rpn_targets_kernel(RtLevels lv, int B, const int32_t* __restrict__ inside_idx, c
         lab = 0;
         lw = ec.pos_weight > 0.f ? ec.pos_weight : 1.f;
         bw = 1.f;
-        const float4 p = inside_anchors[row + j];
-        const float4 q = gt[gt_off[b] + (int)(g - 1)];
-        // bbox2delta in the reference's fp32 operation order
-        const float px = __fmul_rn(__fadd_rn(p.x, p.z), 0.5f), py = __fmul_rn(__fadd_rn(p.y, p.w), 0.5f);
-        const float pw = __fsub_rn(p.z, p.x), ph = __fsub_rn(p.w, p.y);
-        const float gx = __fmul_rn(__fadd_rn(q.x, q.z), 0.5f), gy = __fmul_rn(__fadd_rn(q.y, q.w), 0.5f);
-        const float gw = __fsub_rn(q.z, q.x), gh = __fsub_rn(q.w, q.y);
-        const float dx = __fdiv_rn(__fsub_rn(gx, px), pw), dy = __fdiv_rn(__fsub_rn(gy, py), ph);
-        const float dw = logf(__fdiv_rn(gw, pw)), dh = logf(__fdiv_rn(gh, ph));
-        d = make_float4(__fdiv_rn(__fsub_rn(dx, ec.mean[0]), ec.stdv[0]), __fdiv_rn(__fsub_rn(dy, ec.mean[1]), ec.stdv[1]),
-                        __fdiv_rn(__fsub_rn(dw, ec.mean[2]), ec.stdv[2]), __fdiv_rn(__fsub_rn(dh, ec.mean[3]), ec.stdv[3]));
+        d = bbox2delta(inside_anchors[row + j], gt[gt_off[b] + (int)(g - 1)], ec.mean, ec.stdv);
       } else if (g == 0 && sampled_slot(plan, b, 1, r) >= 0) {
         lw = 1.f;
       }

@@ -1396,3 +1396,131 @@ def rpn_level_loss(cls_score, bbox_pred, labels, label_weights, bbox_targets, bb
                                  _ptr(bbox_weights), M, int(bbox_loss), float(beta), _ptr(loss), None, None, None, _stream()),
           'ptb_rpn_level_loss')
     return loss
+
+
+# ---- RoI head (ptb_roi_*): multi-level RoIAlign, RoI targets, box loss, accuracy and test decode of StandardRoIHead's bbox branch
+ROI_MAX_LEVELS = 4                     # PTB_ROI_MAX_LEVELS
+
+
+def _roi_level_arrays(maps_nhwc, strides):
+    L = len(maps_nhwc)
+    if not 1 <= L <= ROI_MAX_LEVELS or len(strides) != L:
+        raise ValueError(f'1 to {ROI_MAX_LEVELS} levels with one stride each, got {L} maps and {len(strides)} strides')
+    B, C = maps_nhwc[0].shape[0], maps_nhwc[0].shape[3]
+    for m in maps_nhwc:
+        _chk(m, torch.float32, 'feature map')
+        if m.dim() != 4 or m.shape[0] != B or m.shape[3] != C:
+            raise ValueError('feature maps must be channels-last (B, H, W, C) with the same B and C')
+    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for m in maps_nhwc for v in m.shape[1:3]])
+    st = (ctypes.c_float * L)(*[float(s) for s in strides])
+    ptrs = (ctypes.c_void_p * L)(*[m.data_ptr() for m in maps_nhwc])
+    return L, B, C, hw, st, ptrs
+
+
+def roi_align_fwd(maps_nhwc, strides, rois, out_size, sampling_ratio, finest_scale):
+    """ptb_roi_align_fwd.  maps_nhwc: per level (B, H, W, C) fp32 contiguous; rois (R, 5).
+    returns features (R, C, out, out) and levels (R,) int32."""
+    lib = _lib.load()
+    _chk(rois, torch.float32, 'rois')
+    L, B, C, hw, st, ptrs = _roi_level_arrays(maps_nhwc, strides)
+    R = rois.shape[0]
+    y = torch.empty((R, C, out_size, out_size), dtype=torch.float32, device=rois.device)
+    lv = torch.empty((R,), dtype=torch.int32, device=rois.device)
+    check(lib.ptb_roi_align_fwd(ptrs, hw, st, L, B, C, _ptr(rois), R, int(out_size), int(sampling_ratio), float(finest_scale), _ptr(y),
+                                _ptr(lv), _stream()), 'ptb_roi_align_fwd')
+    return y, lv
+
+
+def roi_align_bwd(grad_y, map_shapes, strides, rois, levels, sampling_ratio):
+    """ptb_roi_align_bwd: the gradients (B, H, W, C) of the channels-last maps of shapes map_shapes (zero where no RoI reads)."""
+    lib = _lib.load()
+    _chk(grad_y, torch.float32, 'grad_y'); _chk(rois, torch.float32, 'rois'); _chk(levels, torch.int32, 'levels')
+    grads = [torch.zeros(s, dtype=torch.float32, device=grad_y.device) for s in map_shapes]
+    L, B, C, hw, st, ptrs = _roi_level_arrays(grads, strides)
+    R, out = grad_y.shape[0], grad_y.shape[-1]
+    if tuple(grad_y.shape) != (R, C, out, out) or rois.shape[0] != R or levels.shape != (R,):
+        raise ValueError('roi_align_bwd: inconsistent shapes')
+    check(lib.ptb_roi_align_bwd(ptrs, hw, st, L, B, C, _ptr(rois), _ptr(levels), R, int(out), int(sampling_ratio), _ptr(grad_y), _stream()),
+          'ptb_roi_align_bwd')
+    return grads
+
+
+def roi_targets(cand, gt_inds, rank, plan, row_off, gt_bboxes, gt_off, gt_labels, num_classes, means, stds, pos_weight, R):
+    """ptb_roi_targets.  returns rois (R, 5), labels (R,) int64, label_weights (R,), bbox_targets (R, 4), bbox_weights (R, 4)."""
+    lib = _lib.load()
+    B, N = gt_inds.shape
+    for t, dt, name in ((cand, torch.float32, 'cand'), (gt_inds, torch.int64, 'gt_inds'), (rank, torch.int32, 'rank'),
+                        (plan, torch.int32, 'plan'), (row_off, torch.int32, 'row_off'), (gt_bboxes, torch.float32, 'gt_bboxes'),
+                        (gt_off, torch.int32, 'gt_off'), (gt_labels, torch.int64, 'gt_labels')):
+        _chk(t, dt, name)
+    if tuple(cand.shape) != (B, N, 4) or tuple(rank.shape) != (B, N) or row_off.numel() != 2 * B or tuple(gt_off.shape) != (B + 1,) or \
+            plan.numel() < 4 * B or gt_bboxes.shape[-1] != 4 or gt_labels.shape[0] != gt_bboxes.shape[0]:
+        raise ValueError('roi_targets: inconsistent shapes')
+    dev = cand.device
+    rois = torch.empty((R, 5), dtype=torch.float32, device=dev)
+    labels = torch.empty((R,), dtype=torch.int64, device=dev)
+    lw = torch.empty((R,), dtype=torch.float32, device=dev)
+    bt = torch.empty((R, 4), dtype=torch.float32, device=dev)
+    bw = torch.empty((R, 4), dtype=torch.float32, device=dev)
+    mean = (ctypes.c_float * 4)(*[float(v) for v in means])
+    std = (ctypes.c_float * 4)(*[float(v) for v in stds])
+    check(lib.ptb_roi_targets(B, N, _ptr(cand), _ptr(gt_inds), _ptr(rank), _ptr(plan), _ptr(row_off), _ptr(gt_bboxes), _ptr(gt_off),
+                              _ptr(gt_labels), int(num_classes), mean, std, float(pos_weight), _ptr(rois), _ptr(labels), _ptr(lw), _ptr(bt),
+                              _ptr(bw), _stream()), 'ptb_roi_targets')
+    return rois, labels, lw, bt, bw
+
+
+def roi_bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, num_classes, class_agnostic, bbox_loss, beta, scale=None,
+                  want_grad=False):
+    """ptb_roi_bbox_loss: the (1,) un-normalised box-loss sum over the positive rows, or with want_grad the gradient
+    scale * d/dbbox_pred (zero outside the positive rows' class columns)."""
+    lib = _lib.load()
+    _chk(bbox_pred, torch.float32, 'bbox_pred'); _chk(labels, torch.int64, 'labels')
+    _chk(bbox_targets, torch.float32, 'bbox_targets'); _chk(bbox_weights, torch.float32, 'bbox_weights')
+    R, ld = bbox_pred.shape
+    if labels.shape != (R,) or tuple(bbox_targets.shape) != (R, 4) or tuple(bbox_weights.shape) != (R, 4):
+        raise ValueError('roi_bbox_loss: inconsistent shapes')
+    if want_grad:
+        _chk(scale, torch.float32, 'scale')
+        g = torch.zeros_like(bbox_pred)
+        check(lib.ptb_roi_bbox_loss(_ptr(bbox_pred), ld, _ptr(labels), _ptr(bbox_targets), _ptr(bbox_weights), R, int(num_classes),
+                                    int(bool(class_agnostic)), int(bbox_loss), float(beta), None, _ptr(scale), _ptr(g), _stream()),
+              'ptb_roi_bbox_loss')
+        return g
+    loss = torch.zeros(1, dtype=torch.float32, device=bbox_pred.device)
+    check(lib.ptb_roi_bbox_loss(_ptr(bbox_pred), ld, _ptr(labels), _ptr(bbox_targets), _ptr(bbox_weights), R, int(num_classes),
+                                int(bool(class_agnostic)), int(bbox_loss), float(beta), _ptr(loss), None, None, _stream()),
+          'ptb_roi_bbox_loss')
+    return loss
+
+
+def roi_accuracy(cls_score, labels):
+    """ptb_roi_accuracy: top-1 accuracy in percent (losses/accuracy.py), (1,) fp32."""
+    lib = _lib.load()
+    _chk(cls_score, torch.float32, 'cls_score'); _chk(labels, torch.int64, 'labels')
+    R, C1 = cls_score.shape
+    out = torch.empty((1,), dtype=torch.float32, device=cls_score.device)
+    check(lib.ptb_roi_accuracy(_ptr(cls_score), _ptr(labels), R, C1, float(100.0 / R), _ptr(out), _stream()), 'ptb_roi_accuracy')
+    return out
+
+
+def roi_decode(rois, cls_score, bbox_pred, B, num_classes, class_agnostic, means, stds, max_ratio, img_hw, scale_factor=None):
+    """ptb_roi_decode over B images of N padded RoI rows.  returns boxes (B, N, C, 4) and foreground scores (B, N, C)."""
+    lib = _lib.load()
+    for t, name in ((rois, 'rois'), (cls_score, 'cls_score'), (bbox_pred, 'bbox_pred'), (img_hw, 'img_hw')):
+        _chk(t, torch.float32, name)
+    M = rois.shape[0]
+    N = M // B
+    C = int(num_classes)
+    if M != B * N or tuple(cls_score.shape) != (M, C + 1) or tuple(bbox_pred.shape) != (M, 4 if class_agnostic else 4 * C) or \
+            tuple(img_hw.shape) != (B, 2):
+        raise ValueError('roi_decode: inconsistent shapes')
+    if scale_factor is not None:
+        _chk(scale_factor, torch.float32, 'scale_factor')
+    boxes = torch.empty((B, N, C, 4), dtype=torch.float32, device=rois.device)
+    scores = torch.empty((B, N, C), dtype=torch.float32, device=rois.device)
+    mean = (ctypes.c_float * 4)(*[float(v) for v in means])
+    std = (ctypes.c_float * 4)(*[float(v) for v in stds])
+    check(lib.ptb_roi_decode(_ptr(rois), _ptr(cls_score), _ptr(bbox_pred), B, N, C, int(bool(class_agnostic)), mean, std, float(max_ratio),
+                             _ptr(img_hw), _ptr(scale_factor), _ptr(boxes), _ptr(scores), _stream()), 'ptb_roi_decode')
+    return boxes, scores

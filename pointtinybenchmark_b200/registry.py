@@ -85,6 +85,22 @@ def register_rpn():
     BBOX_SAMPLERS.register_module(name='RandomSampler', force=True, module=RandomSampler)
 
 
+try:   # pragma: no cover
+    from mmdet.models.builder import ROI_EXTRACTORS as _R
+    ROI_EXTRACTORS = _R
+except Exception:
+    ROI_EXTRACTORS = Registry('roi_extractor')
+
+
+def register_roi():
+    """register StandardRoIHead and Shared2FCBBoxHead (HEADS) and SingleRoIExtractor (ROI_EXTRACTORS) with force=True over the reference
+    classes, so a detector built from a Faster R-CNN config afterwards runs its RoI stage here.  Not done on import."""
+    from .roi_head import Shared2FCBBoxHead, SingleRoIExtractor, StandardRoIHead
+    HEADS.register_module(name='StandardRoIHead', force=True, module=StandardRoIHead)
+    HEADS.register_module(name='Shared2FCBBoxHead', force=True, module=Shared2FCBBoxHead)
+    ROI_EXTRACTORS.register_module(name='SingleRoIExtractor', force=True, module=SingleRoIExtractor)
+
+
 def build_assigner(cfg, **default_args):
     return BBOX_ASSIGNERS.build(cfg, default_args)
 
