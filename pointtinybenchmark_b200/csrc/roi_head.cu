@@ -9,7 +9,7 @@
 //                          ptb_rpn_candidate_ranks): the sampled rows in the reference's order (image-major, positives then negatives):
 //                          rois, labels, label weights, bbox2delta targets, bbox weights (bbox_head.py:117-181).
 //   RoIBoxLoss             loss_terms.cuh: L1 / SmoothL1 over the positive rows' class columns, fixed-order sum.
-//   roi_accuracy_kernel    top-1 accuracy (losses/accuracy.py), first maximum of each row.
+//   roi_accuracy_kernel    top-1 accuracy (losses/accuracy.py), torch.argmax of each row (its first NaN, else its first maximum).
 //   roi_decode_kernel      warp per RoI row: the padding rows zeroed (test_mixins.py:79-119), softmax, class-specific delta2bbox,
 //                          img_shape clip and rescale, written [B][N][C][4] / [B][N][C] for the batched multiclass NMS.
 #include "ptb_common.cuh"
@@ -233,7 +233,9 @@ roi_targets_kernel(int B, int N, const float4* __restrict__ cand, const int64_t*
   }
 }
 
-// top-1 accuracy over R rows of num_cols logits: one CTA, a warp per row, the first maximum (NaN never wins); out = correct * scale
+// top-1 accuracy over R rows of num_cols logits: one CTA, a warp per row; out = correct * scale.  The prediction follows torch.argmax,
+// which agrees with the reference's pred.topk(1) wherever the winner is unique: NaN ranks above every number, so a row containing NaN
+// predicts its first NaN column, and any other row its first maximum.
 __global__ void __launch_bounds__(1024)
 roi_accuracy_kernel(const float* __restrict__ x, const int64_t* __restrict__ labels, long long R, int num_cols, float scale,
                     float* __restrict__ out) {
@@ -244,16 +246,17 @@ roi_accuracy_kernel(const float* __restrict__ x, const int64_t* __restrict__ lab
   int mine = 0;
   for (long long m = warp; m < R; m += 32) {
     float best = -INFINITY;
-    int arg = num_cols;
-    for (int c = lane; c < num_cols; c += 32) {
+    int arg = num_cols;                        // num_cols: the lane holds no column
+    for (int c = lane; c < num_cols; c += 32) {           // ascending columns: a tie keeps the earlier one
       const float v = x[m * num_cols + c];
-      if (v > best || (arg == num_cols && v == best)) { best = v; arg = c; }
+      if (arg == num_cols || (best == best && (v != v || v > best))) { best = v; arg = c; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       const float ob = __shfl_xor_sync(0xffffffffu, best, o);
       const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
-      if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+      const bool take = ob != ob ? (best == best || oa < arg) : (best == best && (ob > best || (ob == best && oa < arg)));
+      if (take) { best = ob; arg = oa; }
     }
     if (lane == 0 && arg == labels[m]) ++mine;
   }
