@@ -747,6 +747,41 @@ int ptb_roi_decode(const float* rois, const float* cls_score, const float* bbox_
                    const float* means /*[4]*/, const float* stds /*[4]*/, float max_ratio, const float* img_hw, const float* scale_factor,
                    float* boxes, float* scores, void* stream);
 
+/* ---- test-time augmentation and tile testing of the two-stage detector (csrc/tile_test.cu): StandardRoIHead.aug_test and
+ * TwoStageDetector.tile_aug_test.  An aug meta row is 12 floats: segment, RoI batch index, scale_factor[4], flip (0 none, 1 horizontal,
+ * 2 vertical, 3 diagonal), img_h, img_w, has_offset, dx, dy.
+ *   ptb_box_map        bbox_mapping of rows [0, counts[seg]) of boxes [S][N][ld] for every aug g of meta [G][12]: * scale_factor, flip,
+ *                      and with an offset - (dx, dy), clamp to [0, w-1] x [0, h-1] and keep = (W >= 2 & H >= 2).  rois [G][N][5]
+ *                      (batch index, box; zero boxes past the count), keep [G][N] (or NULL).  counts NULL: N rows.
+ *   ptb_proposal_map_back  merge_aug_proposals' recovery: bbox_mapping_back (flip, / scale_factor, + offset) of the first counts[g]
+ *                      rows of det [T*A][N][5] (box, score; aug g = t * A + a), the augs of tile t concatenated in order into
+ *                      out [T][A*N][5]; out_count [T].
+ *   ptb_aug_merge      merge_aug_bboxes of T tiles of A augs (meta row t * A + a): bbox_mapping_back (flip, / scale_factor, + offset)
+ *                      of boxes [T*A][N][C][4] and torch.stack(...).mean(0) of them and of scores [T*A][N][C], in ATen's CPU order for
+ *                      a stack of (counts[t], box_cols) boxes and (counts[t], C + 1) scores.  box_cols: 4 (class-agnostic) or 4C.
+ *                      out_boxes [T][N][C][4], out_scores [T][N][C] (-inf past the count).  A <= 63.
+ *   ptb_batched_nms    mmcv batched_nms (labels given) or nms (labels NULL) of each of S segments of N <= 65536 rows: the first
+ *                      counts[s] rows (NULL: N) of boxes [S][N][ld], scores [S][N][lds], labels [S][N].  Greedy IoU > iou_thr in the
+ *                      order score descending, position ascending on boxes offset by label * (max + 1); from split_thr rows on only
+ *                      equal labels suppress.  out_count [S], out_det [S][N][5] (box, score), out_label [S][N] (or NULL), out_keep
+ *                      [S][N] row positions, at most max_num rows when max_num > 0.  workspace: ptb_batched_nms_workspace(S, N).
+ *   ptb_tile_concat    the first counts[t] rows of det [T][K][5] / labels [T][K] of each tile, boxes * scale_factor [T][4] (or NULL)
+ *                      + offsets [T][2] (dx, dy), concatenated in tile order, class-major within a tile (the rows of one class in
+ *                      their order): out [T*K][5], out_label [T*K], out_count[0] = the number of rows. */
+#define PTB_BATCHED_NMS_MAX_ROWS 65536
+int ptb_box_map(const float* boxes, int ld, const int32_t* counts, int N, int G, const float* meta, float* rois, uint8_t* keep,
+                void* stream);
+int ptb_proposal_map_back(const float* det, const int32_t* counts, int N, int T, int A, const float* meta, float* out, int32_t* out_count,
+                          void* stream);
+int ptb_aug_merge(const float* boxes, const float* scores, int N, int num_classes, int box_cols, const int32_t* counts, int T, int A,
+                  const float* meta, float* out_boxes, float* out_scores, void* stream);
+uint64_t ptb_batched_nms_workspace(int S, int N);
+int ptb_batched_nms(const float* boxes, int ld, const float* scores, int lds, const int32_t* labels, const int32_t* counts, int S, int N,
+                    float iou_thr, int split_thr, int max_num, int32_t* out_count, float* out_det, int32_t* out_label, int32_t* out_keep,
+                    void* workspace, uint64_t workspace_bytes, void* stream);
+int ptb_tile_concat(const float* det, const int32_t* labels, const int32_t* counts, int T, int K, const float* scale_factor,
+                    const float* offsets, float* out, int32_t* out_label, int32_t* out_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

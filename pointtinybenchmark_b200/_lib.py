@@ -140,6 +140,12 @@ SIGNATURES = {
     'ptb_roi_bbox_loss': (c_int, [P, c_int, P, P, P, c_i64, c_int, c_int, c_int, c_float, P, P, P, P]),
     'ptb_roi_accuracy': (c_int, [P, P, c_i64, c_int, c_float, P, P]),
     'ptb_roi_decode': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, P, P, P, P]),
+    'ptb_box_map': (c_int, [P, c_int, P, c_int, c_int, P, P, P, P]),
+    'ptb_proposal_map_back': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P]),
+    'ptb_aug_merge': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, P, P, P]),
+    'ptb_batched_nms_workspace': (c_u64, [c_int, c_int]),
+    'ptb_batched_nms': (c_int, [P, c_int, P, c_int, P, P, c_int, c_int, c_float, c_int, c_int, P, P, P, P, P, c_u64, P]),
+    'ptb_tile_concat': (c_int, [P, P, P, c_int, c_int, P, P, P, P, P, P]),
 }
 
 

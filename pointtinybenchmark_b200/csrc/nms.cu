@@ -42,16 +42,6 @@ struct NmsImg {       // per-image header in the workspace
 // weigh >= 2 here: its out_count is -1.  Hard NMS, naive and linear only compare the IoU, and NaN compares false everywhere.
 __device__ __forceinline__ int degenerate_weight(float area) { return area > 0.f ? 0 : (area == 0.f ? 1 : 2); }
 
-struct Box {
-  float x1, y1, x2, y2, area;
-};
-__device__ __forceinline__ bool iou_gt(const Box& a, const Box& b, float thr) {
-  const float w = fmaxf(0.f, __fsub_rn(fminf(a.x2, b.x2), fmaxf(a.x1, b.x1)));
-  const float h = fmaxf(0.f, __fsub_rn(fminf(a.y2, b.y2), fmaxf(a.y1, b.y1)));
-  const float inter = __fmul_rn(w, h);
-  const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(a.area, b.area), inter));
-  return ovr > thr;
-}
 
 // un-offset box of point / proposal p: either given explicitly (row p of the image's boxes, see box_row) or the pseudo box
 // pts[p] -/+ (hw, hh)

@@ -167,6 +167,19 @@ __device__ __forceinline__ float sigmoidf_acc(float x) { return __fdiv_rn(1.f, _
 // ---------------------------------------------------------------------------------------------
 // warp / block reductions (fixed order => deterministic)
 // ---------------------------------------------------------------------------------------------
+// an NMS box on the coordinates the IoU sees, area = (x2 - x1) * (y2 - y1); iou_gt: mmcv / torchvision nms (offset 0), IoU > thr in
+// their fp32 operation order.  Shared by every NMS kernel so that they cannot disagree.
+struct Box {
+  float x1, y1, x2, y2, area;
+};
+__device__ __forceinline__ bool iou_gt(const Box& a, const Box& b, float thr) {
+  const float w = fmaxf(0.f, __fsub_rn(fminf(a.x2, b.x2), fmaxf(a.x1, b.x1)));
+  const float h = fmaxf(0.f, __fsub_rn(fminf(a.y2, b.y2), fmaxf(a.y1, b.y1)));
+  const float inter = __fmul_rn(w, h);
+  const float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(a.area, b.area), inter));
+  return ovr > thr;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -4,6 +4,8 @@ only — all math happens in libptb_b200.so.  Every op raises if the library is 
 import ctypes
 import math
 
+import numpy as np
+
 import torch
 
 from . import _lib
@@ -1524,3 +1526,115 @@ def roi_decode(rois, cls_score, bbox_pred, B, num_classes, class_agnostic, means
     check(lib.ptb_roi_decode(_ptr(rois), _ptr(cls_score), _ptr(bbox_pred), B, N, C, int(bool(class_agnostic)), mean, std, float(max_ratio),
                              _ptr(img_hw), _ptr(scale_factor), _ptr(boxes), _ptr(scores), _stream()), 'ptb_roi_decode')
     return boxes, scores
+
+
+# ---- test-time augmentation and tile testing (ptb_box_map / ptb_aug_merge / ptb_batched_nms / ptb_tile_concat)
+BATCHED_NMS_MAX_ROWS = 65536           # PTB_BATCHED_NMS_MAX_ROWS
+FLIP_DIRECTIONS = {'horizontal': 1, 'vertical': 2, 'diagonal': 3}
+
+
+def aug_meta(img_metas, segments, roi_batch, device):
+    """the (G, 12) meta rows of ptb_box_map / ptb_aug_merge: segment, RoI batch index, scale_factor[4], flip, img_h, img_w, has_offset,
+    dx, dy of each aug's meta dict (uploaded in one copy)"""
+    rows = []
+    for m, s, r in zip(img_metas, segments, roi_batch):
+        sf = np.asarray(m['scale_factor'], np.float32).reshape(-1) * np.ones(4, np.float32)
+        flip = FLIP_DIRECTIONS[m.get('flip_direction') or 'horizontal'] if m.get('flip', False) else 0
+        off = m.get('tile_offset', None)
+        rows.append([s, r, *sf.tolist(), flip, float(m['img_shape'][0]), float(m['img_shape'][1]), float(off is not None),
+                     *(np.float32(v) for v in (off if off is not None else (0, 0)))])
+    return torch.tensor(np.array(rows, np.float32)).pin_memory().to(device, non_blocking=True)
+
+
+def box_map(boxes, counts, meta, want_keep=False):
+    """ptb_box_map: boxes (S, N, ld >= 4) fp32, counts (S,) int32 or None, meta (G, 12) -> rois (G, N, 5) [, keep (G, N) bool]"""
+    lib = _lib.load()
+    _chk(boxes, torch.float32, 'boxes'); _chk(meta, torch.float32, 'meta')
+    if counts is not None:
+        _chk(counts, torch.int32, 'counts')
+    S, N, ld = boxes.shape
+    G = meta.shape[0]
+    rois = torch.empty((G, N, 5), dtype=torch.float32, device=boxes.device)
+    keep = torch.empty((G, N), dtype=torch.bool, device=boxes.device) if want_keep else None
+    check(lib.ptb_box_map(_ptr(boxes), ld, _ptr(counts), N, G, _ptr(meta), _ptr(rois), _ptr(keep), _stream()), 'ptb_box_map')
+    return (rois, keep) if want_keep else rois
+
+
+def proposal_map_back(det, counts, meta, A):
+    """ptb_proposal_map_back: det (T*A, N, 5) proposals and counts (T*A,) int32 of every aug -> (T, A*N, 5) recovered and concatenated
+    per tile, count (T,)"""
+    lib = _lib.load()
+    _chk(det, torch.float32, 'det'); _chk(counts, torch.int32, 'counts'); _chk(meta, torch.float32, 'meta')
+    G, N = det.shape[:2]
+    if G % A or det.shape[2] != 5 or meta.shape[0] != G:
+        raise ValueError('proposal_map_back: inconsistent shapes')
+    T = G // A
+    out = torch.empty((T, A * N, 5), dtype=torch.float32, device=det.device)
+    cnt = torch.empty((T,), dtype=torch.int32, device=det.device)
+    check(lib.ptb_proposal_map_back(_ptr(det), _ptr(counts), N, T, A, _ptr(meta), _ptr(out), _ptr(cnt), _stream()), 'ptb_proposal_map_back')
+    return out, cnt
+
+
+def aug_merge(boxes, scores, counts, meta, A, box_cols):
+    """ptb_aug_merge: boxes (T*A, N, C, 4) and scores (T*A, N, C) of ptb_roi_decode -> merged (T, N, C, 4), (T, N, C)"""
+    lib = _lib.load()
+    _chk(boxes, torch.float32, 'boxes'); _chk(scores, torch.float32, 'scores'); _chk(meta, torch.float32, 'meta')
+    if counts is not None:
+        _chk(counts, torch.int32, 'counts')
+    G, N, C = scores.shape
+    if G % A or tuple(boxes.shape) != (G, N, C, 4) or meta.shape[0] != G:
+        raise ValueError('aug_merge: inconsistent shapes')
+    if not 1 <= A <= 63:
+        raise NotImplementedError(f'{A} augs per tile: 1 to 63 are implemented')
+    T = G // A
+    ob = torch.empty((T, N, C, 4), dtype=torch.float32, device=boxes.device)
+    os_ = torch.empty((T, N, C), dtype=torch.float32, device=boxes.device)
+    check(lib.ptb_aug_merge(_ptr(boxes), _ptr(scores), N, C, int(box_cols), _ptr(counts), T, A, _ptr(meta), _ptr(ob), _ptr(os_), _stream()),
+          'ptb_aug_merge')
+    return ob, os_
+
+
+def batched_nms(boxes, scores, labels, counts, iou_thr, split_thr=10000, max_num=-1):
+    """ptb_batched_nms: mmcv batched_nms (labels (S, N) int32) or nms (labels None) of S segments.  boxes (S, N, ld >= 4) and scores
+    (S, N) or (S, N, lds) views of contiguous rows (scores may be boxes[..., 4]), counts (S,) int32 or None.
+    returns count (S,), det (S, N, 5), label (S, N) or None, keep (S, N) int32 in output order."""
+    lib = _lib.load()
+    if boxes.dim() != 3 or not boxes.is_cuda or boxes.dtype != torch.float32 or boxes.stride(2) != 1 or boxes.stride(0) != boxes.shape[1] * boxes.stride(1):
+        raise ValueError('batched_nms: boxes must be (S, N, ld) fp32 CUDA rows with unit column stride')
+    S, N = boxes.shape[:2]
+    if N > BATCHED_NMS_MAX_ROWS:
+        raise NotImplementedError(f'batched_nms over {N} rows: at most {BATCHED_NMS_MAX_ROWS} (PTB_BATCHED_NMS_MAX_ROWS) are implemented')
+    if not scores.is_cuda or scores.dtype != torch.float32 or scores.shape[:2] != (S, N) or scores.stride(0) != N * scores.stride(1):
+        raise ValueError('batched_nms: scores must be (S, N) fp32 CUDA with row-major segments')
+    if labels is not None:
+        _chk(labels, torch.int32, 'labels')
+    if counts is not None:
+        _chk(counts, torch.int32, 'counts')
+    dev = boxes.device
+    cnt = torch.empty((S,), dtype=torch.int32, device=dev)
+    det = torch.empty((S, N, 5), dtype=torch.float32, device=dev)
+    lab = torch.empty((S, N), dtype=torch.int32, device=dev) if labels is not None else None
+    keep = torch.empty((S, N), dtype=torch.int32, device=dev)
+    nbytes = int(lib.ptb_batched_nms_workspace(S, N))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    check(lib.ptb_batched_nms(_ptr(boxes), boxes.stride(1), _ptr(scores), scores.stride(1), _ptr(labels), _ptr(counts), S, N, float(iou_thr),
+                              int(split_thr), int(max_num), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(ws), nbytes, _stream()),
+          'ptb_batched_nms')
+    return cnt, det, lab, keep
+
+
+def tile_concat(det, labels, counts, offsets, scale_factor=None):
+    """ptb_tile_concat: det (T, K, 5), labels (T, K) int32, counts (T,) int32, offsets (T, 2), scale_factor (T, 4) or None
+    -> rows (T*K, 5), labels (T*K,), count (1,)"""
+    lib = _lib.load()
+    _chk(det, torch.float32, 'det'); _chk(labels, torch.int32, 'labels'); _chk(counts, torch.int32, 'counts')
+    _chk(offsets, torch.float32, 'offsets')
+    if scale_factor is not None:
+        _chk(scale_factor, torch.float32, 'scale_factor')
+    T, K = labels.shape
+    out = torch.empty((T * K, 5), dtype=torch.float32, device=det.device)
+    lab = torch.empty((T * K,), dtype=torch.int32, device=det.device)
+    cnt = torch.empty((1,), dtype=torch.int32, device=det.device)
+    check(lib.ptb_tile_concat(_ptr(det), _ptr(labels), _ptr(counts), T, K, _ptr(scale_factor), _ptr(offsets), _ptr(out), _ptr(lab), _ptr(cnt),
+                              _stream()), 'ptb_tile_concat')
+    return out, lab, cnt

@@ -235,7 +235,8 @@ class StandardRoIHead(nn.Module):
     """standard_roi_head.py over base_roi_head.py, bbox branch only: same constructor keywords, `forward_train` (returns
     dict(loss_cls, loss_bbox, acc)), `simple_test` (per image the bbox2result lists), `_bbox_forward`.  Refused with
     NotImplementedError: a mask branch, a shared head, other extractors and bbox heads, samplers other than RandomSampler,
-    and `aug_test`, which the detector's aug_test and tile_aug_test call (with or without test_cfg do_tile_as_aug)."""
+    and `aug_test` under test_cfg do_tile_as_aug=True.  `aug_test` / `aug_test_bboxes` run the reference's test-time augmentation for
+    one image; pointtinybenchmark_b200.tile_test.tile_aug_test runs the detector's tile testing."""
 
     def __init__(self, bbox_roi_extractor=None, bbox_head=None, mask_roi_extractor=None, mask_head=None, shared_head=None,
                  train_cfg=None, test_cfg=None, pretrained=None, init_cfg=None):
@@ -343,9 +344,9 @@ class StandardRoIHead(nn.Module):
         # every sampled row has a positive label weight (pos_weight > 0 or 1, negatives 1): avg_factor is the sample count
         return self.bbox_head.loss(res['cls_score'], res['bbox_pred'], rois, labels, lw, bt, bw, avg_factor=rois.shape[0])
 
-    def simple_test_bboxes(self, x, img_metas, proposals, rcnn_test_cfg, rescale=False):
-        """test_mixins.py:57-155: per image (dets (k, 5), labels (k,)) from one decode launch and one batched NMS call"""
-        cfg = CfgNode(rcnn_test_cfg)
+    def _multiclass_nms(self, boxes, scores, cfg):
+        """the batched multiclass NMS of (B, P, C, 4) boxes and (B, P, C) scores with the test cfg's nms / max_per_img:
+        count (B,), det (B, kmax, 5), label (B, kmax), kmax and max_per_img"""
         nms = dict(cfg.get('nms') or dict(type='nms', iou_threshold=0.5))
         check_split_thr(nms)
         kind = nms.pop('type', 'nms')
@@ -358,6 +359,17 @@ class StandardRoIHead(nn.Module):
         if max_per_img > 1024:
             raise NotImplementedError('max_per_img must be <= 1024')
         kmax = 1024 if max_per_img <= 0 else max_per_img
+        if kind == 'nms':
+            cnt, det, lab, _, _ = ops.multiclass_nms_boxes(boxes, scores, float(cfg.score_thr), iou, kmax)
+        else:
+            cnt, det, lab, _, _ = ops.multiclass_soft_nms(boxes, scores, None, float(cfg.score_thr), iou, kmax,
+                                                          sigma=nms.get('sigma', 0.5), min_score=nms.get('min_score', 1e-3),
+                                                          method=nms.get('method', 'linear'))
+        return cnt, det, lab, kmax, max_per_img
+
+    def simple_test_bboxes(self, x, img_metas, proposals, rcnn_test_cfg, rescale=False):
+        """test_mixins.py:57-155: per image (dets (k, 5), labels (k,)) from one decode launch and one batched NMS call"""
+        cfg = CfgNode(rcnn_test_cfg)
         B = len(proposals)
         dev = proposals[0].device
         N = max(int(p.shape[0]) for p in proposals)
@@ -377,12 +389,7 @@ class StandardRoIHead(nn.Module):
                                         for m in img_metas]), dtype=torch.float32).to(dev)
         boxes, scores = ops.roi_decode(rois, res['cls_score'].detach().float().contiguous(), res['bbox_pred'].detach().float().contiguous(), B,
                                        bh.num_classes, bh.reg_class_agnostic, bh.means, bh.stds, abs(np.log(16 / 1000)), img_hw, sf)
-        if kind == 'nms':
-            cnt, det, lab, _, _ = ops.multiclass_nms_boxes(boxes, scores, float(cfg.score_thr), iou, kmax)
-        else:
-            cnt, det, lab, _, _ = ops.multiclass_soft_nms(boxes, scores, None, float(cfg.score_thr), iou, kmax,
-                                                          sigma=nms.get('sigma', 0.5), min_score=nms.get('min_score', 1e-3),
-                                                          method=nms.get('method', 'linear'))
+        cnt, det, lab, kmax, max_per_img = self._multiclass_nms(boxes, scores, cfg)
         cnt = cnt.cpu().tolist()
         if max_per_img <= 0 and max(cnt) >= kmax:
             raise NotImplementedError('max_per_img=-1: more than 1023 detections survive the NMS (kernel limit 1024)')
@@ -399,8 +406,89 @@ class StandardRoIHead(nn.Module):
         det_h, lab_h = torch.cat(det).cpu().split(n), torch.cat(lab).cpu().split(n)          # one copy for the batch
         return [bbox2result(d, l, self.bbox_head.num_classes) for d, l in zip(det_h, lab_h)]
 
-    def aug_test(self, x, proposal_list, img_metas, rescale=False):
-        raise NotImplementedError('StandardRoIHead.aug_test (test-time augmentation, aug_test_bboxes / tile_aug_test) is not implemented')
+    def _refuse_tile_as_aug(self, cfg):
+        if CfgNode(cfg or {}).get('do_tile_as_aug', False):
+            raise NotImplementedError(
+                'StandardRoIHead.aug_test with test_cfg do_tile_as_aug=True: the detector then feeds every tile of an image as an aug of '
+                "one aug_test call, and the reference's bbox_mapping keeps different proposals per tile, so merge_aug_bboxes' torch.stack "
+                'fails for any image of more than one tile; use do_tile_as_aug=False (tile_aug_test, pointtinybenchmark_b200.tile_test)')
+
+    def shape_batches(self, feats):
+        """the position of every aug among the augs of its FPN shape (its RoI batch index in that shape's one RoIAlign)"""
+        L, seen, out = self.bbox_roi_extractor.num_inputs, {}, []
+        for f in feats:
+            key = tuple(tuple(m.shape[-2:]) for m in f[:L])
+            out.append(seen.get(key, 0))
+            seen[key] = out[-1] + 1
+        return out
+
+    def aug_forward_merge(self, feats, metas, meta, rois, counts, A):
+        """the RoI forward of every aug of T tiles at once and merge_aug_bboxes per tile.  feats: per aug (tile-major, A per tile) its
+        level maps (1, C, H, W); metas: per aug its meta dict; rois (T*A, N, 5) of ptb_box_map (batch index = position of the aug in its
+        FPN-shape group), counts (T,) int32 rows per tile or None.  returns boxes (T, N, C, 4) and scores (T, N, C), -inf past the count."""
+        G, N = rois.shape[:2]
+        dev = rois.device
+        L = self.bbox_roi_extractor.num_inputs
+        groups = {}
+        for g, f in enumerate(feats):
+            groups.setdefault(tuple(tuple(m.shape[-2:]) for m in f[:L]), []).append(g)
+        order = [g for gs in groups.values() for g in gs]
+        parts = []
+        for gs in groups.values():                    # augs at other scales have other map sizes: one RoIAlign per shape group
+            x = [torch.cat([feats[g][l] for g in gs]) for l in range(L)]
+            r = rois if len(groups) == 1 else rois[torch.tensor(gs, device=dev)]
+            parts.append(self.bbox_roi_extractor(x, r.reshape(-1, 5)))
+        bbox_feats = parts[0] if len(parts) == 1 else torch.cat(parts)
+        cls_score, bbox_pred = self.bbox_head(bbox_feats)
+        if len(groups) > 1:                           # back to aug order
+            inv = torch.empty(G, dtype=torch.int64)
+            inv[torch.tensor(order)] = torch.arange(G)
+            rows = (inv.to(dev)[:, None] * N + torch.arange(N, device=dev)[None]).reshape(-1)
+            cls_score, bbox_pred = cls_score[rows], bbox_pred[rows]
+        bh = self.bbox_head
+        img_hw = torch.tensor([[float(m['img_shape'][0]), float(m['img_shape'][1])] for m in metas], dtype=torch.float32)
+        boxes, scores = ops.roi_decode(rois.reshape(-1, 5).contiguous(), cls_score.detach().float().contiguous(),
+                                       bbox_pred.detach().float().contiguous(), G, bh.num_classes, bh.reg_class_agnostic, bh.means, bh.stds,
+                                       abs(np.log(16 / 1000)), img_hw.to(dev, non_blocking=True), None)
+        return ops.aug_merge(boxes, scores, counts, meta, A, 4 if bh.reg_class_agnostic else 4 * bh.num_classes)
 
     def aug_test_bboxes(self, feats, img_metas, proposal_list, rcnn_test_cfg):
-        raise NotImplementedError('StandardRoIHead.aug_test_bboxes (test-time augmentation) is not implemented')
+        """test_mixins.py:157-189 for one image: bbox_mapping of the proposals into every aug, one RoI forward over the augs,
+        merge_aug_bboxes (mean over the augs) and multiclass_nms.  returns (det_bboxes (k, 5), det_labels (k,))."""
+        self._refuse_tile_as_aug(rcnn_test_cfg if rcnn_test_cfg is not None else self.test_cfg)
+        cfg = CfgNode(rcnn_test_cfg)
+        metas = [m[0] for m in img_metas]
+        A = len(feats)
+        prop = proposal_list[0][:, :4].float().contiguous()
+        dev = prop.device
+        if not prop.is_cuda:
+            raise RuntimeError('StandardRoIHead runs on CUDA tensors only; there is no CPU fallback')
+        meta = ops.aug_meta(metas, [0] * A, self.shape_batches(feats), dev)
+        n = prop.shape[0]
+        if any(m.get('tile_offset') is not None for m in metas):
+            rois, keep = ops.box_map(prop[None], None, meta, want_keep=True)
+            kept = keep.sum(1).cpu().tolist()
+            if len(set(kept)) > 1:               # merge_aug_bboxes' torch.stack of the augs' box sets
+                raise RuntimeError(f'stack expects each tensor to be equal size: the tile offsets keep {kept} proposals per aug')
+            n = kept[0]
+            rois = rois[keep].view(A, n, 5)
+        else:
+            rois = ops.box_map(prop[None], None, meta)
+        if n == 0:                                # the reference forwards no RoI and multiclass_nms returns nothing
+            return torch.zeros((0, 5), dtype=torch.float32, device=dev), torch.zeros((0,), dtype=torch.long, device=dev)
+        boxes, scores = self.aug_forward_merge(feats, metas, meta, rois, None, A)
+        cnt, det, lab, kmax, max_per_img = self._multiclass_nms(boxes, scores, cfg)
+        c = int(cnt[0])
+        if max_per_img <= 0 and c >= kmax:
+            raise NotImplementedError('max_per_img=-1: more than 1023 detections survive the NMS (kernel limit 1024)')
+        return det[0, :c], lab[0, :c].long()
+
+    def aug_test(self, x, proposal_list, img_metas, rescale=False):
+        """standard_roi_head.py:246-270: [bbox_results] of one image; without rescale the boxes are multiplied by the first aug's
+        scale_factor"""
+        self._refuse_tile_as_aug(self.test_cfg)
+        det, lab = self.aug_test_bboxes(x, img_metas, proposal_list, self.test_cfg)
+        if not rescale:
+            sf = np.asarray(img_metas[0][0]['scale_factor'], np.float32).reshape(-1) * np.ones(4, np.float32)
+            det = torch.cat([det[:, :4] * torch.from_numpy(sf).to(det.device), det[:, 4:]], 1)
+        return [bbox2result(det.cpu(), lab.cpu(), self.bbox_head.num_classes)]

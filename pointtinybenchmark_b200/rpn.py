@@ -150,10 +150,9 @@ class RPNProposals:
         return self._base_dev[device]
 
     @torch.no_grad()
-    def get_bboxes(self, cls_scores, bbox_preds, img_metas, cfg=None, rescale=False, with_nms=True, return_levels=False):
+    def get_bboxes_padded(self, cls_scores, bbox_preds, img_metas, cfg=None):
+        """one ptb_rpn_proposals launch for the batch, no synchronisation: count (B,) int32, det (B, max_per_img, 5), level (B, max)"""
         assert len(cls_scores) == len(bbox_preds) == self.anchor_generator.num_levels
-        if not with_nms:
-            raise NotImplementedError('with_nms=False')
         if not cls_scores[0].is_cuda:
             raise RuntimeError('RPNProposals runs on CUDA tensors only; there is no CPU fallback')
         cfg = CfgNode(cfg) if cfg is not None else self.test_cfg
@@ -163,9 +162,15 @@ class RPNProposals:
         max_per_img = cfg.get('max_per_img', cfg.get('max_num', cfg.get('nms_post', 1000)))   # older configs spell it max_num / nms_post
         dev = cls_scores[0].device
         img_hw = torch.tensor([[int(m['img_shape'][0]), int(m['img_shape'][1])] for m in img_metas], dtype=torch.int32).to(dev)
-        cnt, det, lvl = ops.rpn_proposals([c.detach().float().contiguous() for c in cls_scores], [r.detach().float().contiguous() for r in bbox_preds],
-                                          self._base(dev), self.anchor_generator.strides, img_hw, self.means, self.stds, self.wh_ratio_clip,
-                                          cfg.get('nms_pre', -1), cfg.get('min_bbox_size', 0), nms.get('iou_threshold', 0.7), max_per_img)
+        return ops.rpn_proposals([c.detach().float().contiguous() for c in cls_scores], [r.detach().float().contiguous() for r in bbox_preds],
+                                 self._base(dev), self.anchor_generator.strides, img_hw, self.means, self.stds, self.wh_ratio_clip,
+                                 cfg.get('nms_pre', -1), cfg.get('min_bbox_size', 0), nms.get('iou_threshold', 0.7), max_per_img)
+
+    @torch.no_grad()
+    def get_bboxes(self, cls_scores, bbox_preds, img_metas, cfg=None, rescale=False, with_nms=True, return_levels=False):
+        if not with_nms:
+            raise NotImplementedError('with_nms=False')
+        cnt, det, lvl = self.get_bboxes_padded(cls_scores, bbox_preds, img_metas, cfg)
         cnt = cnt.cpu().tolist()                      # ragged result lists, like the reference's per-image dets
         out = [det[b, :cnt[b]] for b in range(len(cnt))]
         if return_levels:
