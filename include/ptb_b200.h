@@ -782,6 +782,36 @@ int ptb_batched_nms(const float* boxes, int ld, const float* scores, int lds, co
 int ptb_tile_concat(const float* det, const int32_t* labels, const int32_t* counts, int T, int K, const float* scale_factor,
                     const float* offsets, float* out, int32_t* out_label, int32_t* out_count, void* stream);
 
+/* FCOS head (fcos_head.py).  Rows of a batch: level after level, image after image inside a level, then y, x (the order of the
+ * reference's flattened maps); the point of a row is x * stride + stride // 2 of its level (L <= 8 levels of hw [L][2], strides [L]).
+ *   ptb_fcos_targets   _get_target_single of every (image, point): GTs gt_bboxes [G][4] / gt_labels [G] of image b at rows
+ *                      gt_off[b] .. gt_off[b+1]; regress ranges [L][2]; radius_px [L] = fp32(stride * center_sample_radius) or NULL
+ *                      (no centre sampling); the minimum-area GT wins, ties to the first; label num_classes where every area is
+ *                      excluded.  out_labels [N] int64, out_targets [N][4] (l, t, r, b; / stride when norm_on_bbox).
+ *   ptb_fcos_norm_sums out[0] += the number of positive rows, out[1] += the sum of their centerness targets (fixed order).
+ *   ptb_fcos_bbox_loss the centerness-weighted IoU (mode 0: -log, 1: linear; bbox_overlaps eps overlap_eps, clamp eps) or GIoU (mode 2,
+ *                      eps) loss of distance2bbox(point, pred [N][4]) against distance2bbox(point, targets): loss_sum [1] += the sum,
+ *                      or grad [N][4] = scale[0] * d/dpred (zero rows for negatives).
+ *   ptb_fcos_centerness_loss  binary_cross_entropy_with_logits(logits [N], centerness target) of the positive rows, same convention.
+ *   ptb_fcos_decode    per level and image: rows of the top nms_pre keys max_c sigmoid(cls) * sigmoid(ctr) when 0 < nms_pre < H*W
+ *                      (else every row in order), maps channels-last cls [B][H][W][C], reg [B][H][W][4], ctr [B][H][W]; out_idx
+ *                      [B][R] cell of each row, out_boxes [B][R][4] clipped to img_hw [B][2] (float) and / scale_factor [B][4] (or
+ *                      NULL), out_scores [B][R][C] sigmoid, out_ctr [B][R] sigmoid.  workspace: ptb_fcos_decode_workspace(B, L, hw). */
+int ptb_fcos_targets(const float* gt_bboxes, const int64_t* gt_labels, const int32_t* gt_off, int B, int L, const int32_t* hw,
+                     const float* strides, const float* ranges, const float* radius_px, int norm_on_bbox, int num_classes,
+                     int64_t* out_labels, float* out_targets, void* stream);
+int ptb_fcos_norm_sums(const int64_t* labels, const float* targets, int64_t N, int num_classes, float* out, void* stream);
+int ptb_fcos_bbox_loss(const float* pred, const float* targets, const int64_t* labels, int B, int L, const int32_t* hw, const float* strides,
+                       int num_classes, int mode, float overlap_eps, float eps, float* loss_sum, const float* scale, float* grad,
+                       void* stream);
+int ptb_fcos_centerness_loss(const float* logits, const float* targets, const int64_t* labels, int64_t N, int num_classes, float* loss_sum,
+                             const float* scale, float* grad, void* stream);
+uint64_t ptb_fcos_decode_workspace(int B, int L, const int32_t* hw);
+int ptb_fcos_decode(const float* const* cls_maps, const float* const* reg_maps, const float* const* ctr_maps, int L, const int32_t* hw,
+                    const float* strides, int B, int num_classes, const float* img_hw, const float* scale_factor, int nms_pre,
+                    int32_t* out_idx, float* out_boxes, float* out_scores, float* out_ctr, void* workspace, uint64_t workspace_bytes,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -146,6 +146,12 @@ SIGNATURES = {
     'ptb_batched_nms_workspace': (c_u64, [c_int, c_int]),
     'ptb_batched_nms': (c_int, [P, c_int, P, c_int, P, P, c_int, c_int, c_float, c_int, c_int, P, P, P, P, P, c_u64, P]),
     'ptb_tile_concat': (c_int, [P, P, P, c_int, c_int, P, P, P, P, P, P]),
+    'ptb_fcos_targets': (c_int, [P, P, P, c_int, c_int, P, P, P, P, c_int, c_int, P, P, P]),
+    'ptb_fcos_norm_sums': (c_int, [P, P, c_i64, c_int, P, P]),
+    'ptb_fcos_bbox_loss': (c_int, [P, P, P, c_int, c_int, P, P, c_int, c_int, c_float, c_float, P, P, P, P]),
+    'ptb_fcos_centerness_loss': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
+    'ptb_fcos_decode_workspace': (c_u64, [c_int, c_int, P]),
+    'ptb_fcos_decode': (c_int, [P, P, P, c_int, P, P, c_int, c_int, P, P, c_int, P, P, P, P, P, c_u64, P]),
 }
 
 

@@ -7,6 +7,17 @@ import torch
 import torch.distributed as dist
 
 
+def reduce_mean_(tensor, group=None):
+    """reduce_mean (mmdet core/utils/dist_utils.py:63-69) of a device tensor, in place: divided by the world size, then summed over the
+    ranks in one all-reduce.  Unchanged when torch.distributed is not initialised.  The FCOS loss averages its two normalisers (positive
+    count, centerness sum) this way as one two-element tensor, without a host synchronisation."""
+    if not (dist.is_available() and dist.is_initialized()):
+        return tensor
+    tensor.div_(dist.get_world_size(group))
+    dist.all_reduce(tensor, op=dist.ReduceOp.SUM, group=group)
+    return tensor
+
+
 def allreduce_grads(module, group=None, average=True):
     """all-reduce (sum, then / world) the gradients of `module`'s parameters in place through one flat bucket.
     Parameters without a gradient on this rank contribute zeros (DDP's find_unused_parameters semantics).  Returns the number

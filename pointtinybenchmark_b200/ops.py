@@ -1638,3 +1638,103 @@ def tile_concat(det, labels, counts, offsets, scale_factor=None):
     check(lib.ptb_tile_concat(_ptr(det), _ptr(labels), _ptr(counts), T, K, _ptr(scale_factor), _ptr(offsets), _ptr(out), _ptr(lab), _ptr(cnt),
                               _stream()), 'ptb_tile_concat')
     return out, lab, cnt
+
+
+# ---- FCOS head (ptb_fcos_*): targets, loss normalisers, box and centerness losses, decode
+FCOS_MAX_LEVELS = 8                    # levels of one ptb_fcos_* launch
+FCOS_BOX_LOSS_MODES = {'IoULoss': 0, 'IoULoss_linear': 1, 'GIoULoss': 2}
+
+
+def _fcos_levels(featmap_sizes, strides):
+    L = len(featmap_sizes)
+    if not 1 <= L <= FCOS_MAX_LEVELS or len(strides) != L:
+        raise ValueError(f'{L} feature maps and {len(strides)} strides: 1 to {FCOS_MAX_LEVELS} levels, one stride each')
+    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for s in featmap_sizes for v in s])
+    st = (ctypes.c_float * L)(*[float(s) for s in strides])
+    return L, hw, st
+
+
+def fcos_targets(featmap_sizes, strides, B, gt_bboxes, gt_labels, gt_off, ranges, radius_px, norm_on_bbox, num_classes):
+    """ptb_fcos_targets: gt_bboxes (G, 4) fp32, gt_labels (G,) int64, gt_off (B+1,) int32 CSR offsets of the batch's GTs, ranges (L, 2)
+    fp32 on the device, radius_px (L,) fp32 or None -> labels (N,) int64, bbox_targets (N, 4) fp32 in level / image / y / x row order."""
+    lib = _lib.load()
+    L, hw, st = _fcos_levels(featmap_sizes, strides)
+    _chk(gt_off, torch.int32, 'gt_off'); _chk(ranges, torch.float32, 'ranges')
+    if gt_off.shape != (B + 1,) or ranges.shape != (L, 2):
+        raise ValueError(f'gt_off must be ({B + 1},) and ranges ({L}, 2)')
+    if gt_bboxes is not None:
+        _chk(gt_bboxes, torch.float32, 'gt_bboxes'); _chk(gt_labels, torch.int64, 'gt_labels')
+    if radius_px is not None:
+        _chk(radius_px, torch.float32, 'radius_px')
+    N = B * sum(int(h) * int(w) for h, w in featmap_sizes)
+    dev = gt_off.device
+    labels = torch.empty((N,), dtype=torch.int64, device=dev)
+    targets = torch.empty((N, 4), dtype=torch.float32, device=dev)
+    check(lib.ptb_fcos_targets(_ptr(gt_bboxes), _ptr(gt_labels), _ptr(gt_off), B, L, hw, st, _ptr(ranges), _ptr(radius_px),
+                               int(bool(norm_on_bbox)), int(num_classes), _ptr(labels), _ptr(targets), _stream()), 'ptb_fcos_targets')
+    return labels, targets
+
+
+def fcos_norm_sums(labels, targets, num_classes):
+    """ptb_fcos_norm_sums: (2,) fp32 [number of positive rows, sum of their centerness targets], on the device"""
+    lib = _lib.load()
+    _chk(labels, torch.int64, 'labels'); _chk(targets, torch.float32, 'targets')
+    out = torch.zeros(2, dtype=torch.float32, device=labels.device)
+    check(lib.ptb_fcos_norm_sums(_ptr(labels), _ptr(targets), labels.shape[0], int(num_classes), _ptr(out), _stream()), 'ptb_fcos_norm_sums')
+    return out
+
+
+def fcos_bbox_loss(pred, targets, labels, featmap_sizes, strides, B, num_classes, mode, overlap_eps, eps, scale=None, want_grad=False):
+    """ptb_fcos_bbox_loss: the (1,) sum of the centerness-weighted IoU / GIoU loss over the positive rows of pred (N, 4), or with
+    want_grad the gradient scale * d/dpred (zero rows for negatives)."""
+    lib = _lib.load()
+    _chk(pred, torch.float32, 'pred'); _chk(targets, torch.float32, 'targets'); _chk(labels, torch.int64, 'labels')
+    L, hw, st = _fcos_levels(featmap_sizes, strides)
+    return _loss_sum(lib.ptb_fcos_bbox_loss, pred, (_ptr(targets), _ptr(labels), B, L, hw, st, int(num_classes), int(mode),
+                                                    float(overlap_eps), float(eps)), scale, want_grad)
+
+
+def fcos_centerness_loss(logits, targets, labels, num_classes, scale=None, want_grad=False):
+    """ptb_fcos_centerness_loss: the (1,) sum of the soft-target centerness BCE over the positive rows of logits (N,), or its gradient"""
+    lib = _lib.load()
+    _chk(logits, torch.float32, 'logits'); _chk(targets, torch.float32, 'targets'); _chk(labels, torch.int64, 'labels')
+    return _loss_sum(lib.ptb_fcos_centerness_loss, logits, (_ptr(targets), _ptr(labels), logits.shape[0], int(num_classes)), scale,
+                     want_grad)
+
+
+def fcos_decode_rows(featmap_sizes, nms_pre):
+    """rows per image each level keeps: nms_pre when 0 < nms_pre < H*W (get_k_for_topk), else H*W"""
+    return [nms_pre if 0 < nms_pre < h * w else h * w for h, w in featmap_sizes]
+
+
+def fcos_decode(cls_maps, reg_maps, ctr_maps, strides, num_classes, img_hw, nms_pre, scale_factor=None):
+    """ptb_fcos_decode: channels-last maps cls (B,H,W,C), reg (B,H,W,4), ctr (B,H,W,1) per level, img_hw (B, 2) fp32, scale_factor (B, 4)
+    fp32 or None -> idx (B,R) int32 cells, boxes (B,R,4), scores (B,R,C), centerness (B,R), the levels' rows in level order."""
+    lib = _lib.load()
+    hw_list = [(int(c.shape[1]), int(c.shape[2])) for c in cls_maps]
+    L, hw, st = _fcos_levels(hw_list, strides)
+    B = cls_maps[0].shape[0]
+    if nms_pre > 4096 and any(nms_pre < h * w for h, w in hw_list):
+        raise NotImplementedError(f'test_cfg.nms_pre={nms_pre}: the top-k select takes at most 4096 rows per level')
+    _chk(img_hw, torch.float32, 'img_hw')
+    if img_hw.shape != (B, 2) or (scale_factor is not None and tuple(scale_factor.shape) != (B, 4)):
+        raise ValueError(f'img_hw must be ({B}, 2) and scale_factor ({B}, 4)')
+    if scale_factor is not None:
+        _chk(scale_factor, torch.float32, 'scale_factor')
+    for l, (c, r, k) in enumerate(zip(cls_maps, reg_maps, ctr_maps)):
+        _chk(c, torch.float32, f'cls_maps[{l}]'); _chk(r, torch.float32, f'reg_maps[{l}]'); _chk(k, torch.float32, f'ctr_maps[{l}]')
+        if tuple(c.shape) != (B,) + hw_list[l] + (num_classes,) or tuple(r.shape) != (B,) + hw_list[l] + (4,) \
+                or tuple(k.shape) != (B,) + hw_list[l] + (1,):
+            raise ValueError(f'level {l}: maps must be channels-last (B, H, W, {num_classes} | 4 | 1)')
+    R = sum(fcos_decode_rows(hw_list, nms_pre))
+    dev = cls_maps[0].device
+    idx = torch.empty((B, R), dtype=torch.int32, device=dev)
+    boxes = torch.empty((B, R, 4), dtype=torch.float32, device=dev)
+    scores = torch.empty((B, R, num_classes), dtype=torch.float32, device=dev)
+    ctr = torch.empty((B, R), dtype=torch.float32, device=dev)
+    nbytes = int(lib.ptb_fcos_decode_workspace(B, L, hw))
+    ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
+    arr = lambda ts: (ctypes.c_void_p * L)(*[t.data_ptr() for t in ts])
+    check(lib.ptb_fcos_decode(arr(cls_maps), arr(reg_maps), arr(ctr_maps), L, hw, st, B, int(num_classes), _ptr(img_hw), _ptr(scale_factor),
+                              int(nms_pre), _ptr(idx), _ptr(boxes), _ptr(scores), _ptr(ctr), _ptr(ws), nbytes, _stream()), 'ptb_fcos_decode')
+    return idx, boxes, scores, ctr

@@ -101,6 +101,13 @@ def register_roi():
     ROI_EXTRACTORS.register_module(name='SingleRoIExtractor', force=True, module=SingleRoIExtractor)
 
 
+def register_fcos():
+    """register FCOSHead (HEADS) with force=True over the reference class, so a detector built from an FCOS config afterwards runs its head
+    here.  Not done on import."""
+    from .fcos_head import FCOSHead
+    HEADS.register_module(name='FCOSHead', force=True, module=FCOSHead)
+
+
 def build_assigner(cfg, **default_args):
     return BBOX_ASSIGNERS.build(cfg, default_args)
 
