@@ -20,8 +20,8 @@ import torch.nn.functional as F
 from . import ops
 from .dist import reduce_mean_
 from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled
-from .p2p_head import _LossSumFn, _iou_of
-from .post_processing import check_split_thr
+from .p2p_head import _LossSumFn
+from .post_processing import check_split_thr, parse_nms_cfg, run_multiclass_nms
 from .registry import CfgNode
 
 INF = 1e8
@@ -281,23 +281,22 @@ class FCOSHead(PackedWeightsMixin, nn.Module):
     def _nms(self, boxes, scores, factors, cfg):
         """multiclass_nms (bbox_nms.py:7-94) with score_factors of every image of the batch in one launch: the raw scores pass
         score_thr, the products rank.  -> count (B,), det (B, K, 5), labels (B, K) int32"""
-        nms = dict(cfg.get('nms'))
-        check_split_thr(nms)
-        if nms.get('type', 'nms') != 'nms':
-            raise NotImplementedError(f"FCOSHead test_cfg.nms type {nms.get('type')}: 'nms' is implemented")
-        if nms.get('class_agnostic', False):
+        check_split_thr(cfg.get('nms'))
+        nms = parse_nms_cfg(cfg.get('nms'))
+        if nms.kind != 'nms':
+            raise NotImplementedError(f"FCOSHead test_cfg.nms type {nms.kind}: 'nms' is implemented")
+        if nms.class_agnostic:
             raise NotImplementedError('FCOSHead: class_agnostic NMS is not implemented')
         max_num = int(cfg.get('max_per_img', -1))
         if not 0 < max_num <= 1024:
             raise NotImplementedError(f'FCOSHead test_cfg.max_per_img={max_num}: 1 to 1024 is implemented')
-        iou, thr = _iou_of(nms), float(cfg.get('score_thr'))
+        thr = float(cfg.get('score_thr'))
         B, P, C = scores.shape
         valid = scores > thr
         prod = scores * factors[..., None]
         if P <= MULTICLASS_NMS_MAX:
             s = torch.where(valid, prod, prod.new_full((), float('-inf'))).contiguous()
-            cnt, det, lab, _, _ = ops.multiclass_nms_boxes(boxes.contiguous(), s, FLT_LOWEST, iou, max_num)
-            return cnt, det, lab
+            return run_multiclass_nms(boxes.contiguous(), s, FLT_LOWEST, nms, max_num)[:3]
         # mmcv batched_nms over the candidates in (row, class) order, compacted on the device: candidate i of image b goes to row
         # b * N + (its rank among the image's candidates), the rest to one spare row past the batch
         flat = valid.reshape(B, P * C)
@@ -317,7 +316,7 @@ class FCOSHead(PackedWeightsMixin, nn.Module):
         out_b.index_copy_(0, dst, boxes[:, :, None, :].expand(B, P, C, 4).reshape(-1, 4))
         out_s.index_copy_(0, dst, prod.reshape(-1))
         out_l.index_copy_(0, dst, torch.arange(C, dtype=torch.int32, device=boxes.device).repeat(B * P))
-        cnt, det, lab, _ = ops.batched_nms(out_b[:B * N].view(B, N, 4), out_s[:B * N].view(B, N), out_l[:B * N].view(B, N), count, iou,
+        cnt, det, lab, _ = ops.batched_nms(out_b[:B * N].view(B, N, 4), out_s[:B * N].view(B, N), out_l[:B * N].view(B, N), count, nms.iou,
                                            10000, max_num)
         return cnt, det[:, :max_num], lab[:, :max_num]
 

@@ -538,6 +538,13 @@ def p2p_decode_topk_levels(cls_maps, reg_maps, strides, num_classes, k, point_an
 NMS_WIDE_MAX_POINTS = 8192    # points per image of ptb_multiclass_nms_wide / ptb_multiclass_soft_nms_wide
 
 
+def _nms_outputs(B, max_per_img, device):
+    """the outputs of the multiclass NMS entry points: count (B,), det (B,max,5), label (B,max), keep (B,max), cand_count (B,)"""
+    return (torch.empty((B,), dtype=torch.int32, device=device), torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=device),
+            torch.zeros((B, max_per_img), dtype=torch.int32, device=device), torch.zeros((B, max_per_img), dtype=torch.int32, device=device),
+            torch.empty((B,), dtype=torch.int32, device=device))
+
+
 def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img, wide=False):
     """ptb_multiclass_nms. pts (B,P,2), scores (B,P,C) -> count (B,), det (B,max,5), label (B,max), keep (B,max), cand_count (B,)
     P <= 4096; wide=True: ptb_multiclass_nms_wide, P <= 8192 (the multi-level P2P head's candidates)."""
@@ -545,11 +552,7 @@ def multiclass_nms(pts, scores, pseudo_wh, score_thr, iou_thr, max_per_img, wide
     _chk(pts, torch.float32, 'pts'); _chk(scores, torch.float32, 'scores')
     B, P, C = scores.shape
     dev = pts.device
-    cnt = torch.empty((B,), dtype=torch.int32, device=dev)
-    det = torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=dev)
-    lab = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    keep = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    cc = torch.empty((B,), dtype=torch.int32, device=dev)
+    cnt, det, lab, keep, cc = _nms_outputs(B, max_per_img, dev)
     nbytes = lib.ptb_multiclass_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     fn, name = (lib.ptb_multiclass_nms_wide, 'ptb_multiclass_nms_wide') if wide else (lib.ptb_multiclass_nms, 'ptb_multiclass_nms')
@@ -576,11 +579,7 @@ def multiclass_nms_boxes(boxes, scores, score_thr, iou_thr, max_per_img):
     fn, name = ((lib.ptb_multiclass_nms_cls_boxes, 'ptb_multiclass_nms_cls_boxes') if _cls_boxes(boxes, scores)
                 else (lib.ptb_multiclass_nms_boxes, 'ptb_multiclass_nms_boxes'))
     dev = boxes.device
-    cnt = torch.empty((B,), dtype=torch.int32, device=dev)
-    det = torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=dev)
-    lab = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    keep = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    cc = torch.empty((B,), dtype=torch.int32, device=dev)
+    cnt, det, lab, keep, cc = _nms_outputs(B, max_per_img, dev)
     nbytes = lib.ptb_multiclass_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     check(fn(_ptr(boxes), _ptr(scores), B, P, C, float(score_thr), float(iou_thr), int(max_per_img),
@@ -605,11 +604,7 @@ def multiclass_soft_nms(pts_or_boxes, scores, pseudo_wh, score_thr, iou_thr, max
     dev = scores.device
     cls_boxes = pts_or_boxes.dim() == 4 and _cls_boxes(pts_or_boxes, scores)
     is_boxes = pts_or_boxes.shape[-1] == 4
-    cnt = torch.empty((B,), dtype=torch.int32, device=dev)
-    det = torch.zeros((B, max_per_img, 5), dtype=torch.float32, device=dev)
-    lab = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    keep = torch.zeros((B, max_per_img), dtype=torch.int32, device=dev)
-    cc = torch.empty((B,), dtype=torch.int32, device=dev)
+    cnt, det, lab, keep, cc = _nms_outputs(B, max_per_img, dev)
     nbytes = lib.ptb_multiclass_soft_nms_workspace(B, P, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     outs = (SOFT_NMS_METHODS[method], int(max_per_img), _ptr(cnt), _ptr(det), _ptr(lab), _ptr(keep), _ptr(cc), _ptr(ws), nbytes,

@@ -22,19 +22,10 @@ import torch.nn as nn
 
 from . import ops
 from .assigners import cost_matrix, match_cost_terms
-from .post_processing import check_split_thr
+from .post_processing import check_split_thr, parse_nms_cfg, run_multiclass_nms
 from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, wide_out_conv, \
     wide_out_conv_plan, _packed_tc
 from .registry import CfgNode, register_head
-
-
-def _iou_of(nms_cfg):
-    """IoU threshold of an mmcv nms config: `iou_threshold` (mmcv >= 1.3) or its older spelling `iou_thr`."""
-    v = nms_cfg.get('iou_threshold', None)
-    v = nms_cfg.get('iou_thr', None) if v is None else v
-    if v is None:
-        raise KeyError("test_cfg.nms needs 'iou_threshold' (or 'iou_thr')")
-    return float(v)
 
 
 class _LossSumFn(torch.autograd.Function):
@@ -487,17 +478,11 @@ class P2PHead(PackedWeightsMixin, nn.Module):
             idx, pts, scores = decode(cmap, rmap, self.num_classes, self.num_points, self.point_anchor.to(dev), self.strides[0],
                                       self.pts_gamma, img_hw, cfg.get('nms_pre', -1), scale_xy)
         wh = cfg.get('pseudo_wh', (16, 16))
-        nms = cfg.get('nms')
-        check_split_thr(nms)
-        if nms.get('type', 'nms') == 'soft_nms':       # batched_nms dispatches on nms_cfg['type'] (mmcv/ops/nms.py)
-            cnt, det, lab, keep, cc = ops.multiclass_soft_nms(pts, scores, wh, cfg.get('score_thr'), nms.get('iou_threshold', 0.3),
-                                                              cfg.get('max_per_img'), nms.get('sigma', 0.5),
-                                                              nms.get('min_score', 1e-3), nms.get('method', 'linear'), wide=multi)
-        elif nms.get('type', 'nms') == 'nms':
-            cnt, det, lab, keep, cc = ops.multiclass_nms(pts, scores, wh, cfg.get('score_thr'), _iou_of(nms),
-                                                         cfg.get('max_per_img'), wide=multi)
-        else:
-            raise NotImplementedError(f"nms type {nms.get('type')}")
+        check_split_thr(cfg.get('nms'))
+        nms = parse_nms_cfg(cfg.get('nms'))
+        if nms.class_agnostic:
+            raise NotImplementedError('P2PHead: class_agnostic NMS is not implemented')
+        cnt, det, lab, keep, cc = run_multiclass_nms(pts, scores, cfg.get('score_thr'), nms, cfg.get('max_per_img'), wh, wide=multi)
         cnt_h = cnt.cpu().tolist()
         res = []
         for b in range(B):
@@ -554,15 +539,11 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         cfg = self.test_cfg
         if boxes.shape[0] == 0 or scores.shape[1] == 0:
             return [(boxes.new_zeros((0, 5)), boxes.new_zeros((0,), dtype=torch.long))]
-        nms = cfg.get('nms')
-        check_split_thr(nms)
-        if nms.get('type', 'nms') == 'soft_nms':
-            cnt, det, lab, _, _ = ops.multiclass_soft_nms(boxes[None], scores[None], None, cfg.get('score_thr'),
-                                                          nms.get('iou_threshold', 0.3), cfg.get('max_per_img'), nms.get('sigma', 0.5),
-                                                          nms.get('min_score', 1e-3), nms.get('method', 'linear'))
-        else:
-            cnt, det, lab, _, _ = ops.multiclass_nms_boxes(boxes[None], scores[None], cfg.get('score_thr'),
-                                                           _iou_of(nms), cfg.get('max_per_img'))
+        check_split_thr(cfg.get('nms'))
+        nms = parse_nms_cfg(cfg.get('nms'))
+        if nms.class_agnostic:
+            raise NotImplementedError('P2PHead: class_agnostic NMS is not implemented')
+        cnt, det, lab, _, _ = run_multiclass_nms(boxes[None], scores[None], cfg.get('score_thr'), nms, cfg.get('max_per_img'))
         n = int(cnt[0])
         d = det[0, :n].clone()
         if not rescale:

@@ -19,7 +19,7 @@ import torch.nn as nn
 
 from . import ops
 from .assigners import MaxIoUAssigner, random_sample_plan, sampled_counts, upload_sample_plan
-from .post_processing import check_split_thr
+from .post_processing import check_kept, check_split_thr, keep_limit, parse_nms_cfg, run_multiclass_nms
 from .registry import CfgNode
 from .results import bbox2result
 
@@ -346,26 +346,15 @@ class StandardRoIHead(nn.Module):
 
     def _multiclass_nms(self, boxes, scores, cfg):
         """the batched multiclass NMS of (B, P, C, 4) boxes and (B, P, C) scores with the test cfg's nms / max_per_img:
-        count (B,), det (B, kmax, 5), label (B, kmax), kmax and max_per_img"""
-        nms = dict(cfg.get('nms') or dict(type='nms', iou_threshold=0.5))
-        check_split_thr(nms)
-        kind = nms.pop('type', 'nms')
-        if kind not in ('nms', 'soft_nms'):
-            raise NotImplementedError(f'RoI head nms type {kind}')
-        if nms.pop('class_agnostic', False):
+        count (B,), det (B, kmax, 5), label (B, kmax) and keep_limit's (kmax, unlimited)"""
+        nms_cfg = cfg.get('nms') or {}
+        check_split_thr(nms_cfg)
+        nms = parse_nms_cfg(nms_cfg, default_iou=0.5)
+        if nms.class_agnostic:
             raise NotImplementedError('RoI head class_agnostic NMS')
-        iou = nms.pop('iou_threshold', nms.pop('iou_thr', 0.5))
-        max_per_img = int(cfg.get('max_per_img', -1))
-        if max_per_img > 1024:
-            raise NotImplementedError('max_per_img must be <= 1024')
-        kmax = 1024 if max_per_img <= 0 else max_per_img
-        if kind == 'nms':
-            cnt, det, lab, _, _ = ops.multiclass_nms_boxes(boxes, scores, float(cfg.score_thr), iou, kmax)
-        else:
-            cnt, det, lab, _, _ = ops.multiclass_soft_nms(boxes, scores, None, float(cfg.score_thr), iou, kmax,
-                                                          sigma=nms.get('sigma', 0.5), min_score=nms.get('min_score', 1e-3),
-                                                          method=nms.get('method', 'linear'))
-        return cnt, det, lab, kmax, max_per_img
+        kmax, unlimited = keep_limit(cfg.get('max_per_img', -1))
+        cnt, det, lab, _, _ = run_multiclass_nms(boxes, scores, float(cfg.score_thr), nms, kmax)
+        return cnt, det, lab, kmax, unlimited
 
     def simple_test_bboxes(self, x, img_metas, proposals, rcnn_test_cfg, rescale=False):
         """test_mixins.py:57-155: per image (dets (k, 5), labels (k,)) from one decode launch and one batched NMS call"""
@@ -389,10 +378,9 @@ class StandardRoIHead(nn.Module):
                                         for m in img_metas]), dtype=torch.float32).to(dev)
         boxes, scores = ops.roi_decode(rois, res['cls_score'].detach().float().contiguous(), res['bbox_pred'].detach().float().contiguous(), B,
                                        bh.num_classes, bh.reg_class_agnostic, bh.means, bh.stds, abs(np.log(16 / 1000)), img_hw, sf)
-        cnt, det, lab, kmax, max_per_img = self._multiclass_nms(boxes, scores, cfg)
+        cnt, det, lab, kmax, unlimited = self._multiclass_nms(boxes, scores, cfg)
         cnt = cnt.cpu().tolist()
-        if max_per_img <= 0 and max(cnt) >= kmax:
-            raise NotImplementedError('max_per_img=-1: more than 1023 detections survive the NMS (kernel limit 1024)')
+        check_kept(max(cnt), kmax, unlimited)
         return [det[b, :cnt[b]] for b in range(B)], [lab[b, :cnt[b]].long() for b in range(B)]
 
     def simple_test(self, x, proposal_list, img_metas, proposals=None, rescale=False):
@@ -477,10 +465,9 @@ class StandardRoIHead(nn.Module):
         if n == 0:                                # the reference forwards no RoI and multiclass_nms returns nothing
             return torch.zeros((0, 5), dtype=torch.float32, device=dev), torch.zeros((0,), dtype=torch.long, device=dev)
         boxes, scores = self.aug_forward_merge(feats, metas, meta, rois, None, A)
-        cnt, det, lab, kmax, max_per_img = self._multiclass_nms(boxes, scores, cfg)
+        cnt, det, lab, kmax, unlimited = self._multiclass_nms(boxes, scores, cfg)
         c = int(cnt[0])
-        if max_per_img <= 0 and c >= kmax:
-            raise NotImplementedError('max_per_img=-1: more than 1023 detections survive the NMS (kernel limit 1024)')
+        check_kept(c, kmax, unlimited)
         return det[0, :c], lab[0, :c].long()
 
     def aug_test(self, x, proposal_list, img_metas, rescale=False):

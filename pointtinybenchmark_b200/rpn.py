@@ -18,6 +18,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .assigners import MaxIoUAssigner, random_sample_plan, sampled_counts, upload_sample_plan
+from .post_processing import parse_nms_cfg
 from .registry import CfgNode
 
 
@@ -156,15 +157,15 @@ class RPNProposals:
         if not cls_scores[0].is_cuda:
             raise RuntimeError('RPNProposals runs on CUDA tensors only; there is no CPU fallback')
         cfg = CfgNode(cfg) if cfg is not None else self.test_cfg
-        nms = dict(cfg.get('nms', dict(type='nms', iou_threshold=cfg.get('nms_thr', 0.7))))
-        if nms.get('type', 'nms') != 'nms':
-            raise NotImplementedError(f"rpn nms type {nms.get('type')}")
+        nms = parse_nms_cfg(cfg.get('nms', dict(iou_threshold=cfg.get('nms_thr', 0.7))), default_iou=0.7)
+        if nms.kind != 'nms':
+            raise NotImplementedError(f'rpn nms type {nms.kind}')
         max_per_img = cfg.get('max_per_img', cfg.get('max_num', cfg.get('nms_post', 1000)))   # older configs spell it max_num / nms_post
         dev = cls_scores[0].device
         img_hw = torch.tensor([[int(m['img_shape'][0]), int(m['img_shape'][1])] for m in img_metas], dtype=torch.int32).to(dev)
         return ops.rpn_proposals([c.detach().float().contiguous() for c in cls_scores], [r.detach().float().contiguous() for r in bbox_preds],
                                  self._base(dev), self.anchor_generator.strides, img_hw, self.means, self.stds, self.wh_ratio_clip,
-                                 cfg.get('nms_pre', -1), cfg.get('min_bbox_size', 0), nms.get('iou_threshold', 0.7), max_per_img)
+                                 cfg.get('nms_pre', -1), cfg.get('min_bbox_size', 0), nms.iou, max_per_img)
 
     @torch.no_grad()
     def get_bboxes(self, cls_scores, bbox_preds, img_metas, cfg=None, rescale=False, with_nms=True, return_levels=False):

@@ -13,33 +13,33 @@ import numpy as np
 import torch
 
 from . import ops
+from .post_processing import HARD_NMS_KEYS, check_kept, parse_nms_cfg
 from .registry import CfgNode
 from .results import bbox2result
 
 
 def _rpn_merge_cfg(cfg):
-    """merge_aug_proposals' reading of the RPN test cfg: (iou_threshold, max_per_img), max_num being the older max_per_img"""
+    """merge_aug_proposals' reading of the RPN test cfg: (IoU threshold, max_per_img), max_num being the older max_per_img"""
     cfg = CfgNode(cfg)
-    nms = dict(cfg.get('nms') or dict(type='nms', iou_threshold=cfg.get('nms_thr')))
-    if nms.get('type', 'nms') != 'nms':
-        raise NotImplementedError(f"merge_aug_proposals nms type {nms.get('type')}")
+    nms = parse_nms_cfg(cfg.get('nms') or dict(iou_threshold=cfg.get('nms_thr')))
+    if nms.kind != 'nms':
+        raise NotImplementedError(f'merge_aug_proposals nms type {nms.kind}')
     max_per_img = cfg.get('max_per_img', cfg.get('max_num'))
     if 'max_num' in cfg and max_per_img != cfg.max_num:
         raise AssertionError(f'You set max_num and max_per_img at the same time, but get {cfg.max_num} and {max_per_img} respectively')
-    return float(nms['iou_threshold']), int(max_per_img)
+    return nms.iou, int(max_per_img)
 
 
 def _merge_nms_cfg(rcnn_test_cfg):
-    nms = dict(CfgNode(rcnn_test_cfg).get('nms') or dict(type='nms', iou_threshold=0.5))
-    if nms.pop('type', 'nms') != 'nms':
+    nms_cfg = CfgNode(rcnn_test_cfg).get('nms') or {}
+    nms = parse_nms_cfg(nms_cfg, default_iou=0.5)
+    if nms.kind != 'nms':
         raise NotImplementedError('tile_aug_test: soft-NMS at the cross-tile merge is not implemented (nms type must be nms)')
-    if nms.pop('class_agnostic', False):
+    if nms.class_agnostic:
         raise NotImplementedError('tile_aug_test: class_agnostic NMS at the cross-tile merge')
-    iou = float(nms.pop('iou_threshold', nms.pop('iou_thr', 0.5)))
-    split_thr = int(nms.pop('split_thr', 10000))
-    if nms:
-        raise NotImplementedError(f'tile_aug_test: nms options {sorted(nms)} at the cross-tile merge')
-    return iou, split_thr
+    if set(nms_cfg) - HARD_NMS_KEYS:
+        raise NotImplementedError(f'tile_aug_test: nms options {sorted(set(nms_cfg) - HARD_NMS_KEYS)} at the cross-tile merge')
+    return nms.iou, int(nms.split_thr)
 
 
 def group_tiles(img_metas):
@@ -74,7 +74,6 @@ def tile_aug_test(rpn_head, roi_head, feats, img_metas, rcnn_test_cfg, rescale=F
     iou_rpn, max_prop = _rpn_merge_cfg(rpn_head.test_cfg)
     iou, split_thr = _merge_nms_cfg(rcnn_test_cfg)
     roi_cfg = CfgNode(rcnn_test_cfg)
-    max_per_img = int(roi_cfg.get('max_per_img', -1))
     # RPN: one forward and one proposal launch per FPN shape
     batch = roi_head.shape_batches(fts)
     groups = {}
@@ -100,7 +99,7 @@ def tile_aug_test(rpn_head, roi_head, feats, img_metas, rcnn_test_cfg, rescale=F
     # the RoI head's aug test of every tile
     rois = ops.box_map(props, pcnt, meta_back)
     boxes, scores = roi_head.aug_forward_merge(fts, metas, meta_back, rois, pcnt, A)
-    tcnt, tdet, tlab, kmax, _ = roi_head._multiclass_nms(boxes, scores, roi_cfg)
+    tcnt, tdet, tlab, kmax, unlimited = roi_head._multiclass_nms(boxes, scores, roi_cfg)
     first = [metas[t * A] for t in range(T)]
     host = np.array([[float(o[0]), float(o[1])] for o, _ in tiles], np.float32)
     if not rescale:
@@ -113,12 +112,11 @@ def tile_aug_test(rpn_head, roi_head, feats, img_metas, rcnn_test_cfg, rescale=F
         raise NotImplementedError(f'tile_aug_test: {T} tiles x {kmax} detections exceed the cross-tile NMS limit of '
                                   f'{ops.BATCHED_NMS_MAX_ROWS} rows (PTB_BATCHED_NMS_MAX_ROWS)')
     fcnt, fdet, flab, _ = ops.batched_nms(rows[None], rows[None, :, 4], rlab[None], rcnt, iou, split_thr,
-                                          max_per_img if max_per_img > 0 else -1)
+                                          -1 if unlimited else kmax)
     n = fdet.shape[1]
     out = torch.cat([fcnt.float(), tcnt.float(), fdet[0].reshape(-1), flab[0].float()]).cpu()   # the one device-to-host copy
     k = int(out[0])
-    if max_per_img <= 0 and int(out[1:1 + T].max()) >= kmax:
-        raise NotImplementedError('max_per_img=-1: more than 1023 detections of a tile survive its NMS (kernel limit 1024)')
+    check_kept(int(out[1:1 + T].max()), kmax, unlimited)
     d = out[1 + T:1 + T + 5 * n].view(n, 5)[:k]
     lab = out[1 + T + 5 * n:].long()[:k]
     return [bbox2result(d, lab, C)]
