@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, _packed_tc
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, no_tf32, normal_init_, tower, tower_path, _packed_tc
 from .registry import register_head
 
 _SUPPORTED_POS = ('CirclePtFeatGenerator', 'GridCirclesPtFeatGenerator')
@@ -497,9 +497,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         """CPRHead.loss0 (cpr_head.py:1131-1229) + MILLoss.forward (multi_instance_learning_loss.py:153-203), R = 1."""
         B, H, W, C = fmap.shape
         N, eps, dev = self.num_classes, hp['eps'], fmap.device
-        tf32 = torch.backends.cuda.matmul.allow_tf32
-        torch.backends.cuda.matmul.allow_tf32 = False
-        try:
+        with no_tf32():
             bags = self._bags(self.train_pts_extractor['pos_generator'], dev)
             feats, valid = _BagGatherFn.apply(fmap, gt, bags)                     # (G,K,C), (G,K)
             G, K, _ = feats.shape
@@ -558,8 +556,6 @@ class CPRHead(PackedWeightsMixin, nn.Module):
                 neg_prob = self.get_cls_prob(neg_cls)
                 losses['neg_loss'] = hp['neg_loss_weight'] * (_gfocal(neg_prob, torch.zeros_like(neg_prob), nm, eps).sum() / num_pos)
             return losses
-        finally:
-            torch.backends.cuda.matmul.allow_tf32 = tf32
 
     @torch.no_grad()
     @torch.autocast('cuda', enabled=False)
@@ -567,13 +563,9 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         """refine for the variants: bag features (CUDA gather) -> FC stack / cls_out / get_cls_prob (torch) -> ptb_cpr_refine (staged)."""
         pr = self.point_refiner
         dev = fmap.device
-        tf32 = torch.backends.cuda.matmul.allow_tf32
-        torch.backends.cuda.matmul.allow_tf32 = False
-        try:
+        with no_tf32():
             f, pts, valid, _ = self._bags(self.refine_pts_extractor['pos_generator'], dev).gather(fmap, gt, pts=True)
             prob = self.get_cls_prob(self.get_pts_outs(f, want_ins=False)).contiguous()
-        finally:
-            torch.backends.cuda.matmul.allow_tf32 = tf32
         groups = ops.label_groups(gt.bag_img, gt.labels, self.num_classes)
         cfg = ops._refine_cfg(pr['merge_th'], pr['gt_alpha'], pr['refine_th'], pr['nearest_filter'], pr['classify_filter'],
                               pr['return_score_type'] == 'max')
@@ -589,7 +581,7 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         info = {}
         for x in feats:
             c = tower(self.cls_convs, x, info)
-            self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
+            self._record_tower(info)
             cls_feats.append(c)
             ins_feats.append(c)
         return cls_feats, ins_feats
@@ -608,19 +600,15 @@ class CPRHead(PackedWeightsMixin, nn.Module):
         as the fp16 operand pair and the class-logit map comes from the same wgmma kernel (1 tap, N = num_classes),
         so neither the fp32 feature map nor an FFMA GEMM appears in the step; results are identical within 1e-4.
         An fp16 / bf16 feats[0] takes the same path (see forward); the detections are fp32."""
-        x = feats[0]
-        if len(feats) == 1 and self._default_variant() and tc_enabled(x, self.cls_convs, self.cls_out) and not torch.is_grad_enabled() \
-                and self.in_channels % 32 == 0 and self.feat_channels == 256:
+        if len(feats) == 1 and self._default_variant() and not torch.is_grad_enabled() \
+                and tower_path(self.cls_convs, feats[0], also=(self.cls_out,)) == 'wgmma-f16x2':
             info = {}
-            pair = tower(self.cls_convs, x, info, want='f16pair')
-            if pair is not None:
-                self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
-                self.last_overflow_flag = info.get('overflow_flag')
-                if self.debug and self.last_overflow_flag is not None and int(self.last_overflow_flag) != 0:    # host sync: debug only
-                    raise FloatingPointError('CPRHead: a GroupNorm output exceeded the fp16 operand range (|x| > 6e4) and was clamped')
-                h, l = pair
-                lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1), 1, self.num_classes, bias=self.cls_out.bias.detach())
-                return self._get_bboxes_from_logit_map(lmap, img_metas, rescale=rescale, **kwargs)
+            h, l = tower(self.cls_convs, feats[0], info, want='f16pair')
+            self._record_tower(info)
+            if self.debug and int(self.last_overflow_flag) != 0:    # host sync: debug only
+                raise FloatingPointError('CPRHead: a GroupNorm output exceeded the fp16 operand range (|x| > 6e4) and was clamped')
+            lmap = ops.conv_tc_f16(h, l, _packed_tc(self.cls_out, 1), 1, self.num_classes, bias=self.cls_out.bias.detach())
+            return self._get_bboxes_from_logit_map(lmap, img_metas, rescale=rescale, **kwargs)
         outs = self.forward(feats)
         return self.get_bboxes(*outs, img_metas, rescale=rescale, **kwargs)
 

@@ -19,7 +19,8 @@ import torch.nn.functional as F
 
 from . import ops
 from .dist import reduce_mean_
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, no_tf32, tower, tower_path, _packed_tc, \
+    _packed_tc_stacked
 from .p2p_head import _LossSumFn
 from .post_processing import check_split_thr, parse_nms_cfg, run_multiclass_nms
 from .registry import CfgNode
@@ -134,50 +135,32 @@ class FCOSHead(PackedWeightsMixin, nn.Module):
         nn.init.constant_(self.conv_cls.bias, bias_init_with_prob(0.01))
 
     # ------------------------------------------------------------------------------------------------
-    def _fused_out(self, first, taps=9):
-        """the packed weights and bias of `first` (conv_cls or conv_reg) with conv_centerness appended as the last output channel,
-        cached per parameter version"""
-        ws = (first.weight, first.bias, self.conv_centerness.weight, self.conv_centerness.bias)
-        key = tuple((w.data_ptr(), w._version) for w in ws) + (str(first.weight.device),)
-        cache = getattr(first, '_ptb_fcos_fused', None)
-        if cache is None or cache[0] != key:
-            w = torch.cat([first.weight.detach(), self.conv_centerness.weight.detach()]).reshape(first.out_channels + 1, -1, taps)
-            first._ptb_fcos_fused = (key, ops.conv_tc_pack_weight_f16(w.contiguous(), taps),
-                                     torch.cat([first.bias.detach(), self.conv_centerness.bias.detach()]).contiguous())
-        return first._ptb_fcos_fused[1], first._ptb_fcos_fused[2]
-
     def _out_tc(self, pc, pr):
         """inference output convs on the wgmma conv: two launches, the centerness channel appended to the conv sharing its input"""
-        from .layers import _packed_tc
         C = self.num_classes
         if self.centerness_on_reg:
-            packs, bias = self._fused_out(self.conv_reg)
+            packs, bias = _packed_tc_stacked((self.conv_reg, self.conv_centerness))
             yr = ops.conv_tc_f16(pr[0], pr[1], packs, 9, 5, bias=bias)
             yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.conv_cls, 9), 9, C, bias=self.conv_cls.bias.detach())
             return yc[..., :C], yr[..., :4], yr[..., 4:5]
-        packs, bias = self._fused_out(self.conv_cls)
+        packs, bias = _packed_tc_stacked((self.conv_cls, self.conv_centerness))
         yc = ops.conv_tc_f16(pc[0], pc[1], packs, 9, C + 1, bias=bias)
         yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.conv_reg, 9), 9, 4, bias=self.conv_reg.bias.detach())
         return yc[..., :C], yr[..., :4], yc[..., C:C + 1]
 
     def forward_single(self, x, scale, stride):
         """fcos_head.py:131-160: (cls_score, bbox_pred, centerness) of one level.  x: fp32, or an fp16 / bf16 map taken as it is."""
-        out = None
-        if tc_enabled(x, self.cls_convs, self.reg_convs, self.conv_cls, self.conv_reg, self.conv_centerness, scale) \
-                and self.in_channels % 32 == 0:
-            info = {}
+        info = {}
+        if tower_path([*self.cls_convs, *self.reg_convs], x,
+                      also=(self.conv_cls, self.conv_reg, self.conv_centerness, scale)) == 'wgmma-f16x2':
             pc = tower(self.cls_convs, x, info, want='f16pair')
-            pr = tower(self.reg_convs, x, info, want='f16pair') if pc is not None else None
-            if pc is not None and pr is not None:
-                self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
-                out = [t.permute(0, 3, 1, 2) for t in self._out_tc(pc, pr)]
-        if out is None:
-            info = {}
+            pr = tower(self.reg_convs, x, info, want='f16pair')
+            self._record_tower(info)
+            out = [t.permute(0, 3, 1, 2) for t in self._out_tc(pc, pr)]
+        else:
             fc, fr = tower(self.cls_convs, x, info), tower(self.reg_convs, x, info)
-            self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
-            with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
-                                            deterministic=torch.backends.cudnn.deterministic, allow_tf32=False), \
-                    torch.autocast('cuda', enabled=False):
+            self._record_tower(info)
+            with no_tf32(), torch.autocast('cuda', enabled=False):
                 out = [self.conv_cls(fc), self.conv_reg(fr), self.conv_centerness(fr if self.centerness_on_reg else fc)]
         cls_score, bbox_pred, centerness = out
         bbox_pred = scale(bbox_pred).float()

@@ -10,7 +10,9 @@ Input dtype: fp32, or the fp16 / bf16 feature map of a backbone under torch.auto
 the first conv's hi operand itself, a bf16 tensor is split from its 2-byte storage, and the input gradient comes back in that dtype.
 Everything after the first conv, parameters and outputs stay fp32.
 """
+import contextlib
 import math
+import os
 
 import torch
 import torch.nn as nn
@@ -56,18 +58,33 @@ def bias_init_with_prob(p):
     return float(-math.log((1 - p) / p))
 
 
-_PACK_ATTRS = ('_ptb_packed_f16', '_ptb_packed_f16_t', '_ptb_packed', '_ptb_packed_tc')
+_PACK_ATTRS = ('_ptb_packs',)      # the one attribute cached_pack keeps a module's packings in
 
 
 def invalidate_packed(module):
-    """drop every cached tensor-core packing of `module`'s weights.  The caches are keyed on (data_ptr, Tensor._version, device);
-    in-place writes through `.data` (mmcv's EMAHook swap, manual weight surgery) do NOT bump `_version`, so the heads call this from
-    train() / eval() and after load_state_dict, and anything else that writes `.data` must call it explicitly (`.data` writes are
+    """drop every cached tensor-core packing of `module`'s weights (`cached_pack`).  The caches are keyed on (data_ptr, Tensor._version,
+    device); in-place writes through `.data` (mmcv's EMAHook swap, manual weight surgery) do NOT bump `_version`, so the heads call this
+    from train() / eval() and after load_state_dict, and anything else that writes `.data` must call it explicitly (`.data` writes are
     otherwise unsupported: the packed copy would go stale).  Costs nothing when there is no cache."""
     for m in module.modules():
         for a in _PACK_ATTRS:
             if hasattr(m, a):
                 delattr(m, a)
+
+
+def cached_pack(module, name, tensors, make):
+    """make(), kept in `module`'s one dict of packings under `name` until a tensor of `tensors` is replaced (data_ptr), written in
+    place (Tensor._version) or moved to another device.  Every packing of a head's weights goes through here, so that
+    invalidate_packed drops them all."""
+    key = tuple((t.data_ptr(), t._version) for t in tensors) + (str(tensors[0].device),)
+    packs = getattr(module, _PACK_ATTRS[0], None)
+    if packs is None:
+        packs = {}
+        setattr(module, _PACK_ATTRS[0], packs)
+    hit = packs.get(name)
+    if hit is None or hit[0] != key:
+        hit = packs[name] = (key, make())
+    return hit[1]
 
 
 class PackedWeightsMixin:
@@ -82,6 +99,25 @@ class PackedWeightsMixin:
 
     def invalidate_packed(self):
         invalidate_packed(self)
+
+    def _record_tower(self, info):
+        """what the last tower() call ran (its `info`): backend, input path and, on wgmma-f16x2, the fp16-overflow flag"""
+        self.last_tower_backend, self.last_input_path, self.last_overflow_flag = \
+            info.get('backend'), info.get('input_path'), info.get('overflow_flag')
+
+
+@contextlib.contextmanager
+def no_tf32():
+    """cuDNN convolutions and cuBLAS matmuls in full fp32 inside the block, whatever the global TF32 flags say (the heads' float
+    outputs must match the fp32 reference to 1e-4); the other cuDNN flags stay as they are."""
+    matmul_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
+                                        deterministic=torch.backends.cudnn.deterministic, allow_tf32=False):
+            yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = matmul_tf32
 
 
 HALF_INPUT_DTYPES = (torch.float16, torch.bfloat16)
@@ -116,67 +152,50 @@ def _first_operands(xm):
     return ops.split_f16(xm, auto_scale=True)
 
 
-def _tc_supported(convs, x):
-    """the wgmma path covers the shipped head geometry: conv3x3 s1 p1 without bias -> 256 channels, GroupNorm with
-    channels-per-group % 4 == 0, Cin % 32 == 0, fp32 / fp16 / bf16 CUDA input, inference (no autograd graph)."""
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in convs for p in m.parameters())):
-        return False
-    if not x.is_cuda or x.dtype not in _INPUT_DTYPES or len(convs) == 0:
-        return False
-    for m in convs:
-        c = m.conv
-        if (c.kernel_size != (3, 3) or c.stride != (1, 1) or c.padding != (1, 1) or c.dilation != (1, 1) or c.groups != 1
-                or c.bias is not None or c.out_channels != 256 or c.in_channels % 32 != 0 or m.norm_name != 'gn' or not m.with_act):
-            return False
-        if (256 // m.gn.num_groups) % 4 != 0 or m.gn.num_groups != 32:
-            return False
-    return True
-
-
 def _packed_weight_f16(m):
+    """fp16 (h, l, device 1/scale) packing of a tower conv's weight for ops.conv3x3_c256_f16*"""
     from . import ops
     w = m.conv.weight
-    key = (w.data_ptr(), w._version, str(w.device), 'f16')
-    cache = getattr(m, '_ptb_packed_f16', None)
-    if cache is None or cache[0] != key:
-        m._ptb_packed_f16 = (key, ops.conv3x3_pack_weight_f16(w))
-    return m._ptb_packed_f16[1]
+    return cached_pack(m, 'f16', (w,), lambda: ops.conv3x3_pack_weight_f16(w))
 
 
 def _packed_weight_f16_t(m):
-    """dgrad operand: W^T with the taps reversed ([ci][co][8 - tap]), packed like a forward weight; cached per version."""
+    """dgrad operand: W^T with the taps reversed ([ci][co][8 - tap]), packed like a forward weight"""
     from . import ops
     w = m.conv.weight
-    key = (w.data_ptr(), w._version, str(w.device), 'f16t')
-    cache = getattr(m, '_ptb_packed_f16_t', None)
-    if cache is None or cache[0] != key:
-        wt = w.detach().flip(2, 3).transpose(0, 1).reshape(w.shape[1], w.shape[0], 9).contiguous()
-        m._ptb_packed_f16_t = (key, ops.conv_tc_pack_weight_f16(wt, 9))
-    return m._ptb_packed_f16_t[1]
+    return cached_pack(m, 'f16t', (w,), lambda: ops.conv_tc_pack_weight_f16(
+        w.detach().flip(2, 3).transpose(0, 1).reshape(w.shape[1], w.shape[0], 9).contiguous(), 9))
 
 
 def _packed_weight(m):
-    """TF32 hi/lo packing of a conv weight, cached per parameter version (re-packed after every optimizer step)."""
+    """TF32 hi/lo packing of a tower conv's weight for ops.conv3x3_c256"""
     from . import ops
     w = m.conv.weight
-    key = (w.data_ptr(), w._version, str(w.device))
-    cache = getattr(m, '_ptb_packed', None)
-    if cache is None or cache[0] != key:
-        m._ptb_packed = (key, ops.conv3x3_pack_weight(w))
-    return m._ptb_packed[1]
+    return cached_pack(m, 'tf32', (w,), lambda: ops.conv3x3_pack_weight(w))
 
 
 def _packed_tc(module, taps):
     """fp16 (h, l) column-slice packing (ops.conv_tc_pack_weight_f16) of a Linear (taps 1) / Conv2d (taps 9) weight for
-    ops.conv_tc_f16, cached per parameter version."""
+    ops.conv_tc_f16"""
     from . import ops
     w = module.weight
-    key = (w.data_ptr(), w._version, str(w.device), taps)
-    cache = getattr(module, '_ptb_packed_tc', None)
-    if cache is None or cache[0] != key:
+
+    def make():
         w2 = w.detach().reshape(w.shape[0], w.shape[1], -1) if w.dim() == 4 else w.detach()
-        module._ptb_packed_tc = (key, ops.conv_tc_pack_weight_f16(w2.contiguous(), taps))
-    return module._ptb_packed_tc[1]
+        return ops.conv_tc_pack_weight_f16(w2.contiguous(), taps)
+    return cached_pack(module, ('tc', taps), (w,), make)
+
+
+def _packed_tc_stacked(convs):
+    """(packing, bias) of 3x3 Conv2d layers that read one input, their output channels stacked in order, so that one ops.conv_tc_f16
+    launch computes them all; kept on convs[0]"""
+    from . import ops
+
+    def make():
+        w = torch.cat([c.weight.detach() for c in convs])
+        return (ops.conv_tc_pack_weight_f16(w.reshape(w.shape[0], w.shape[1], 9).contiguous(), 9),
+                torch.cat([c.bias.detach() for c in convs]).contiguous())
+    return cached_pack(convs[0], 'tc_stacked', [t for c in convs for t in (c.weight, c.bias)], make)
 
 
 INT32_MAX = 2 ** 31 - 1
@@ -257,31 +276,39 @@ def wide_out_conv(conv, x, k=1):
     return y[..., :conv.out_channels].permute(0, 3, 1, 2)
 
 
-def tc_enabled(x, *modules):
-    """inference-only tensor-core path: CUDA fp32 / fp16 / bf16, no autograd graph, fp16-split mode selected."""
-    import os
-    if os.environ.get('PTB_CONV_MODE', 'f16x2') != 'f16x2' or not x.is_cuda or x.dtype not in _INPUT_DTYPES:
-        return False
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for m in modules for p in m.parameters())):
-        return False
-    return True
+def _tc_geometry(convs, train):
+    """the shipped head geometry of the tensor-core towers: conv3x3 s1 p1 without bias -> 256 channels, GroupNorm(32), ReLU; at
+    inference Cin % 32 == 0, in training 256 -> 256 with an affine GroupNorm"""
+    return len(convs) > 0 and all(
+        m.conv.kernel_size == (3, 3) and m.conv.stride == (1, 1) and m.conv.padding == (1, 1) and m.conv.dilation == (1, 1)
+        and m.conv.groups == 1 and m.conv.bias is None and m.conv.out_channels == 256 and m.norm_name == 'gn' and m.with_act
+        and m.gn.num_groups == 32 and ((m.conv.in_channels == 256 and m.gn.affine) if train else m.conv.in_channels % 32 == 0)
+        for m in convs)
 
 
-def _tc_train_supported(convs, x):
-    """the tensor-core TRAINING tower (forward + dgrad + wgrad + GroupNorm backward kernels) covers the shipped head geometry:
-    256 -> 256 conv3x3 s1 p1 without bias, GroupNorm with 8 | channels-per-group, ReLU, fp32 / fp16 / bf16 CUDA input."""
-    import os
-    if os.environ.get('PTB_CONV_MODE', 'f16x2') != 'f16x2' or os.environ.get('PTB_TOWER_TRAIN', 'tc') != 'tc':
-        return False
-    if not x.is_cuda or x.dtype not in _INPUT_DTYPES or len(convs) == 0:
-        return False
-    for m in convs:
-        c = m.conv
-        if not (c.in_channels == 256 and c.out_channels == 256 and c.kernel_size == (3, 3) and c.stride == (1, 1)
-                and c.padding == (1, 1) and c.dilation == (1, 1) and c.groups == 1 and c.bias is None and m.norm_name == 'gn'
-                and m.with_act and m.gn.num_groups == 32 and m.gn.affine):
-            return False
-    return True
+def tower_path(convs, x, also=()):
+    """The backend a tower of `convs` runs on for the input `x`, decided on the host from PTB_CONV_MODE, PTB_TOWER_TRAIN, the grad
+    mode and, of x, only is_cuda, dtype and requires_grad:
+      'wgmma-f16x2'        inference (grad disabled, or nothing of x, convs and `also` requires grad), a CUDA fp32 / fp16 / bf16
+                           input and the inference geometry (_tc_geometry), with PTB_CONV_MODE=f16x2 (the default)
+      'wgmma-3xtf32'       the same with any other PTB_CONV_MODE
+      'wgmma-f16x2-train'  otherwise under grad, whatever requires it: PTB_CONV_MODE=f16x2, PTB_TOWER_TRAIN=tc (the default), a CUDA
+                           fp32 / fp16 / bf16 input and the training geometry
+      'cudnn'              everything else: torch's convs
+    `also`: modules whose parameters count only toward "is this inference?" (a head's output convs, which run after the tower).
+    A half-precision input raises here on the CPU (RuntimeError), and under a PTB_CONV_MODE other than f16x2 (input_plan)."""
+    mode = os.environ.get('PTB_CONV_MODE', 'f16x2')
+    if x.dtype in HALF_INPUT_DTYPES and not x.is_cuda:
+        raise RuntimeError(f'tower: expected a CUDA tensor for a {x.dtype} input (pointtinybenchmark_b200 has no CPU path)')
+    input_plan(x.dtype, mode)
+    tc_input = x.is_cuda and x.dtype in _INPUT_DTYPES
+    grad = torch.is_grad_enabled()
+    inference = not (grad and (x.requires_grad or any(p.requires_grad for m in (*convs, *also) for p in m.parameters())))
+    if tc_input and inference and _tc_geometry(convs, train=False):
+        return 'wgmma-f16x2' if mode == 'f16x2' else 'wgmma-3xtf32'
+    if tc_input and grad and mode == 'f16x2' and os.environ.get('PTB_TOWER_TRAIN', 'tc') == 'tc' and _tc_geometry(convs, train=True):
+        return 'wgmma-f16x2-train'
+    return 'cudnn'
 
 
 class _TowerTCFn(torch.autograd.Function):
@@ -351,26 +378,40 @@ class _TowerTCFn(torch.autograd.Function):
 
 
 def tower(convs, x, info=None, want='fp32'):
-    """4 x [conv3x3 + GN + ReLU].  Inference: hand-written wgmma implicit GEMM (fp16 two-term split or 3xTF32) with GroupNorm
-    statistics in the epilogue (csrc/conv_tc.cu).  Training (autograd): _TowerTCFn for the shipped 256 -> 256 geometry (same forward
-    kernel + hand-written backward), else cuDNN fp32 through torch.
+    """4 x [conv3x3 + GN + ReLU] on the backend tower_path names.  Inference: hand-written wgmma implicit GEMM (fp16 two-term split or
+    3xTF32) with GroupNorm statistics in the epilogue (csrc/conv_tc.cu).  Training (autograd): _TowerTCFn for the shipped 256 -> 256
+    geometry (same forward kernel + hand-written backward), else cuDNN fp32 through torch.
     x: fp32, or an fp16 / bf16 CUDA feature map on the tensor-core paths (`input_plan`; the output is fp32 either way).
-    info (optional dict) receives 'backend' and, on the tensor-core paths, 'input_path'."""
-    import os
-    mode = os.environ.get('PTB_CONV_MODE', 'f16x2')
-    if x.dtype in HALF_INPUT_DTYPES and not x.is_cuda:
-        raise RuntimeError(f'tower: expected a CUDA tensor for a {x.dtype} input (pointtinybenchmark_b200 has no CPU path)')
-    plan = input_plan(x.dtype, mode)
-    if want == 'f16pair' and not (_tc_supported(convs, x) and mode == 'f16x2' and all(m.conv.in_channels % 32 == 0 for m in convs)):
-        return None
-    if _tc_supported(convs, x) and mode == 'f16x2' and all(m.conv.in_channels % 32 == 0 for m in convs):
+    want='f16pair' returns the (B,H,W,C) fp16 operand pair of the output instead, on the wgmma-f16x2 path only (ValueError elsewhere:
+    ask tower_path first).  info (optional dict) receives 'backend' and, on the tensor-core paths, 'input_path'; on wgmma-f16x2 also
+    'overflow_flag'."""
+    from . import ops
+    path = tower_path(convs, x)
+    if want == 'f16pair' and path != 'wgmma-f16x2':
+        raise ValueError(f"tower: want='f16pair' needs the wgmma-f16x2 path; this tower and input take {path}")
+    if path == 'cudnn':
+        if x.dtype in HALF_INPUT_DTYPES:
+            raise NotImplementedError(f'tower: a {x.dtype} input needs the tensor-core geometry (conv3x3 s1 p1 without bias -> 256 '
+                                      'channels, GroupNorm(32), ReLU, Cin % 32 == 0; 256 -> 256 under autograd); convert it to fp32 for '
+                                      'the cuDNN path')
+        if info is not None:
+            info['backend'] = 'cudnn'
+        x = x.contiguous(memory_format=torch.channels_last)
+        with no_tf32():
+            for m in convs:
+                x = m(x)
+        return x
+    xm = ops.to_nhwc(x).contiguous()
+    if info is not None:
+        info['backend'] = path
+        info['input_path'] = input_plan(x.dtype)[0]
+    if path == 'wgmma-f16x2':
         # two-term fp16 split (22 significant bits), kind::f16: half the tensor-pipe time of 3xTF32.  The first layer's input
         # is scaled by a power of two chosen on the device from max|x| (no host sync); later layers consume GroupNorm outputs.
-        from . import ops
-        xm = ops.to_nhwc(x).contiguous()
         h, l, dev_inv = _first_operands(xm)
         flag = torch.zeros(1, dtype=torch.int32, device=x.device)
-        out = None
+        if info is not None:
+            info['overflow_flag'] = flag
         for i, m in enumerate(convs):
             wh, wl, inv_w = _packed_weight_f16(m)
             # conv + GroupNorm + ReLU in one launch: the apply runs inside the conv kernel (ptb_conv3x3_c256_f16_gn)
@@ -381,18 +422,10 @@ def tower(convs, x, info=None, want='fp32'):
                 out = a
             else:
                 h, l = a, b
-        if info is not None:
-            info['backend'] = 'wgmma-f16x2'
-            info['input_path'] = plan[0]
-            info['overflow_flag'] = flag
         if want == 'f16pair':
-            return h, l              # (B,H,W,C) fp16 operand pair of the tower output: feeds ptb_conv_tc_f16x2 directly
-        return out.permute(0, 3, 1, 2)
-    if _tc_supported(convs, x):
-        from . import ops
-        xm = ops.to_nhwc(x).contiguous()
+            return h, l              # feeds ptb_conv_tc_f16x2 directly
+    elif path == 'wgmma-3xtf32':
         hi, lo = ops.split_tf32(xm)
-        out = None
         for i, m in enumerate(convs):
             wh, wl = _packed_weight(m)
             y, stats = ops.conv3x3_c256(hi, lo, wh, wl)
@@ -403,29 +436,9 @@ def tower(convs, x, info=None, want='fp32'):
                 out = res
             else:
                 hi, lo = res
-        if info is not None:
-            info['backend'] = 'wgmma-3xtf32'
-            info['input_path'] = plan[0]
-        return out.permute(0, 3, 1, 2)          # (B,C,H,W) view with channels_last strides
-    if want == 'fp32' and torch.is_grad_enabled() and _tc_train_supported(convs, x):
-        from . import ops
+    else:
         params = []
         for m in convs:
             params += [m.conv.weight, m.gn.weight, m.gn.bias]
-        out = _TowerTCFn.apply(ops.to_nhwc(x).contiguous(), convs, *params)
-        if info is not None:
-            info['backend'] = 'wgmma-f16x2-train'
-            info['input_path'] = plan[0]
-        return out.permute(0, 3, 1, 2)
-    if x.dtype in HALF_INPUT_DTYPES:
-        raise NotImplementedError(f'tower: a {x.dtype} input needs the tensor-core geometry (conv3x3 s1 p1 without bias -> 256 channels, '
-                                  'GroupNorm(32), ReLU, Cin % 32 == 0; 256 -> 256 under autograd); convert it to fp32 for the cuDNN path')
-    if info is not None:
-        info['backend'] = 'cudnn'
-    x = x.contiguous(memory_format=torch.channels_last)
-    # the head's logits must match the fp32 reference to 1e-4: never let cuDNN drop to TF32 here, whatever the global flag says
-    with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
-                                    deterministic=torch.backends.cudnn.deterministic, allow_tf32=False):
-        for m in convs:
-            x = m(x)
-    return x
+        out = _TowerTCFn.apply(xm, convs, *params)
+    return out.permute(0, 3, 1, 2)          # (B,C,H,W) view with channels_last strides

@@ -23,7 +23,7 @@ import torch.nn as nn
 from . import ops
 from .assigners import cost_matrix, match_cost_terms
 from .post_processing import check_split_thr, parse_nms_cfg, run_multiclass_nms
-from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, tower, tc_enabled, wide_out_conv, \
+from .layers import ConvModule, PackedWeightsMixin, bias_init_with_prob, normal_init_, no_tf32, tower, tower_path, wide_out_conv, \
     wide_out_conv_plan, _packed_tc
 from .registry import CfgNode, register_head
 
@@ -203,32 +203,27 @@ class P2PHead(PackedWeightsMixin, nn.Module):
         front of the head).  The outputs are fp32; `last_input_path` names the path the towers took."""
         cls_outs, pts_outs = [], []
         for x in feats:
-            if tc_enabled(x, self.cls_convs, self.reg_convs, self.cls_out, self.reg_out) and self.feat_channels == 256 \
-                    and self.in_channels % 32 == 0:
-                info = {}
+            info = {}
+            if tower_path([*self.cls_convs, *self.reg_convs], x, also=(self.cls_out, self.reg_out)) == 'wgmma-f16x2':
                 pc = tower(self.cls_convs, x, info, want='f16pair')
-                pr = tower(self.reg_convs, x, info, want='f16pair') if pc is not None else None
-                if pc is not None and pr is not None:
-                    self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
-                    nc, nr = self.cls_out.out_channels, self.reg_out.out_channels
-                    ldy = None
-                    if nc > MAX_OUT_CHANNELS:      # ldy = ceil4(nc): [..., :nc] is the whole map if 4 | nc
-                        B_, H_, W_ = pc[0].shape[:3]
-                        ldy = wide_out_conv_plan(B_, H_, W_, nc, self.num_points)
-                    yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9), 9, nc, bias=self.cls_out.bias.detach(), ldy=ldy)
-                    yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9), 9, nr, bias=self.reg_out.bias.detach())
-                    cls_outs.append(yc[..., :nc].permute(0, 3, 1, 2))
-                    pts_outs.append(yr[..., :nr].permute(0, 3, 1, 2))
-                    continue
+                pr = tower(self.reg_convs, x, info, want='f16pair')
+                self._record_tower(info)
+                nc, nr = self.cls_out.out_channels, self.reg_out.out_channels
+                ldy = None
+                if nc > MAX_OUT_CHANNELS:      # ldy = ceil4(nc): [..., :nc] is the whole map if 4 | nc
+                    B_, H_, W_ = pc[0].shape[:3]
+                    ldy = wide_out_conv_plan(B_, H_, W_, nc, self.num_points)
+                yc = ops.conv_tc_f16(pc[0], pc[1], _packed_tc(self.cls_out, 9), 9, nc, bias=self.cls_out.bias.detach(), ldy=ldy)
+                yr = ops.conv_tc_f16(pr[0], pr[1], _packed_tc(self.reg_out, 9), 9, nr, bias=self.reg_out.bias.detach())
+                cls_outs.append(yc[..., :nc].permute(0, 3, 1, 2))
+                pts_outs.append(yr[..., :nr].permute(0, 3, 1, 2))
+                continue
             # autograd path: the towers run layers._TowerTCFn (tensor-core forward + dgrad + wgrad + GroupNorm backward) for the
             # shipped geometry; output convs of up to 512 channels stay cuDNN fp32, never TF32 (1e-4 logits); a wider cls_out runs
             # layers._WideOutConvFn on the tensor cores (selected from the width alone)
-            info = {}
             fc, fr = tower(self.cls_convs, x, info), tower(self.reg_convs, x, info)
-            self.last_tower_backend, self.last_input_path = info.get('backend'), info.get('input_path')
-            with torch.backends.cudnn.flags(enabled=torch.backends.cudnn.enabled, benchmark=torch.backends.cudnn.benchmark,
-                                            deterministic=torch.backends.cudnn.deterministic, allow_tf32=False), \
-                    torch.autocast('cuda', enabled=False):
+            self._record_tower(info)
+            with no_tf32(), torch.autocast('cuda', enabled=False):
                 if self.cls_out.out_channels > MAX_OUT_CHANNELS:
                     cls_outs.append(wide_out_conv(self.cls_out, fc, self.num_points))
                 else:

@@ -221,3 +221,19 @@ def test_stale_packed_weights_are_dropped_by_eval_and_invalidate(ops):
     assert torch.equal(y_stale, y0), 'documented hazard: without invalidation the stale pack is used'
     assert not torch.equal(y1, y0), 'eval() must make the new weights visible'
     assert torch.equal(y2, y0), 'invalidate_packed() after restoring the weights gives the original output back'
+    # FCOS: conv_centerness runs in the same launch as conv_cls, from one packing of both
+    from pointtinybenchmark_b200.fcos_head import FCOSHead
+    fcos = FCOSHead(num_classes=4, in_channels=256, strides=(8,), regress_ranges=((-1, 1e8),)).cuda().eval()
+    with torch.no_grad():
+        c0 = fcos((x,))[2][0].clone()
+        fcos.conv_centerness.weight.data.mul_(-1.0)
+        c_stale = fcos((x,))[2][0].clone()
+        fcos.eval()
+        c1 = fcos((x,))[2][0].clone()
+        fcos.conv_centerness.weight.data.mul_(-1.0)
+        fcos.invalidate_packed()
+        c2 = fcos((x,))[2][0].clone()
+    assert fcos.last_tower_backend == 'wgmma-f16x2'
+    assert torch.equal(c_stale, c0), 'documented hazard: without invalidation the stale pack is used'
+    assert not torch.equal(c1, c0), 'eval() must make the new centerness weights visible'
+    assert torch.equal(c2, c0), 'invalidate_packed() after restoring the weights gives the original output back'

@@ -86,7 +86,7 @@ def test_every_finite_fp16_value_is_its_own_hi_operand():
     assert np.all(lo == 0) and not np.any(np.signbit(lo))
 
 
-def test_heads_keep_their_constructor_surface_and_refuse_cpu_half_inputs():
+def test_heads_keep_their_constructor_surface_and_tower_path_refuses_cpu_half_inputs():
     cpr, p2p = build_head(cpr_cfg(D)), build_head(p2p_cfg(dict(D, stride=4)))
     assert all(p.dtype == torch.float32 for h in (cpr, p2p) for p in h.parameters()), 'parameters stay fp32'
     for dt in (torch.float16, torch.bfloat16):
@@ -97,4 +97,5 @@ def test_heads_keep_their_constructor_surface_and_refuse_cpu_half_inputs():
             p2p.forward((x,))
         with pytest.raises(RuntimeError, match='no CPU'):
             layers.tower(cpr.cls_convs, x)
-        assert not layers.tc_enabled(x, cpr.cls_convs)
+        with pytest.raises(RuntimeError, match='no CPU'):
+            layers.tower_path(cpr.cls_convs, x)

@@ -163,9 +163,13 @@ def test_state_dict_matches_reference_for_every_shipped_config(golden_dir):
 def test_packed_weight_caches_are_invalidated_by_train_eval_and_load_state_dict():
     """ADVICE r1: the tensor-core packings are keyed on Tensor._version, which `.data` writes (EMA swaps, weight surgery) do not bump.
     The heads drop the caches on train() / eval(), after load_state_dict (also when loaded as a SUBMODULE of a detector) and on demand."""
+    from pointtinybenchmark_b200.fcos_head import FCOSHead
     from pointtinybenchmark_b200.layers import _PACK_ATTRS
-    for h in (build_head(cpr_cfg(D)), build_head(p2p_cfg(dict(D, stride=4)))):
-        mods = [h.cls_convs[0], h.cls_convs[3], h.cls_out]
+    fcos = FCOSHead(num_classes=80, in_channels=256)
+    for h, mods in ((build_head(cpr_cfg(D)), 'cls_convs.0 cls_convs.3 cls_out'),
+                    (build_head(p2p_cfg(dict(D, stride=4))), 'cls_convs.0 cls_convs.3 cls_out'),
+                    (fcos, 'cls_convs.0 reg_convs.3 conv_cls conv_reg conv_centerness')):
+        mods = [h.get_submodule(n) for n in mods.split()]
 
         def plant():
             for m in mods:
