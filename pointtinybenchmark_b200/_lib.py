@@ -1,158 +1,91 @@
-"""ctypes binding of libptb_b200.so (the C ABI declared in include/ptb_b200.h).
+"""ctypes binding of libptb_b200.so, derived from the C ABI's header include/ptb_b200.h.
+
+The header is the one place that states a signature, a struct or a constant: on import this module parses its prototypes into
+SIGNATURES, its two structs into RefineCfg and MatchCost, and its integer #defines into DEFINES, so the binding agrees with the
+header by construction.  A type the parser does not know raises instead of being guessed.
 
 There is NO fallback: if the CUDA library is missing or fails to load, every op raises.
 """
 import ctypes
 import os
+import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libptb_b200.so')
+HEADER_PATH = os.path.normpath(os.path.join(_HERE, '..', 'include', 'ptb_b200.h'))
 
 _lib = None
 MISSING = []
 
-c_int, c_float, c_void_p, c_u64, c_i64, c_double = ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int64, \
-    ctypes.c_double
+# by-value C types of the ABI; every pointer is a c_void_p
+_SCALARS = {'int': ctypes.c_int, 'int32_t': ctypes.c_int, 'int64_t': ctypes.c_int64, 'uint64_t': ctypes.c_uint64,
+            'float': ctypes.c_float, 'double': ctypes.c_double}
 
 
-class RefineCfg(ctypes.Structure):
-    _fields_ = [('merge_th', c_float), ('gt_alpha', c_float), ('refine_th', c_float), ('flags', ctypes.c_int32)]
+def _struct_name(c_name):
+    """ptb_refine_cfg -> RefineCfg"""
+    return ''.join(w.capitalize() for w in c_name[len('ptb_'):].split('_'))
 
 
-class MatchCost(ctypes.Structure):
-    """ptb_match_cost: one term of ptb_p2p_cost_matrix_terms."""
-    _fields_ = [('kind', ctypes.c_int32), ('weight', c_float), ('alpha', c_float), ('gamma', c_float), ('eps', c_float),
-                ('p', ctypes.c_int32), ('norm_with_img_wh', ctypes.c_int32)]
+def parse_header(text):
+    """(SIGNATURES, structs, defines) of a header's text: {name: (restype, argtypes)} of every ptb_* prototype,
+    {C typedef name: ctypes.Structure subclass} and {PTB_*: int}.  Raises ValueError, naming the declaration, on a
+    type or a statement it does not know."""
+    defines = {m[1]: int(m[2]) for m in re.finditer(r'^\s*#\s*define\s+(PTB_\w+)\s+(-?\d+)\s*$', text, re.M)}
+    src = re.sub(r'/\*.*?\*/', ' ', text, flags=re.S)
+    src = re.sub(r'^\s*#.*$', '', src, flags=re.M)
+
+    structs = {}
+    for m in re.finditer(r'typedef\s+struct\s*\{(.*?)\}\s*(\w+)\s*;', src, re.S):
+        fields = []
+        for member in filter(None, (s.strip() for s in m[1].split(';'))):
+            f = re.fullmatch(r'(\w+)\s+(\w+(?:\s*,\s*\w+)*)', member)
+            if f is None or f[1] not in _SCALARS:
+                raise ValueError(f'struct {m[2]}: unknown member {member!r}')
+            fields += [(n.strip(), _SCALARS[f[1]]) for n in f[2].split(',')]
+        structs[m[2]] = type(_struct_name(m[2]), (ctypes.Structure,), {'_fields_': fields})
+    src = re.sub(r'typedef\s+struct\s*\{.*?\}\s*\w+\s*;', '', src, flags=re.S)
+    src = re.sub(r'extern\s+"C"\s*\{|\}', '', src)
+
+    def ctype(t, decl, ret=False):
+        t = ' '.join(t.replace('*', ' * ').split())
+        if '*' in t:
+            return ctypes.c_char_p if ret and t == 'const char *' else ctypes.c_void_p
+        if t in _SCALARS:
+            return _SCALARS[t]
+        if t in structs and not ret:
+            return structs[t]
+        raise ValueError(f'unknown type {t!r} in {decl!r}')
+
+    signatures = {}
+    for decl in filter(None, (' '.join(s.split()) for s in src.split(';'))):
+        m = re.fullmatch(r'(.+?)\b(ptb_\w+)\s*\((.*)\)', decl)
+        if m is None:
+            raise ValueError(f'not a ptb_* prototype: {decl!r}')
+        params = [p.strip() for p in m[3].split(',')]
+        if params == ['void']:
+            params = []
+        args = []
+        for p in params:
+            a = re.fullmatch(r'(.*?)\b\w+', p)           # the type, without the parameter's name
+            if a is None or not a[1].strip():
+                raise ValueError(f'unnamed parameter {p!r} in {decl!r}')
+            args.append(ctype(a[1], decl))
+        signatures[m[2]] = (ctype(m[1], decl, ret=True), args)
+    return signatures, structs, defines
 
 
-P = c_void_p
-# name -> (restype, argtypes); must list every symbol of include/ptb_b200.h (tests/test_capi_symbols.py checks)
-SIGNATURES = {
-    'ptb_abi_version': (c_int, []),
-    'ptb_last_error': (ctypes.c_char_p, []),
-    'ptb_launch_count': (c_u64, []),
-    'ptb_reset_stream_state': (c_int, [P]),
-    'ptb_cpr_bag_gather': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, c_float, P, P, P, P, P]),
-    'ptb_cpr_bag_gather_bwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, P, P]),
-    'ptb_linear_rows': (c_int, [P, c_int, c_int, c_int, P, P, c_int, P, c_int, P]),
-    'ptb_linear_rows_bwd_x': (c_int, [P, c_int, c_int, c_int, P, c_int, P, c_int, c_int, P]),
-    'ptb_linear_rows_bwd_w': (c_int, [P, c_int, c_int, c_int, P, c_int, c_int, P, P, P, c_u64, P]),
-    'ptb_linear_rows_bwd_w_workspace': (c_u64, [c_int, c_int, c_int]),
-    'ptb_cpr_neg_mask': (c_int, [c_int, c_int, c_int, c_float, P, P, P, P, c_int, c_float, c_int, c_int, P, P]),
-    'ptb_cpr_grid_bag': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, c_float, c_float, c_int, P, P, P, P, P, P]),
-    'ptb_cpr_grid_bag_bwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, P, c_int, c_int, c_float, P, P]),
-    'ptb_label_groups': (c_int, [P, P, c_int, c_int, c_int, c_int, P, P, P, P]),
-    'ptb_cpr_refine': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, RefineCfg, P, P, P, P, P, P]),
-    'ptb_cpr_refine_fused': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, P, c_int, P, c_int, c_float, c_float, P, P, P, P, P,
-                                     P, RefineCfg, P, P, P, P, P]),
-    'ptb_mil_loss_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P, P]),
-    'ptb_cpr_bag_mil_fwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, c_int, c_float, P, P, c_float, c_int,
-                                    P, P, P, P, P, P, P]),
-    'ptb_cpr_loss_bwd_map': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
-                                     P, P, P, P, P, P, c_int, P, P, P, P]),
-    'ptb_cpr_loss_bwd_map_workspace': (c_u64, [c_int, c_int]),
-    'ptb_cpr_loss_bwd_scatter': (c_int, [P, P, P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
-                                         P, P, P, c_int, P, P, P, P]),
-    'ptb_mil_loss_bwd': (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P]),
-    'ptb_gfocal_sigmoid_fwd': (c_int, [P, c_i64, c_int, c_i64, P, P, c_int, c_float, P, P]),
-    'ptb_cpr_allpos_fwd': (c_int, [P, c_int, c_int, c_int, c_int, P, P, c_float, c_int, P, P, P, P]),
-    'ptb_sigmoid_loss_bwd': (c_int, [P, c_i64, c_int, c_i64, P, P, c_int, c_float, c_int, P, P, c_i64, c_int, P]),
-    'ptb_p2p_decode_topk': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, c_float, c_float, P, P, c_int, P, P, P, P,
-                                    c_u64, P]),
-    'ptb_p2p_decode_topk_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
-    'ptb_p2p_decode_topk_softmax': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, c_float, c_float, P, P, c_int, P, P, P, P,
-                                            c_u64, P]),
-    'ptb_multiclass_nms': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, P, P, P, P, P, P,
-                                   c_u64, P]),
-    'ptb_multiclass_nms_workspace': (c_u64, [c_int, c_int, c_int]),
-    'ptb_multiclass_nms_wide': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, P, P, P, P, P, P,
-                                        c_u64, P]),
-    'ptb_multiclass_soft_nms_wide': (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_int,
-                                             c_int, P, P, P, P, P, P, c_u64, P]),
-    'ptb_p2p_decode_topk_levels': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P, c_float, P, P, c_int, P, P, P, P, c_u64, P]),
-    'ptb_p2p_decode_topk_levels_softmax': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, P, c_float, P, P, c_int, P, P, P, P, c_u64,
-                                                   P]),
-    'ptb_p2p_decode_topk_levels_workspace': (c_u64, [c_int, c_int, P, c_int]),
-    'ptb_multiclass_soft_nms': (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_int, c_int,
-                                        P, P, P, P, P, P, c_u64, P]),
-    'ptb_multiclass_soft_nms_workspace': (c_u64, [c_int, c_int, c_int]),
-    'ptb_multiclass_nms_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_int, P, P, P, P, P, P, c_u64, P]),
-    'ptb_multiclass_nms_cls_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_int, P, P, P, P, P, P, c_u64, P]),
-    'ptb_multiclass_soft_nms_cls_boxes': (c_int, [P, P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, c_int, c_int,
-                                                  P, P, P, P, P, P, c_u64, P]),
-    'ptb_p2p_cost_matrix': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, c_float, c_float, c_float, c_float, c_float,
-                                    c_float, c_float, P, P]),
-    'ptb_p2p_cost_matrix_terms': (c_int, [P, P, c_int, P, c_int, c_int, P, P, c_int, P, c_int, c_float, c_float, P, P, c_u64, P]),
-    'ptb_p2p_cost_matrix_terms_workspace': (c_u64, [c_int]),
-    'ptb_rpn_proposals_workspace': (c_u64, [P, c_int, c_int, c_int, c_int, c_int]),
-    'ptb_rpn_proposals': (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, P, P, c_float, c_int, c_float, c_float, c_int, P, P, P, P, P, P, P, P, c_u64, P]),
-    'ptb_hungarian_v2_workspace': (c_u64, [c_int, c_int]),
-    'ptb_hungarian_v2_batch': (c_int, [P, P, c_int, c_int, c_int, c_int, P, P, P, P, P]),
-    'ptb_point_assigner': (c_int, [P, c_int, P, c_int, c_float, c_int, P, P, c_u64, P]),
-    'ptb_point_assigner_workspace': (c_u64, [c_int, c_int]),
-    'ptb_sigmoid_focal_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, c_float, c_float, P, P, P, P]),
-    'ptb_smooth_l1_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, c_float, P, P, P, P]),
-    'ptb_sigmoid_bce_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
-    'ptb_mse_fwd_bwd': (c_int, [P, P, P, c_i64, c_float, P, P, P, P]),
-    'ptb_smooth_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, P, P, P, P]),
-    'ptb_mse_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, P, P, P, P]),
-    'ptb_sigmoid_bce_cw_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
-    'ptb_softmax_ce_fwd_bwd': (c_int, [P, P, P, P, c_i64, c_int, P, P, P, P]),
-    'ptb_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, P, P, P, P]),
-    'ptb_balanced_l1_rows_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, c_float, c_float, P, P, P, P]),
-    'ptb_ghmc_bin_weights': (c_int, [P, P, P, c_int, c_i64, c_int, P, c_int, c_double, P, P, P, P, P]),
-    'ptb_ghmc_fwd_bwd': (c_int, [P, P, P, c_i64, c_int, P, c_int, P, P, P, P, P]),
-    'ptb_ghmr_bin_weights': (c_int, [P, P, P, P, c_float, c_int, c_i64, P, c_int, c_double, P, P, P, P, P]),
-    'ptb_ghmr_fwd_bwd': (c_int, [P, P, P, c_i64, P, c_float, P, c_int, P, P, P, P, P]),
-    'ptb_split_tf32': (c_int, [P, c_i64, P, P, P]),
-    'ptb_conv3x3_pack_weight': (c_int, [P, c_int, c_int, P, P, P]),
-    'ptb_conv3x3_c256_tf32x3': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P, P]),
-    'ptb_gn_relu_apply': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, c_int, P, P, P]),
-    'ptb_split_f16': (c_int, [P, c_i64, c_int, P, P, P, P, P]),
-    'ptb_conv3x3_pack_weight_f16': (c_int, [P, c_int, c_int, c_float, P, P, P]),
-    'ptb_conv3x3_c256_f16x2': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, P, P, P, P]),
-    'ptb_conv_tc_pack_weight_f16': (c_int, [P, c_int, c_int, c_int, c_int, c_float, P, P, P]),
-    'ptb_conv_tc_f16x2': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, c_int, P]),
-    'ptb_gn_relu_apply_f16': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, c_int, P, P, P, P]),
-    'ptb_split_f16_from_bf16': (c_int, [P, c_i64, P, P, P, P, P]),
-    'ptb_conv_tc_f16x1a': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, c_int, P, P]),
-    'ptb_conv_tc_f16x2_half_out': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, c_int, c_int, P]),
-    'ptb_conv3x3_c256_f16_gn': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, P, P, P, P, P, c_float, P, P, P, P]),
-    'ptb_max_iou_assign_workspace': (c_u64, [c_int, c_int]),
-    'ptb_max_iou_assign': (c_int, [P, c_int, P, c_int, P, P, c_int, c_float, c_float, c_float, c_float, c_int, c_int, c_float, c_int,
-                                   P, P, P, P, c_u64, P]),
-    'ptb_bbox_overlaps': (c_int, [P, c_int, P, c_int, c_int, P, P]),
-    'ptb_gn_relu_bwd_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
-    'ptb_gn_relu_bwd': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_float, c_int, P, P, P, P, P, P]),
-    'ptb_split_f16_amax': (c_int, [P, c_i64, P, P, P, P, P]),
-    'ptb_conv_tc_wgrad_workspace': (c_u64, [c_int, c_int, c_int, c_int]),
-    'ptb_conv_tc_wgrad_f16x2_ld': (c_int, [P, P, c_int, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, P, P, P, P, c_int, P]),
-    'ptb_col_sum_workspace': (c_u64, [c_i64, c_int]),
-    'ptb_col_sum': (c_int, [P, c_i64, c_int, c_int, P, P, P]),
-    'ptb_rpn_inside_anchors': (c_int, [P, P, P, c_int, c_int, c_int, P, P, P, P, P]),
-    'ptb_rpn_candidate_ranks': (c_int, [P, P, c_int, c_int, P, P, P]),
-    'ptb_rpn_anchor_targets': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_float, P, P, P, P, P]),
-    'ptb_rpn_sampled_indices': (c_int, [P, P, c_int, P, P, P, P]),
-    'ptb_rpn_level_loss': (c_int, [P, P, P, P, P, P, c_i64, c_int, c_float, P, P, P, P, P]),
-    'ptb_roi_align_fwd': (c_int, [P, P, P, c_int, c_int, c_int, P, c_int, c_int, c_int, c_float, P, P, P]),
-    'ptb_roi_align_bwd': (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_int, c_int, c_int, P, P]),
-    'ptb_roi_targets': (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, c_int, P, P, c_float, P, P, P, P, P, P]),
-    'ptb_roi_bbox_loss': (c_int, [P, c_int, P, P, P, c_i64, c_int, c_int, c_int, c_float, P, P, P, P]),
-    'ptb_roi_accuracy': (c_int, [P, P, c_i64, c_int, c_float, P, P]),
-    'ptb_roi_decode': (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, P, P, P, P]),
-    'ptb_box_map': (c_int, [P, c_int, P, c_int, c_int, P, P, P, P]),
-    'ptb_proposal_map_back': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P]),
-    'ptb_aug_merge': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, P, P, P]),
-    'ptb_batched_nms_workspace': (c_u64, [c_int, c_int]),
-    'ptb_batched_nms': (c_int, [P, c_int, P, c_int, P, P, c_int, c_int, c_float, c_int, c_int, P, P, P, P, P, c_u64, P]),
-    'ptb_tile_concat': (c_int, [P, P, P, c_int, c_int, P, P, P, P, P, P]),
-    'ptb_fcos_targets': (c_int, [P, P, P, c_int, c_int, P, P, P, P, c_int, c_int, P, P, P]),
-    'ptb_fcos_norm_sums': (c_int, [P, P, c_i64, c_int, P, P]),
-    'ptb_fcos_bbox_loss': (c_int, [P, P, P, c_int, c_int, P, P, c_int, c_int, c_float, c_float, P, P, P, P]),
-    'ptb_fcos_centerness_loss': (c_int, [P, P, P, c_i64, c_int, P, P, P, P]),
-    'ptb_fcos_decode_workspace': (c_u64, [c_int, c_int, P]),
-    'ptb_fcos_decode': (c_int, [P, P, P, c_int, P, P, c_int, c_int, P, P, c_int, P, P, P, P, P, c_u64, P]),
-}
+def _read_header():
+    if not os.path.exists(HEADER_PATH):
+        raise RuntimeError(f'{HEADER_PATH} is missing: the ctypes binding of libptb_b200.so is read from this C ABI header, which '
+                           'ships with the repository')
+    with open(HEADER_PATH) as f:
+        return parse_header(f.read())
+
+
+SIGNATURES, STRUCTS, DEFINES = _read_header()
+RefineCfg = STRUCTS['ptb_refine_cfg']
+MatchCost = STRUCTS['ptb_match_cost']
 
 
 def load():
@@ -176,7 +109,7 @@ def load():
         fn.argtypes = args
     global MISSING
     MISSING = missing      # tests/test_capi_symbols.py requires this to be empty
-    if lib.ptb_abi_version() != 2:
+    if lib.ptb_abi_version() != DEFINES['PTB_ABI_VERSION']:
         raise RuntimeError('libptb_b200.so ABI version mismatch')
     _lib = lib
     return lib

@@ -6,7 +6,7 @@ Also here: PointAssigner, HungarianAssignerV2 (the P2P point assigner named by B
 SamplingResult mirrors and RandomSampler with its host draw plan.  `registry.register_core()` registers them into mmdet's BBOX_ASSIGNERS / BBOX_SAMPLERS when mmdet is importable."""
 import torch
 
-from . import ops
+from . import _lib, ops
 
 
 class AssignResult:
@@ -75,7 +75,7 @@ class PointAssigner:
         return AssignResult(g.shape[0], gt_inds, None, labels)
 
 
-MAX_MATCH_COST_TERMS = 8        # per list (PTB_MAX_MATCH_COST_TERMS)
+MAX_MATCH_COST_TERMS = _lib.DEFINES['PTB_MAX_MATCH_COST_TERMS']        # per list
 _BOX_COSTS = ('BBoxL1Cost', 'IoUCost', 'IoUCostV2')
 
 
